@@ -1,7 +1,7 @@
 """ctypes binding of libbags_b200.so (C ABI declared in include/bags_b200.h).
 
 There is no fallback: if the shared library is missing, or the device is not a
-B200 (sm_100), every op raises.  Build it with ``python -m
+H100 (sm_90), every op raises.  Build it with ``python -m
 balancedgroupsoftmax_b200.build`` (or ``__graft_entry__.build()``).
 """
 from __future__ import annotations

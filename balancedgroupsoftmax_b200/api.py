@@ -72,7 +72,7 @@ class GraphedHeadStep(object):
                  exchange=None, stream: Optional[torch.cuda.Stream] = None, warmup: int = 2, grad_bucket=None):
         dev = weight.device
         if dev.type != 'cuda':
-            raise ops.nat.BagsNativeError('GraphedHeadStep runs on a B200 GPU only (weight is on %s)' % dev)
+            raise ops.nat.BagsNativeError('GraphedHeadStep runs on an H100 GPU only (weight is on %s)' % dev)
         self.weight, self.bias = weight, bias
         self.dt = tables if isinstance(tables, ops.DeviceTables) else ops.DeviceTables.from_tables(tables, dev)
         self.ratio = float(others_sample_ratio)
@@ -138,7 +138,7 @@ class GraphedHeadStep(object):
 
 
 class _GraphedPair(object):
-    """Static buffers + two CUDA graphs (forward: sampler + fused forward; backward: merged backward) for ONE RoI count."""
+    """Static buffers + two CUDA graphs (forward: sampler + fused forward; backward: preparation + merged backward) for ONE RoI count."""
 
     def __init__(self, n: int, k: int, c: int, dt: ops.DeviceTables, ratio: float, seed: int, op_dtype: torch.dtype,
                  has_bias: bool, need_dx: bool, device):
@@ -228,7 +228,7 @@ class GraphCachedHeadLoss(object):
     mmdet/core/bbox/samplers/base_sampler.py:30-78) but who still want graph-replay host costs inside an ordinary
     autograd graph (x comes from the trunk, dX flows back into it).
 
-    Per RoI count N it keeps static buffers and two CUDA graphs (sampler + fused forward; merged backward); a call with a
+    Per RoI count N it keeps static buffers and two CUDA graphs (sampler + fused forward; preparation + merged backward); a call with a
     cached N costs a few small copies and two graph launches instead of ~220 us of Python / allocator / launch work.  A
     new N runs the eager path the first ``capture_after`` times it is seen and is captured after that; at most
     ``max_graphs`` counts stay cached (least recently used first out).  The "others" sampler's seed advances on the device

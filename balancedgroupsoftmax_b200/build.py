@@ -1,4 +1,4 @@
-"""Build libbags_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libbags_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m balancedgroupsoftmax_b200.build [--force] [--verbose]
 """
@@ -13,11 +13,11 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, 'csrc')
 OUT = os.path.join(_HERE, 'libbags_b200.so')
 SOURCES = [os.path.join(CSRC, 'bags_api.cu')]
-HEADERS = [os.path.join(CSRC, f) for f in ('bags_ptx.cuh', 'bags_gemm.cuh', 'bags_kernels.cuh', 'bags_fused_fwd.cuh', 'bags_bwd_fused.cuh', 'bags_allreduce.cuh', 'bags_nms.cuh')] + [
+HEADERS = [os.path.join(CSRC, f) for f in ('bags_ptx.cuh', 'bags_wgmma.cuh', 'bags_gemm.cuh', 'bags_kernels.cuh', 'bags_fused_fwd.cuh', 'bags_allreduce.cuh', 'bags_nms.cuh')] + [
     os.path.join(os.path.dirname(_HERE), 'include', 'bags_b200.h')]
 
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
     '-shared', '-Xcompiler', '-fPIC',
 ]
 

@@ -1,4 +1,4 @@
-// Gradient exchange of the fc_cls bucket over NVLink peer memory (sm_100a, NVSwitch).
+// Gradient exchange of the fc_cls bucket over NVLink peer memory (sm_90a, NVSwitch).
 //
 // Replaces the reference's NCCL all-reduce + div of the flattened gradients
 // (mmdet/core/utils/dist_utils.py:9-41: _allreduce_coalesced -> dist.all_reduce, tensor.div_(world_size),
@@ -13,8 +13,7 @@
 //   barrier (every rank's slice has landed everywhere)
 //
 // Each element is reduced by exactly one rank in a fixed order, so all ranks end with bit-identical buckets.
-// 5.07 MB per head: 2 * (N-1)/N * 5.07 MB cross each GPU's links (~6-9 us at 770 GB/s) plus two flag round
-// trips; NCCL's ring/tree launch measured ~53 us per step for the same bucket (profiles/r01_bench_2gpu_v5.json).
+// 5.07 MB per head: 2 * (N-1)/N * 5.07 MB cross each GPU's links plus two flag round trips.
 //
 // Flags (inside every rank's bucket allocation, zeroed once by the caller):
 //   slot[b][r]  written by rank r's block b with an EPOCH number (st.release.sys, fire and forget), polled locally by

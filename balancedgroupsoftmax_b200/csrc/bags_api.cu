@@ -14,7 +14,6 @@
 #include "../../include/bags_b200.h"
 #include "bags_gemm.cuh"
 #include "bags_fused_fwd.cuh"
-#include "bags_bwd_fused.cuh"
 #include "bags_kernels.cuh"
 #include "bags_allreduce.cuh"
 #include "bags_nms.cuh"
@@ -65,11 +64,8 @@ static bool g_dev_ok[64] = {false};
 
 // test hook: device buffer [ctas][8] int64 that the next launches stamp with %globaltimer values
 static long long* g_timing = nullptr;
-static int g_dbg = 0;
 extern "C" int bags_debug_set_timing(void* dev_ptr) {
   g_timing = reinterpret_cast<long long*>(dev_ptr);
-  g_dbg = 0;
-  if (const char* v = getenv("BAGS_DBG")) g_dbg = atoi(v);   // test hook, not on the per-step path
   return BAGS_OK;
 }
 
@@ -78,34 +74,6 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 static EncodeTiledFn g_encode = nullptr;
-
-// Library-owned counter pairs for the merged backward kernel's in-kernel grid synchronisation: one 256-byte slot
-// per (device, stream) that has used it, zeroed once here and left zero by every launch.
-static unsigned int* g_sync_pool[64] = {nullptr};
-static cudaStream_t g_sync_streams[64][64];
-static int g_sync_count[64] = {0};
-static unsigned int* sync_slot(int dev, cudaStream_t stream) {
-  std::lock_guard<std::mutex> lk(g_mutex);
-  if (g_sync_pool[dev] == nullptr) {
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    if (cudaStreamIsCapturing(stream, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
-      (void)cudaGetLastError();
-      return nullptr;   // cannot allocate while capturing: the caller falls back to the separate preparation kernel
-    }
-    void* ptr = nullptr;
-    if (cudaMalloc(&ptr, 64 * 256) != cudaSuccess || cudaMemset(ptr, 0, 64 * 256) != cudaSuccess) {
-      (void)cudaGetLastError();
-      return nullptr;
-    }
-    g_sync_pool[dev] = static_cast<unsigned int*>(ptr);
-  }
-  for (int i = 0; i < g_sync_count[dev]; ++i)
-    if (g_sync_streams[dev][i] == stream) return g_sync_pool[dev] + i * 64;
-  if (g_sync_count[dev] >= 64) return nullptr;
-  const int i = g_sync_count[dev]++;
-  g_sync_streams[dev][i] = stream;
-  return g_sync_pool[dev] + i * 64;
-}
 
 static int device_info(DeviceInfo& out) {
   int dev = 0;
@@ -120,8 +88,8 @@ static int device_info(DeviceInfo& out) {
     g_dev_ok[dev] = true;
   }
   out = g_dev[dev];
-  if (out.cc_major != 10)
-    return fail(BAGS_ERR_ARCH, "libbags_b200 requires an sm_100 (B200) device; found compute capability %d.x",
+  if (out.cc_major != 9)
+    return fail(BAGS_ERR_ARCH, "libbags_b200 is built for sm_90a (H100); found compute capability %d.x",
                 out.cc_major);
   if (g_encode == nullptr) {
     void* fn = nullptr;
@@ -236,17 +204,17 @@ static int launch_gemm(const GemmArgs& ga, const DeviceInfo& di, cudaStream_t st
   auto kernel = bags_gemm_kernel<BLOCK_N, A_MN, B_MN, EPI, TF32, STAGES>;
   CUtensorMap ta, tb;
   int rc;
-  // A
-  if (A_MN) rc = make_tmap(&ta, ga.a, ga.dtype, ga.M, ga.K, ga.lda, Cfg::SLAB, Cfg::BLOCK_K, TF32);
+  // A (an MN-major fp32 operand is read without TMA: the tensor map is still encoded, which validates alignment)
+  if (A_MN) rc = make_tmap(&ta, ga.a, ga.dtype, ga.M, ga.K, ga.lda, Cfg::SLAB, Cfg::BLOCK_K);
   else      rc = make_tmap(&ta, ga.a, ga.dtype, ga.K, ga.M, ga.lda, Cfg::BLOCK_K, Cfg::BLOCK_M);
   if (rc) return rc;
-  if (B_MN) rc = make_tmap(&tb, ga.b, ga.dtype, ga.N, ga.K, ga.ldb, Cfg::SLAB, Cfg::BLOCK_K, TF32);
-  else      rc = make_tmap(&tb, ga.b, ga.dtype, ga.K, ga.N, ga.ldb, Cfg::BLOCK_K, Cfg::UMMA_N);
+  if (B_MN) rc = make_tmap(&tb, ga.b, ga.dtype, ga.N, ga.K, ga.ldb, Cfg::SLAB, Cfg::BLOCK_K);
+  else      rc = make_tmap(&tb, ga.b, ga.dtype, ga.K, ga.N, ga.ldb, Cfg::BLOCK_K, BLOCK_N);
   if (rc) return rc;
 
   GemmParams p = ga.p;
-  p.timing = g_timing;
-  p.dbg = g_timing ? g_dbg : 0;
+  p.a_ptr = static_cast<const float*>(ga.a); p.lda = ga.lda; p.a_rows = ga.M; p.a_k = ga.K;
+  p.b_ptr = static_cast<const float*>(ga.b); p.ldb = ga.ldb; p.b_rows = ga.N; p.b_k = ga.K;
   p.M = ga.M; p.N = ga.N; p.K = ga.K;
   p.num_m_tiles = (ga.M + Cfg::BLOCK_M - 1) / Cfg::BLOCK_M;
   p.num_n_tiles = (ga.N + BLOCK_N - 1) / BLOCK_N;
@@ -286,18 +254,6 @@ static int pick_splits(int tiles, int kblocks, int num_sms) {
   return s;
 }
 
-// forward tile width: fewest (waves x tile width)
-static int pick_fwd_block_n(int N, int C, int num_sms) {
-  const int forced = env_int("BAGS_FWD_BN", 0);
-  if (forced == 256 || forced == 320) return forced;
-  const int mt = (N + 127) / 128;
-  auto cost = [&](int bn) {
-    const int tiles = mt * ((C + bn - 1) / bn);
-    return ((tiles + num_sms - 1) / num_sms) * bn;
-  };
-  return cost(320) < cost(256) ? 320 : 256;
-}
-
 // ----------------------------------------------------------------------------
 // public entry points
 // ----------------------------------------------------------------------------
@@ -322,16 +278,11 @@ extern "C" int bags_linear_fwd(const void* x, long long ldx, const void* w, long
   ga.M = N; ga.N = C; ga.K = K; ga.dtype = dtype; ga.splits = 1;
   ga.p.out = out; ga.p.ldo = ldo; ga.p.bias = bias; ga.p.gscale = nullptr; ga.p.G = 0;
   ga.p.colsum_in = nullptr; ga.p.colsum_out = nullptr;
-  const int bn = pick_fwd_block_n(N, C, di.num_sms);
-  if (dtype == BAGS_DTYPE_BF16) {
-    return bn == 320 ? launch_gemm<320, false, false, EPI_STORE_F32, false, 3>(ga, di, stream)
-                     : launch_gemm<256, false, false, EPI_STORE_F32, false, 4>(ga, di, stream);
-  }
-  return bn == 320 ? launch_gemm<320, false, false, EPI_STORE_F32, true, 3>(ga, di, stream)
-                   : launch_gemm<256, false, false, EPI_STORE_F32, true, 4>(ga, di, stream);
+  if (dtype == BAGS_DTYPE_BF16) return launch_gemm<256, false, false, EPI_STORE_F32, false, 4>(ga, di, stream);
+  return launch_gemm<256, false, false, EPI_STORE_F32, true, 4>(ga, di, stream);
 }
 
-// y = act(x W^T + b): the head's shared FCs (ReLU) and fc_reg (identity) on the same tcgen05 pipeline
+// y = act(x W^T + b): the head's shared FCs (ReLU) and fc_reg (identity) on the same wgmma pipeline
 // (convfc_bbox_head.py:138-143,167: nn.Linear + ReLU through cuBLAS / ATen in the reference)
 extern "C" int bags_linear_act_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
                                    void* out, long long ldo, int N, int K, int C, int dtype, int out_dtype, int relu,
@@ -360,7 +311,7 @@ extern "C" int bags_linear_act_fwd(const void* x, long long ldx, const void* w, 
 }
 
 // Split-K factor worth using for a forward layer (1 = the single-pass kernel): few output tiles and a long contraction --
-// shared_fcs.0 at 2 x 512 RoIs is 8 x 4 tiles of 128 x 256 with K = 12544, i.e. 32 busy SMs out of 148 without it.
+// shared_fcs.0 at 2 x 512 RoIs is 8 x 4 tiles of 128 x 256 with K = 12544, i.e. 32 busy SMs out of 132 without it.
 extern "C" int bags_linear_act_splits(int N, int K, int C, int dtype) {
   DeviceInfo di;
   if (device_info(di)) return 1;
@@ -399,7 +350,7 @@ extern "C" int bags_linear_act_fwd_splitk(const void* x, long long ldx, const vo
   if (rc) return rc;
   const long long quads = static_cast<long long>(N) * ((C + 3) / 4);
   long long grid = (quads + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   if (out_dtype == BAGS_DTYPE_BF16)
     bias_act_store_kernel<true><<<static_cast<unsigned>(grid), 256, 0, stream>>>(ws, ldws, bias, out, ldo, N, C, relu ? 1 : 0);
   else
@@ -420,7 +371,7 @@ extern "C" int bags_act_bwd(const void* dy, long long lddy, int dy_dtype, const 
   const bool f_dy = dy_dtype == BAGS_DTYPE_F32, f_y = y_dtype == BAGS_DTYPE_F32, f_g = g_dtype == BAGS_DTYPE_F32;
   const long long quads = static_cast<long long>(rows) * (cols / 4);
   long long grid = (quads + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   const dim3 gr(static_cast<unsigned>(grid)), bl(256);
   typedef __nv_bfloat16 bf;
 #define BAGS_ACT(TDY, TY, OB) act_bwd_kernel<TDY, TY, OB><<<gr, bl, 0, stream>>>(                                   \
@@ -583,14 +534,6 @@ static bool fused_eligible(const int32_t* slices_host, int G, int C) {
     end += slices_host[2 * g + 1];
   }
   if (end != C) return false;
-  for (int c0 = 0; c0 < C; c0 += 16) {   // at most two bins per 16-column chunk
-    int cnt = 0;
-    for (int g = 0; g < G; ++g) {
-      const int s = slices_host[2 * g], e = s + slices_host[2 * g + 1];
-      if (s < c0 + 16 && e > c0) ++cnt;
-    }
-    if (cnt > 2) return false;
-  }
   return env_int("BAGS_FUSED", 1) != 0;
 }
 
@@ -606,7 +549,7 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   CUtensorMap tx, tw;
   int rc = make_tmap(&tx, x, dtype, p0.K, p0.N, ldx, Cfg::BLOCK_K, Cfg::BLOCK_M);
   if (rc) return rc;
-  rc = make_tmap(&tw, w, dtype, p0.K, p0.C, ldw, Cfg::BLOCK_K, Cfg::UMMA_N);
+  rc = make_tmap(&tw, w, dtype, p0.K, p0.C, ldw, Cfg::BLOCK_K, Cfg::HALF_N);
   if (rc) return rc;
   if (dz != nullptr && (reinterpret_cast<uintptr_t>(dz) & 15) != 0)
     return fail(BAGS_ERR_INVALID, "bags_fwd: dz must be 16-byte aligned");
@@ -615,8 +558,6 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   p.ldd = ldd;
   p.kblocks = (p.K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
   p.want_dz = dz != nullptr ? 1 : 0;
-  p.timing = g_timing;
-  p.dbg = g_timing ? g_dbg : 0;
   auto kernel = wf ? bags_fwd_fused_kernel<TF32, true> : bags_fwd_fused_kernel<TF32, false>;
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   const int grid = Cfg::CLUSTER * ((p.N + Cfg::BLOCK_M - 1) / Cfg::BLOCK_M);
@@ -668,7 +609,7 @@ static int fwd_impl(const void* x, long long ldx, const void* w, long long ldw,
     return group_ce_impl(logits, ldz, labels, label2bin, slices_host, wmask, wf, avg, N, C, G, classes, loss,
                          lse, dz, ldd, dtype, colsum, workspace, workspace_bytes, stream_);
   }
-  // fused path: logits stay in TMEM
+  // fused path: logits stay in registers
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   BAGS_REQUIRE(fused_eligible(slices_host, G, C),
                "bags_fwd: logits == NULL requests the fused kernel, but this bin table / C=%d / G=%d is not eligible "
@@ -764,114 +705,25 @@ scale_colsum_kernel(const float* __restrict__ colsum, int tiles, float* __restri
 }
 
 
-template <bool TF32, int MT>
-static int launch_bwd_merged(const void* dz, long long ldd, const void* x, long long ldx, const void* wb, const void* w,
-                             long long ldw, const BwdFusedParams& p0, const DeviceInfo& di, cudaStream_t stream) {
-  using Cfg = BwdCfg<TF32, MT>;
+template <bool TF32>
+static int launch_bwd_merged(const void* dz, long long ldd, const void* x, long long ldx, const void* w, const void* wb,
+                             long long ldw, const BwdMergedParams& bp, const DeviceInfo& di, cudaStream_t stream) {
+  using CW = BwdDwCfg<TF32>;
+  using CX = BwdDxCfg<TF32>;
   const int dtype = TF32 ? BAGS_DTYPE_F32 : BAGS_DTYPE_BF16;
-  CUtensorMap t_dzT, t_xT, t_dz, t_wT, t_w;
+  const int C = bp.dw.M, K = bp.dw.N, N = bp.dw.K;
+  CUtensorMap t_dzT, t_xT, t_dz, t_w, t_wp;
   int rc;
-  if ((rc = make_tmap(&t_w, w, dtype, p0.Kf, p0.C, ldw, Cfg::SLAB, Cfg::BLOCK_K, TF32))) return rc;
-  if ((rc = make_tmap(&t_dzT, dz, dtype, p0.C, p0.Nr, ldd, Cfg::SLAB, Cfg::BLOCK_K, TF32))) return rc;
-  if ((rc = make_tmap(&t_xT, x, dtype, p0.Kf, p0.Nr, ldx, Cfg::SLAB, Cfg::BLOCK_K, TF32))) return rc;
-  if ((rc = make_tmap(&t_dz, dz, dtype, p0.C, p0.Nr, ldd, Cfg::BLOCK_K, Cfg::BLOCK_M))) return rc;
-  if ((rc = make_tmap(&t_wT, wb, dtype, p0.Kf, p0.C, ldw, Cfg::SLAB, Cfg::BLOCK_K, TF32))) return rc;
-  BwdFusedParams p = p0;
-  p.timing = g_timing ? g_timing + 2048 * 8 : nullptr;   // rows [2048, ..): the forward of the same step uses [0, 2048)
-  if (p.dw_units > 0 && p.dw_splits == 1 && p.prep_jobs > 0) {
-    // no split-K: every dW unit owns its output tile -> plain stores, and the zeroing job (the first z_ctas tickets)
-    // disappears.  (Only with in-kernel preparation: a separate preparation kernel has already been launched.)
-    p.dw_store = 1;
-    p.prep_jobs -= p.prep.z_ctas;
-    p.prep.z_ctas = 0;
-    if (p.prep.c_ctas == 0) p.dw_needs_prep = 0;
-  }
-  // preparation jobs handed out by an atomic ticket (no co-residency requirement); BAGS_BWD_TICKET=0: static assignment
-  auto kernel = (p.prep_jobs > 0 && env_int("BAGS_BWD_TICKET", 1)) ? bags_bwd_fused_kernel<TF32, MT, true>
-                                                                  : bags_bwd_fused_kernel<TF32, MT, false>;
-  BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  const int units = p.dw_units + p.dx_units;
+  if ((rc = make_tmap(&t_dzT, dz, dtype, C, N, ldd, CW::SLAB, CW::BLOCK_K))) return rc;   // dW: A = dz^T
+  if ((rc = make_tmap(&t_xT, x, dtype, K, N, ldx, CW::SLAB, CW::BLOCK_K))) return rc;     // dW: B = x^T
+  if ((rc = make_tmap(&t_dz, dz, dtype, C, N, ldd, CX::BLOCK_K, CX::BLOCK_M))) return rc;  // dX: A = dz
+  if ((rc = make_tmap(&t_w, w, dtype, K, C, ldw, CX::SLAB, CX::BLOCK_K))) return rc;      // dX: B = W^T
+  if ((rc = make_tmap(&t_wp, wb, dtype, K, C, ldw, CX::SLAB, CX::BLOCK_K))) return rc;    // dX: B = W'^T
+  auto kernel = bags_bwd_merged_kernel<TF32>;
+  BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CW::SMEM_BYTES));
+  const int units = bp.dw_units + bp.dx_units;
   const int grid = units < di.num_sms ? units : di.num_sms;
-  BAGS_CUDA(launch_pdl(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, t_dzT, t_xT, t_dz, t_wT, t_w, p));
-  return BAGS_OK;
-}
-
-// CTA pairs that can be co-resident (GPCs with an odd number of usable SMs leave one SM without a partner)
-template <bool TF32>
-static int pair_capacity(const DeviceInfo& di) {
-  static int cached[2] = {0, 0};
-  int& c = cached[TF32 ? 1 : 0];
-  if (c > 0) return c;
-  using Cfg = BwdPairCfg<TF32>;
-  auto kernel = bags_bwd_pair_kernel<TF32>;
-  int n = di.num_sms / 2;
-  if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES) == cudaSuccess) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2 * (di.num_sms / 2));
-    cfg.blockDim = dim3(Cfg::NUM_THREADS);
-    cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int q = 0;
-    if (cudaOccupancyMaxActiveClusters(&q, kernel, &cfg) == cudaSuccess && q > 0 && q < n) n = q;
-    else (void)cudaGetLastError();
-  }
-  const int forced = env_int("BAGS_PAIRS", 0);
-  if (forced > 0 && forced < n) n = forced;
-  c = n;
-  return c;
-}
-
-// split-K factor of the dW units for the pair kernel: fewest (rounds x longest unit), units costed in k-blocks
-static int pick_pair_splits(int dw_tiles, int dw_kblocks, int dx_units, int dx_kblocks, int pairs) {
-  int best = 1;
-  long best_cost = -1;
-  for (int s = 1; s <= 16 && s <= dw_kblocks; ++s) {
-    const int units = dw_tiles * s + dx_units;
-    const int rounds = (units + pairs - 1) / pairs;
-    const int dwk = (dw_kblocks + s - 1) / s;
-    const long unit = ((dx_units > 0 && dx_kblocks > dwk) ? dx_kblocks : dwk) + 4;   // + epilogue, in k-block equivalents
-    const long cost = rounds * unit;
-    if (best_cost < 0 || cost < best_cost) { best_cost = cost; best = s; }
-  }
-  return best;
-}
-
-// CTA-pair (cta_group::2) variant: cluster of 2, units are 256-row pairs
-template <bool TF32>
-static int launch_bwd_pair(const void* dz, long long ldd, const void* x, long long ldx, const void* wb, long long ldw,
-                           const BwdFusedParams& p0, const DeviceInfo& di, cudaStream_t stream) {
-  using Cfg = BwdPairCfg<TF32>;
-  const int dtype = TF32 ? BAGS_DTYPE_F32 : BAGS_DTYPE_BF16;
-  CUtensorMap t_dzT, t_xT, t_dz, t_wT;
-  int rc;
-  if ((rc = make_tmap(&t_dzT, dz, dtype, p0.C, p0.Nr, ldd, Cfg::SLAB, Cfg::BLOCK_K, TF32))) return rc;
-  if ((rc = make_tmap(&t_xT, x, dtype, p0.Kf, p0.Nr, ldx, Cfg::SLAB, Cfg::BLOCK_K, TF32))) return rc;
-  if ((rc = make_tmap(&t_dz, dz, dtype, p0.C, p0.Nr, ldd, Cfg::BLOCK_K, Cfg::BLOCK_M))) return rc;
-  if ((rc = make_tmap(&t_wT, wb, dtype, p0.Kf, p0.C, ldw, Cfg::SLAB, Cfg::BLOCK_K, TF32))) return rc;
-  BwdFusedParams p = p0;
-  p.timing = g_timing ? g_timing + 2048 * 8 : nullptr;
-  auto kernel = bags_bwd_pair_kernel<TF32>;
-  BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  const int units = p.dw_units + p.dx_units;
-  const int max_pairs = pair_capacity<TF32>(di);
-  const int pairs = units < max_pairs ? units : max_pairs;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pairs);
-  cfg.blockDim = dim3(Cfg::NUM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = env_int("BAGS_PDL", 1) ? 2 : 1;
-  BAGS_CUDA(cudaLaunchKernelEx(&cfg, kernel, t_dzT, t_xT, t_dz, t_wT, p));
+  BAGS_CUDA(launch_pdl(kernel, dim3(grid), dim3(CW::NUM_THREADS), CW::SMEM_BYTES, stream, t_dzT, t_xT, t_dz, t_w, t_wp, bp));
   return BAGS_OK;
 }
 
@@ -944,32 +796,11 @@ extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long lo
     BAGS_REQUIRE(((ldd * (bf ? 2 : 4)) % 16) == 0 && (reinterpret_cast<uintptr_t>(dz) & 15) == 0,
                  "bags_bwd: dz rows must be 16-byte aligned");
 
-  // ---- preparation: zero dW, W' = gout-scaled W, bias-gradient partial column sums.  On the merged single-CTA path
-  // these jobs run inside the GEMM kernel (no extra launch in the dependent chain); otherwise one small kernel. ----
-  // dW (+ db) alone also runs on the merged kernel (no dX units): in-kernel preparation, 256 x 256 units when the
-  // problem is large enough -- the launch the split in-step schedule (dW -> exchange || dX) puts on its critical path
-  // ... unless there is nothing to prepare (dW zeroed and the bias-gradient partials supplied by the forward): then the
-  // plain split-K GEMM (4-stage ring, no job machinery) is the faster dW-only launch -- 52.9 vs 53.7 us per
-  // forward + dW-only + dX-only sequence, and 54.6 with the jobs in the backward (profiles/r02_dwonly_path.log)
-  const bool nothing_to_prepare = prezeroed && (db == nullptr || colsum != nullptr);
-  const bool dw_only_merged = dW != nullptr && dX == nullptr && w != nullptr && N > 0 && (K % 8) == 0 &&
-                              (reinterpret_cast<uintptr_t>(w) & 15) == 0 && !env_int("BAGS_BWD_PAIR", 0) &&
-                              env_int("BAGS_BWD_DW_MERGED", nothing_to_prepare ? 0 : 1);
-  // dX alone with per-bin upstream gradients: the merged kernel decides ON THE DEVICE whether they are uniform (then it
-  // reads W and scales in the epilogue: no scaled copy W', no preparation launch); with gout == NULL the plain GEMM is used
-  const bool dx_only_merged = dW == nullptr && db == nullptr && dX != nullptr && gout != nullptr && x != nullptr &&
-                              w != nullptr && N > 0 && (K % 8) == 0 && env_int("BAGS_BWD_DX_MERGED", 1) &&
-                              !env_int("BAGS_BWD_PAIR", 0);
-  const bool merged_path = ((dW != nullptr && dX != nullptr && N > 0 && (K % 8) == 0) || dw_only_merged || dx_only_merged) &&
-                           env_int("BAGS_BWD_MERGED", 1);
-  unsigned int* sync = nullptr;
-  if (merged_path && !env_int("BAGS_BWD_PAIR", 0) && env_int("BAGS_BWD_INKERNEL_PREP", 1)) {
-    int dev = 0;
-    BAGS_CUDA(cudaGetDevice(&dev));
-    sync = sync_slot(dev, stream);
-  }
+  // ---- preparation (one small kernel): zero dW, W' = gout-scaled W, bias-gradient partial column sums; then both
+  // contractions in one merged launch, or the one requested as a plain split-K dW (red.add) / dX GEMM ----
+  // both contractions requested: one merged persistent launch after the preparation kernel (see bags_bwd_merged_kernel)
+  const bool merged = dW != nullptr && dX != nullptr && N > 0 && env_int("BAGS_BWD_MERGED", 1);
   BwdPrepParams pp{};
-  int prep_jobs = 0;
   bool prep_launched = false;
   if (dW != nullptr || want_scale || want_colpart) {
     pp.dW = dW; pp.lddw = lddw; pp.C = C; pp.K = K;
@@ -978,9 +809,9 @@ extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long lo
     pp.z_ctas = (dW != nullptr && !prezeroed) ? di.num_sms : 0;
     pp.s_ctas = want_scale ? di.num_sms : 0;
     pp.c_ctas = want_colpart ? ((C + 63) / 64) * kColsumTiles : 0;
+    pp.skip_scale_if_uniform = merged ? 1 : 0;   // the merged kernel reads W itself when all gout[g] are equal
     const int grid = pp.z_ctas + pp.s_ctas + pp.c_ctas;
     if (grid == 0) { /* nothing to prepare */ }
-    else if (sync != nullptr) prep_jobs = grid;
     else if (bf) { BAGS_CUDA(launch_pdl(bwd_prep_kernel<false>, dim3(grid), dim3(256), 0, stream, pp)); prep_launched = true; }
     else         { BAGS_CUDA(launch_pdl(bwd_prep_kernel<true>, dim3(grid), dim3(256), 0, stream, pp)); prep_launched = true; }
   }
@@ -988,70 +819,50 @@ extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long lo
   const int cs_tiles = (colsum != nullptr) ? colsum_tiles : kColsumTiles;
   if (db != nullptr) BAGS_REQUIRE(cs_in != nullptr && cs_tiles >= 1, "bags_bwd: db requested but no column sums available");
 
-  // ---- both contractions in one persistent launch when both are requested ----
-  if (merged_path) {
-    BAGS_REQUIRE(w != nullptr, "bags_bwd: w is NULL but dX requested");
-    if (dX != nullptr)
-      BAGS_REQUIRE((reinterpret_cast<uintptr_t>(dX) & 15) == 0 && ((lddx * (bf ? 2 : 4)) % 16) == 0,
-                   "bags_bwd: dX rows must be 16-byte aligned");
+  if (merged) {
+    BAGS_REQUIRE(w != nullptr && x != nullptr, "bags_bwd: w / x is NULL but dW and dX requested");
+    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(dX) & 15) == 0, "bags_bwd: dX not 16-byte aligned");
     const int bk = bf ? 64 : 32;
-    BwdFusedParams bp{};
-    bp.C = C; bp.Kf = K; bp.Nr = N;
-    bp.dw_m_tiles = (C + 127) / 128; bp.dw_n_tiles = (K + 255) / 256; bp.dw_kblocks = (N + bk - 1) / bk;
-    bp.dw_splits = env_int("BAGS_DW_SPLITS", pick_splits(bp.dw_m_tiles * bp.dw_n_tiles, bp.dw_kblocks, di.num_sms));
-    if (bp.dw_splits > bp.dw_kblocks) bp.dw_splits = bp.dw_kblocks;
-    bp.dx_m_tiles = (N + 127) / 128; bp.dx_n_tiles = (K + 255) / 256; bp.dx_kblocks = (C + bk - 1) / bk;
-    bp.dw_units = (dW != nullptr) ? bp.dw_m_tiles * bp.dw_n_tiles * bp.dw_splits : 0;
-    bp.dx_units = (dX != nullptr) ? bp.dx_m_tiles * bp.dx_n_tiles : 0;
-    bp.dW = dW; bp.lddw = lddw; bp.dX = dX; bp.lddx = lddx;
-    bp.gscale = gout; bp.G = (gout != nullptr) ? gt.G : 0;
-    for (int g = 0; g < kMaxGroups; ++g) { bp.gstart[g] = gt.start[g]; bp.glen[g] = gt.len[g]; }
-    bp.colsum_in = (db != nullptr) ? cs_in : nullptr;
-    bp.colsum_tiles = cs_tiles;
-    bp.db = db;
-    bp.prep = pp; bp.prep_jobs = prep_jobs; bp.sync = sync;
-    // the first operand load must wait for the producer of dz unless a preparation kernel sits in between (its own wait
-    // covers it); the dW epilogues only depend on the zeroing / column-sum jobs
-    bp.wait_dz = (prep_jobs > 0 || !prep_launched) ? 1 : 0;
-    bp.dw_needs_prep = (pp.z_ctas > 0 || pp.c_ctas > 0 || prep_launched) ? 1 : 0;
+    BwdMergedParams bp{};
+    GemmParams& pw = bp.dw;
+    pw.M = C; pw.N = K; pw.K = N;
+    pw.num_m_tiles = (C + 127) / 128; pw.num_n_tiles = (K + 255) / 256; pw.kblocks_total = (N + bk - 1) / bk;
+    GemmParams& px = bp.dx;
+    px.M = N; px.N = K; px.K = C;
+    px.num_m_tiles = (N + 127) / 128; px.num_n_tiles = (K + 255) / 256; px.kblocks_total = (C + bk - 1) / bk;
+    px.num_splits = 1;
+    // split-K factor of the dW units: fewest (rounds of the work list over the SMs x longest unit), in k-blocks
+    const int dw_tiles = pw.num_m_tiles * pw.num_n_tiles, dx_units = px.num_m_tiles * px.num_n_tiles;
+    int splits = 1;
+    long best = -1;
+    for (int sp = 1; sp <= 16 && sp <= pw.kblocks_total; ++sp) {
+      const long rounds = (dw_tiles * sp + dx_units + di.num_sms - 1) / di.num_sms;
+      const int dwk = (pw.kblocks_total + sp - 1) / sp;
+      const long cost = rounds * (dwk > px.kblocks_total ? dwk : px.kblocks_total);
+      if (best < 0 || cost < best) { best = cost; splits = sp; }
+    }
+    splits = env_int("BAGS_DW_SPLITS", splits);
+    if (splits < 1) splits = 1;
+    if (splits > pw.kblocks_total) splits = pw.kblocks_total;
+    pw.num_splits = splits;
+    pw.out = dW; pw.ldo = lddw;
+    pw.gscale = gout; pw.G = (gout != nullptr) ? gt.G : 0;
+    for (int g = 0; g < kMaxGroups; ++g) { pw.gstart[g] = gt.start[g]; pw.glen[g] = gt.len[g]; }
+    pw.colsum_in = (db != nullptr) ? cs_in : nullptr;
+    pw.colsum_tiles = cs_tiles;
+    pw.colsum_out = db;
+    pw.a_ptr = static_cast<const float*>(dz); pw.lda = ldd; pw.a_rows = C; pw.a_k = N;
+    pw.b_ptr = static_cast<const float*>(x); pw.ldb = ldx; pw.b_rows = K; pw.b_k = N;
     const void* wb = want_scale ? wscratch : w;
-    if (env_int("BAGS_BWD_PAIR", 0)) {
-      // units are 256-row CTA pairs
-      bp.dw_m_tiles = (bp.dw_m_tiles + 1) / 2;
-      bp.dx_m_tiles = (bp.dx_m_tiles + 1) / 2;
-      const int cap = bf ? pair_capacity<false>(di) : pair_capacity<true>(di);
-      bp.dw_splits = env_int("BAGS_DW_SPLITS", pick_pair_splits(bp.dw_m_tiles * bp.dw_n_tiles, bp.dw_kblocks,
-                                                                bp.dx_m_tiles * bp.dx_n_tiles, bp.dx_kblocks, cap));
-      if (bp.dw_splits > bp.dw_kblocks) bp.dw_splits = bp.dw_kblocks;
-      bp.dw_units = bp.dw_m_tiles * bp.dw_n_tiles * bp.dw_splits;
-      bp.dx_units = bp.dx_m_tiles * bp.dx_n_tiles;
-      const int only = env_int("BAGS_PAIR_ONLY", 0);   // timing experiments: 1 = dW units only, 2 = dX units only
-      if (only == 1) bp.dx_units = 0;
-      if (only == 2) bp.dw_units = 0;
-      return bf ? launch_bwd_pair<false>(dz, ldd, x, ldx, wb, ldw, bp, di, stream)
-                : launch_bwd_pair<true>(dz, ldd, x, ldx, wb, ldw, bp, di, stream);
-    }
-    bp.dx_uniform_ok = (want_scale && env_int("BAGS_DX_UNIFORM", 1)) ? 1 : 0;
-    bp.prep.skip_scale_if_uniform = (bp.dx_uniform_ok && prep_jobs > 0) ? 1 : 0;
-    // 256 x 256 units (two accumulator sub-tiles sharing the B tile) once the problem fills the machine with them
-    int mt_auto = (bp.dx_units + bp.dw_m_tiles * bp.dw_n_tiles >= di.num_sms) ? 2 : 1;
-    if (dW == nullptr) mt_auto = (bp.dx_units / 2 >= di.num_sms) ? 2 : 1;   // dX alone: 128-row units fill the machine sooner
-    // dW alone: 128 x 256 units.  Filling the machine with 256 x 256 units takes a 7-way split at the benchmark shape, i.e.
-    // 35 MB of red.add for a 5 MB result -- the L2 atomic rate (~3 TB/s) then costs more than the larger tile saves
-    if (dX == nullptr) mt_auto = env_int("BAGS_DW_ONLY_MT", 1);
-    if (env_int("BAGS_BWD_MT", mt_auto) == 2) {
-      bp.dw_m_tiles = (C + 255) / 256;
-      bp.dx_m_tiles = (N + 255) / 256;
-      bp.dx_units = (dX != nullptr) ? bp.dx_m_tiles * bp.dx_n_tiles : 0;
-      bp.dw_splits = env_int("BAGS_DW_SPLITS", pick_pair_splits(bp.dw_m_tiles * bp.dw_n_tiles, bp.dw_kblocks, bp.dx_units,
-                                                                bp.dx_kblocks, di.num_sms));
-      if (bp.dw_splits > bp.dw_kblocks) bp.dw_splits = bp.dw_kblocks;
-      bp.dw_units = (dW != nullptr) ? bp.dw_m_tiles * bp.dw_n_tiles * bp.dw_splits : 0;
-      return bf ? launch_bwd_merged<false, 2>(dz, ldd, x, ldx, wb, w, ldw, bp, di, stream)
-                : launch_bwd_merged<true, 2>(dz, ldd, x, ldx, wb, w, ldw, bp, di, stream);
-    }
-    return bf ? launch_bwd_merged<false, 1>(dz, ldd, x, ldx, wb, w, ldw, bp, di, stream)
-              : launch_bwd_merged<true, 1>(dz, ldd, x, ldx, wb, w, ldw, bp, di, stream);
+    px.out = dX; px.ldo = lddx;
+    px.b_ptr = static_cast<const float*>(wb); px.ldb = ldw; px.b_rows = K; px.b_k = C;
+    bp.dw_units = pw.num_m_tiles * pw.num_n_tiles * splits;
+    bp.dx_units = px.num_m_tiles * px.num_n_tiles;
+    bp.w = static_cast<const float*>(w);
+    bp.gout = gout;
+    bp.G = gt.G;
+    return bf ? launch_bwd_merged<false>(dz, ldd, x, ldx, w, wb, ldw, bp, di, stream)
+              : launch_bwd_merged<true>(dz, ldd, x, ldx, w, wb, ldw, bp, di, stream);
   }
 
   if (dW != nullptr && N > 0) {
@@ -1149,10 +960,9 @@ extern "C" int bags_grad_allreduce(void* const* peer_bufs_host, void* mc_buf, lo
   long long blocks = (per_rank + static_cast<long long>(threads) * 4 - 1) / (static_cast<long long>(threads) * 4);
   if (blocks < 1) blocks = 1;
   const bool mm = p.mc != nullptr && !env_int("BAGS_AR_NO_MULTIMEM", 0);
-  // Default grid (measured inside the step at 2 ranks, profiles/r02_exchange_2gpu.md): one block per SM on the multimem
-  // path (a 16-block grid, right for an exchange hidden under the NEXT step in round 1, costs 2x inside the step); the
-  // plain peer path keeps one vector per thread in flight.
-  if (max_blocks <= 0) max_blocks = env_int("BAGS_AR_MAX_BLOCKS", mm ? 148 : kArMaxBlocks);
+  // Default grid: one block per SM on the multimem path (the exchange runs inside the step, where a small grid leaves
+  // the switch bandwidth unused); the plain peer path keeps one vector per thread in flight.
+  if (max_blocks <= 0) max_blocks = env_int("BAGS_AR_MAX_BLOCKS", mm ? di.num_sms : kArMaxBlocks);
   if (max_blocks <= 0 || max_blocks > kArMaxBlocks) max_blocks = kArMaxBlocks;
   if (blocks > max_blocks) blocks = max_blocks;
   const bool epoch = env_int("BAGS_AR_EPOCH", 1) != 0;
@@ -1201,7 +1011,7 @@ extern "C" int bags_debug_spin(int blocks, int threads, int micros, void* stream
 }
 
 // test hook: how many clusters of `cluster` CTAs (each `threads` threads + `smem_bytes` dynamic shared memory, i.e. one CTA
-// per SM for the GEMM-sized value) can be resident at once -- the GPC layout decides (148 SMs do not split evenly)
+// per SM for the GEMM-sized value) can be resident at once -- the GPC layout decides (an SM count such as 132 does not split evenly)
 extern "C" int bags_debug_max_clusters(int cluster, int threads, int smem_bytes) {
   if (cluster < 1 || cluster > 16 || threads < 32 || threads > 1024 || smem_bytes < 0) return -1;
   DeviceInfo di;
@@ -1265,7 +1075,7 @@ extern "C" int bags_cast_bf16(const float* src, long long lds, void* dst, long l
   if (rows == 0 || cols == 0) return BAGS_OK;
   const long long total = (long long)rows * (cols / 4);
   long long grid = (total + 255) / 256;
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   cast_bf16_kernel<<<(int)grid, 256, 0, stream>>>(src, lds, reinterpret_cast<__nv_bfloat16*>(dst), ldd, rows, cols);
   BAGS_CUDA(cudaGetLastError());
   return BAGS_OK;
@@ -1287,9 +1097,6 @@ extern "C" int bags_gemm_probe(const void* a, long long lda, int a_mn, const voi
   const bool bf = dtype == BAGS_DTYPE_BF16;
   BAGS_REQUIRE(bf || dtype == BAGS_DTYPE_F32, "bags_gemm_probe: bad dtype");
   // the instantiations the product uses
-  if (!a_mn && !b_mn && epi == 0 && block_n == 320)
-    return bf ? launch_gemm<320, false, false, EPI_STORE_F32, false, 3>(ga, di, stream)
-              : launch_gemm<320, false, false, EPI_STORE_F32, true, 3>(ga, di, stream);
   if (!a_mn && !b_mn && epi == 0 && block_n == 256)
     return bf ? launch_gemm<256, false, false, EPI_STORE_F32, false, 4>(ga, di, stream)
               : launch_gemm<256, false, false, EPI_STORE_F32, true, 4>(ga, di, stream);

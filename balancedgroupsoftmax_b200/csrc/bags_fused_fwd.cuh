@@ -1,38 +1,31 @@
-// Fused BAGS forward for sm_100a:  fc_cls GEMM  ->  grouped softmax-CE  ->  dz~  in ONE kernel.
+// Fused BAGS forward for sm_90a:  fc_cls GEMM  ->  grouped softmax-CE  ->  dz~  in ONE kernel.
 //
-//   z = x W^T + b  is accumulated in TMEM and never written to HBM.
+//   z = x W^T + b  is accumulated in registers and never written to HBM.
 //
-// A cluster of 4 CTAs owns one 128-row tile of RoIs; CTA r holds logit columns [320r, 320r+320)
-// of those rows in its TMEM (128 lanes x 320 fp32 columns).  The epilogue maps ONE THREAD TO ONE
-// ROW (TMEM lane), so walking the columns of a bin is a plain sequential loop: no masks, no
-// shuffles, bin boundaries are warp-uniform.  16 epilogue warps (4 per TMEM lane quarter) each own an
-// 80-column group; the four groups' per-row partial (max, sum-exp) of every bin are combined inside the
-// CTA, and since bins usually span several CTAs the CTA-level partials are published to all four CTAs
-// through distributed shared memory; after one cluster barrier every thread combines the four
-// partials into the bin's log-sum-exp and makes a second pass over its TMEM columns:
+// A cluster of 4 CTAs owns one 128-row tile of RoIs; CTA r holds logit columns [320r, 320r+320) of those rows.
+// Warpgroup 0 is the producer (one TMA thread; its other three warps load the per-row labels / weights and run the
+// optional clear hook while the MMAs run); warpgroups 1 and 2 each own 64 rows and keep their 64 x 320 fp32
+// accumulators in registers (two wgmma m64n160 per K step).  In the wgmma fragment a row is held by the four lanes
+// of a quad (80 columns each), so row reductions are a walk over the thread's own columns plus two quad shuffles.
+// Bins are contiguous column ranges, so every walk keeps a running (bin, value) pair and touches shared memory only
+// where the bin changes:
 //
-//   bias -> TMEM before the first MMA (the accumulators start at b, so the epilogue never adds it)
-//   pass A  (after the mainloop):  per bin segment, online (max, sum exp(z - max)); the exponentials
-//            e = exp(z - m_chunk) are written back over z in TMEM, m_chunk (the running max they refer to)
-//            goes to shared memory (two floats per thread and chunk)
-//   exchange + barrier.cluster
-//   pass C:  dz~ = e * [ w/avg * exp(m_chunk - lse_bin) ] - onehot * w/avg : one MUFU per chunk instead of
-//            one per element  -> bf16/fp32 -> swizzled smem -> transposed, fully coalesced 16-byte stores ;
-//            column sums of dz~ (bias gradient) from the staged tile ;
-//            loss_bin += w/avg * -log p[target]
-//
-// Costs that shaped this (profiles/README.md): TMEM reads run at ~64 B/clk/SM (1.3 us per pass over the
-// 128 x 320 fp32 tile), MUFU at 4 lanes/clk per sub-partition, and the first version spent ~45 issue slots
-// per element on bin lookups, bias adds and generic-address shared loads.
+//   accumulators := bias before the first MMA (the epilogue never adds it)
+//   pass A  : per row and bin, the max over this CTA's columns; pass B: sum exp(z - max)
+//   exchange: every CTA sends its (max, sum) per row and bin to the four CTAs of the cluster (st.async into
+//             distributed shared memory, completion counted on an mbarrier); each combines the four into the lse
+//   pass C  : dz~ = w/avg * (exp(z - lse) - onehot) -> operand dtype -> HBM ; column sums of dz~ (bias gradient) ;
+//             loss_bin += w/avg * (lse - z[target])
 //
 // reference semantics: gs_bbox_head_with0.py:91-112 (labels/weights), :134-171 (slices + CE),
 // cross_entropy_loss.py:9-19, losses/utils.py:26-53 (sum / avg_factor).
 //
 // Preconditions (checked on the host, otherwise the unfused path runs): C <= 1280, G <= 6, bins
-// tile [0, C) contiguously, and no 32-column chunk intersects more than two bins.
+// tile [0, C) contiguously.
 #pragma once
 #include "bags_kernels.cuh"
 #include "bags_ptx.cuh"
+#include "bags_wgmma.cuh"
 
 namespace bags {
 
@@ -53,10 +46,8 @@ struct FusedFwdParams {
   void* dz;                 // [N, ldd] operand dtype, or nullptr (loss only)
   long long ldd;
   int want_dz;
-  long long* timing;        // debug timeline [grid][8] or nullptr
-  int dbg;                  // test hook: bit0 skip dz stores, bit2 skip column sums
-  // optional: a buffer the idle epilogue warps set to zero while the MMAs run (the caller's dW: the backward's split-K
-  // red.add then needs no zeroing job and, with `colsum` taken from here too, no preparation at all)
+  // optional: a buffer the producer warpgroup's idle warps set to zero while the MMAs run (the caller's dW: the
+  // backward's split-K red.add then needs no zeroing job)
   float4* clear;
   long long clear_vecs;
 };
@@ -65,42 +56,23 @@ template <bool TF32>
 struct FusedCfg {
   static constexpr int BLOCK_M = 128;
   static constexpr int BLOCK_N = 320;
-  static constexpr int UMMA_N = 160;
+  static constexpr int HALF_N = 160;
   static constexpr int STAGES = 3;
   static constexpr int ELT = TF32 ? 4 : 2;
   static constexpr int BLOCK_K = 128 / ELT;
-  static constexpr int UMMA_K = 32 / ELT;
-  static constexpr int K_STEPS = BLOCK_K / UMMA_K;
+  static constexpr int K_STEPS = 4;
   static constexpr int A_BYTES = BLOCK_M * 128;
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int CLUSTER = 4;
-  // Epilogue: 16 warps = 4 per TMEM lane quarter (thread = RoI row) x 4 column groups of 80 columns, walked in
-  // 16-column chunks.  Four warps per SM sub-partition hide the TMEM / shared-memory / MUFU latencies that left a
-  // two-warp version issue-bound at ~25 % (profiles/README.md).
-  static constexpr int EPI_WARPS = 16;
-  static constexpr int NUM_THREADS = 64 + 32 * EPI_WARPS;
-  static constexpr int CGROUPS = 4;
-  static constexpr int CG_COLS = BLOCK_N / CGROUPS;   // 80
-  static constexpr int CH = 16;                       // chunk width
-  static constexpr int CHUNKS = CG_COLS / CH;         // 5
+  static constexpr int NUM_THREADS = 384;
   static constexpr int MAXG = 6;
   static constexpr int XCH_BYTES = CLUSTER * MAXG * BLOCK_M * 8;   // cluster-level partials, float2 (max, sum)
-  static constexpr int LOC_BYTES = CGROUPS * MAXG * BLOCK_M * 8;   // CTA-local partials of the 4 column groups
-  static constexpr int DZ_ROW_BYTES = CH * (TF32 ? 4 : 2);         // one staged row of a chunk: 64 B / 32 B
-  static constexpr int DZ_BUF_BYTES = 2048;                        // per-warp staging buffer (32 rows)
-  static constexpr int META_BYTES = CGROUPS * 8 * 16;             // chunk table per column group (int4 per chunk)
-  static constexpr int MISC_BYTES = BLOCK_N * 4 /*bias*/ + 2 * MAXG * BLOCK_M * 4 /*tcol, coef*/ +
-                                    BLOCK_N * 4 /*colsum*/ + 64 /*loss*/ + META_BYTES + 256 /*barriers*/;
-  // after the mainloop the pipeline stages are idle: [0, 32 KB) stages the dz tiles, then the chunk references
-  static constexpr int REF_OFFSET = EPI_WARPS * DZ_BUF_BYTES;
-  static constexpr int REF_BYTES = CHUNKS * 32 * EPI_WARPS * 8;
-  static constexpr int ZT_OFFSET = REF_OFFSET + REF_BYTES;          // [MAXG][128] logit of each row's target column
-  static constexpr int ZT_BYTES = MAXG * BLOCK_M * 4;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + XCH_BYTES + LOC_BYTES + MISC_BYTES + 1024;
+  static constexpr int ROW_BYTES = 4 * MAXG * BLOCK_M * 4;          // tcol, coef, max, lse per (bin, row)
+  static constexpr int PART_BYTES = MAXG * 2 * 256 * 4;             // per-thread running partials
+  static constexpr int MISC_BYTES = 3 * BLOCK_N * 4 /*bias, bin, colsum*/ + 64 /*loss*/ + 256 /*barriers*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + XCH_BYTES + ROW_BYTES + PART_BYTES + MISC_BYTES + 1024;
   static_assert(SMEM_BYTES <= 232448, "fused forward exceeds shared memory");
-  static_assert(ZT_OFFSET + ZT_BYTES <= STAGES * STAGE_BYTES, "staging + references must fit in the idle pipeline buffers");
-  static_assert(32 * DZ_ROW_BYTES <= DZ_BUF_BYTES, "staging buffer too small");
 };
 
 __device__ __forceinline__ void cluster_arrive() {
@@ -109,39 +81,11 @@ __device__ __forceinline__ void cluster_arrive() {
 __device__ __forceinline__ void cluster_wait() {
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void cluster_arrive_wait() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
 }
-__device__ __forceinline__ void st_cluster_f2(uint32_t local_smem_addr, uint32_t rank, float a, float b) {
-  uint32_t raddr;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(local_smem_addr), "r"(rank));
-  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(raddr), "f"(a), "f"(b) : "memory");
-}
-// single-MUFU 2^x (ex2.approx.ftz, ~2 ulp): the inputs are <= 0 after max subtraction
-__device__ __forceinline__ float fast_exp2(float x) {
-#ifdef BAGS_X_NOMUFU   // timing experiment only: wrong results
-  return x * 0.5f;
-#else
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-#endif
-}
-#ifdef BAGS_X_NOTMEMLD   // timing experiment only: wrong results
-#define BAGS_TMEM_LD16(addr, regs) do { } while (0)
-#else
-#define BAGS_TMEM_LD16(addr, regs) tmem_ld_32x32b_x16(addr, regs)
-#endif
-#ifdef BAGS_X_NOTMEMST
-#define BAGS_TMEM_ST16(addr, regs) do { asm volatile("" :: "r"(regs[0]), "r"(regs[5]), "r"(regs[15])); } while (0)
-#else
-#define BAGS_TMEM_ST16(addr, regs) tmem_st_32x32b_x16(addr, regs)
-#endif
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
@@ -155,7 +99,7 @@ __device__ __forceinline__ void st_async_cluster_f2(uint32_t local_smem_addr, ui
   uint32_t raddr, rbar;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(raddr) : "r"(local_smem_addr), "r"(rank));
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbar) : "r"(local_bar_addr), "r"(rank));
-  asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];"
                ::"r"(raddr), "f"(a), "f"(b), "r"(rbar) : "memory");
 }
 __device__ __forceinline__ unsigned int atom_add_release_gpu(unsigned int* addr, unsigned int v) {
@@ -167,57 +111,52 @@ __device__ __forceinline__ unsigned int atom_add_release_gpu(unsigned int* addr,
 // WF = true: p.wmask points at fp32 per-(bin, RoI) weights instead of 0/1 bytes (the reweight head variant,
 // gs_bbox_head_with0_reweight.py:57-85)
 template <bool TF32, bool WF = false>
-__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(FusedCfg<TF32>::NUM_THREADS, 1)
+__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(384, 1)
 bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                       const FusedFwdParams p) {
   using Cfg = FusedCfg<TF32>;
   constexpr int BLOCK_M = Cfg::BLOCK_M, BLOCK_N = Cfg::BLOCK_N, BLOCK_K = Cfg::BLOCK_K, STAGES = Cfg::STAGES;
-  constexpr int MAXG = Cfg::MAXG, CH = Cfg::CH;
+  constexpr int MAXG = Cfg::MAXG, HALF_N = Cfg::HALF_N;
 
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1 KB aligned, still a shared-space pointer
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1 KB aligned
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;
-  float2* xch = reinterpret_cast<float2*>(smem + STAGES * Cfg::STAGE_BYTES);                 // [4 ranks][MAXG][128]
-  float2* loc = reinterpret_cast<float2*>(reinterpret_cast<uint8_t*>(xch) + Cfg::XCH_BYTES);  // [4 cgroups][MAXG][128]
-  float* s_bias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(loc) + Cfg::LOC_BYTES);  // [320]
-  int* s_tcol = reinterpret_cast<int*>(s_bias + BLOCK_N);             // [MAXG][128] absolute target column
-  float* s_coef = reinterpret_cast<float*>(s_tcol + MAXG * BLOCK_M);  // [MAXG][128] w / avg
-  float* s_colsum = s_coef + MAXG * BLOCK_M;                          // [320]
-  float* s_loss = s_colsum + BLOCK_N;                                 // [8]
-  int4* s_meta = reinterpret_cast<int4*>(s_loss + 16);                // [CGROUPS][8] (gA, bpos, gB, hiB) per chunk
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(s_meta) + Cfg::META_BYTES);
+  float2* xch = reinterpret_cast<float2*>(smem + STAGES * Cfg::STAGE_BYTES);          // [4 ranks][MAXG][128]
+  int* s_tcol = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(xch) + Cfg::XCH_BYTES);   // [MAXG][128]
+  float* s_coef = reinterpret_cast<float*>(s_tcol + MAXG * BLOCK_M);                 // [MAXG][128] w / avg
+  float* s_mrow = s_coef + MAXG * BLOCK_M;                                           // [MAXG][128] CTA row max
+  float* s_lse = s_mrow + MAXG * BLOCK_M;                                            // [MAXG][128]
+  float* s_part = s_lse + MAXG * BLOCK_M;                                            // [MAXG][2][256]
+  float* s_bias = s_part + MAXG * 2 * 256;                                           // [320]
+  int* s_colbin = reinterpret_cast<int*>(s_bias + BLOCK_N);                          // [320] bin or -1
+  float* s_colsum = reinterpret_cast<float*>(s_colbin + BLOCK_N);                    // [320]
+  float* s_loss = s_colsum + BLOCK_N;                                                // [16]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_loss + 16);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* bias_bar = bars + 2 * STAGES + 1;
-  uint64_t* xch_bar = bars + 2 * STAGES + 2;   // counts the bytes of the four CTAs' softmax partials landing in xch
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 3);
-  __shared__ int s_gs[kMaxG], s_ge[kMaxG];   // bin start / end, for runtime-indexed access
+  uint64_t* xch_bar = bars + 2 * STAGES;   // counts the bytes of the four CTAs' softmax partials landing in xch
+  __shared__ int s_gs[kMaxG], s_ge[kMaxG];
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
   const uint32_t rank = cluster_ctarank();
   const int row_tile = blockIdx.x / Cfg::CLUSTER;
   const int m0 = row_tile * BLOCK_M;
   const int n0 = static_cast<int>(rank) * BLOCK_N;   // first logit column of this CTA
   const int G = p.gt.G;
-  if (threadIdx.x == 0) { stamp(p.timing, 0); if (p.timing) p.timing[blockIdx.x * 8 + 7] = sm_id(); }
   pdl_trigger();   // dependents guard their own first dependent access with griddepcontrol.wait
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_x);
     tma_prefetch_desc(&tmap_w);
 #pragma unroll
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(tfull_bar, 1);
-    mbar_init(bias_bar, Cfg::EPI_WARPS);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     mbar_init(xch_bar, 1);
     fence_mbar_init();
     // every row of every CTA of the cluster sends one float2 per bin
     mbar_arrive_expect_tx(xch_bar, static_cast<uint32_t>(G) * Cfg::CLUSTER * BLOCK_M * 8u);
   }
-  if (warp == 1) { tmem_alloc(tmem_holder, 512); tmem_relinquish(); }
-  if (threadIdx.x < 8) s_loss[threadIdx.x] = 0.f;
+  if (threadIdx.x < 16) s_loss[threadIdx.x] = 0.f;
   if (threadIdx.x < kMaxG) {
     int gs = 0, ge = 0;
 #pragma unroll
@@ -226,68 +165,23 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     s_gs[threadIdx.x] = gs;
     s_ge[threadIdx.x] = ge;
   }
-  // the bias reaches shared memory while warp 0 issues the first loads and warp 1 allocates tensor memory
-  if (threadIdx.x >= 64) {
-    for (int c = threadIdx.x - 64; c < BLOCK_N; c += Cfg::NUM_THREADS - 64) {
-      s_colsum[c] = 0.f;
-      s_bias[c] = (p.bias != nullptr && n0 + c < p.C) ? __ldg(p.bias + n0 + c) : 0.f;
-    }
+  for (int c = threadIdx.x; c < BLOCK_N; c += Cfg::NUM_THREADS) {
+    const int col = n0 + c;
+    int b = -1;
+#pragma unroll
+    for (int i = 0; i < MAXG; ++i)
+      if (i < G && col < p.C && col >= p.gt.start[i] && col < p.gt.start[i] + p.gt.len[i]) b = i;
+    s_colbin[c] = b;
+    s_colsum[c] = 0.f;
+    s_bias[c] = (p.bias != nullptr && col < p.C) ? __ldg(p.bias + col) : 0.f;
   }
-  tc_fence_before();
-  // CTA-wide setup barrier.  The TMA producer warp only ARRIVES (its barrier initialisation is ordered before the
-  // arrive): it starts loading at once instead of waiting for the bias / tensor-memory setup of the others.
-  if (warp == 0) { __syncwarp(); named_bar_arrive(4, Cfg::NUM_THREADS); }
-  else           named_bar_sync(4, Cfg::NUM_THREADS);
-  tc_fence_after();
+  __syncthreads();
   cluster_arrive();   // phase 1 of the cluster barrier; waited for just before the first remote shared-memory store
-  const uint32_t tmem_base = (warp == 0) ? 0u : *tmem_holder;   // (warp 0 never touches tensor memory)
-  if (threadIdx.x == 32) stamp(p.timing, 1);   // setup done
 
-  // warp-uniform helpers over the bin table -----------------------------------------------------
-  auto bin_of = [&](int col) -> int {   // -1 : not a logit column
-    int g = -1;
-#pragma unroll
-    for (int i = 0; i < MAXG; ++i)
-      if (i < G && col >= p.gt.start[i] && col < p.gt.start[i] + p.gt.len[i]) g = i;
-    return g;
-  };
-  auto bin_end = [&](int g) -> int {
-    int e = 0;
-#pragma unroll
-    for (int i = 0; i < MAXG; ++i)
-      if (i == g) e = p.gt.start[i] + p.gt.len[i];
-    return e;
-  };
-
-  const int ew = warp - 2;                 // epilogue warp index 0..15 (valid when warp >= 2)
-  const int quarter = warp & 3;            // TMEM lane quarter
-  const int cg = (ew >= 0) ? (ew >> 2) : 0;   // column group 0..3
-  const int row_l = quarter * 32 + lane;   // row inside the tile == TMEM lane
-  const int row = m0 + row_l;
-  const int c_cg = cg * Cfg::CG_COLS;      // first TMEM column of this warp's range
-  const int col_lo = n0 + c_cg, col_hi = col_lo + Cfg::CG_COLS;   // global logit columns of this warp
-
-  // (address arithmetic done here, i.e. under the mainloop, by the epilogue warps)
-  const int m_warp = m0 + quarter * 32;
-  // transposed stores: the rows / 16-byte columns this lane writes for every chunk, and whether it may
-  constexpr int ST_ITERS = TF32 ? 4 : 2;            // 16-byte stores per lane and chunk
-  constexpr int ST_ROWS = 32 / ST_ITERS;            // rows covered by one warp-wide store
-  constexpr int ST_CHN = TF32 ? 4 : 2;              // 16-byte pieces per staged row
-  constexpr int ST_ELT = TF32 ? 4 : 2;
-  const int st_r0 = lane / ST_CHN, st_ch = lane % ST_CHN;
-  uint8_t* st_ptr[ST_ITERS];
-  bool st_ok[ST_ITERS];
-#pragma unroll
-  for (int it = 0; it < ST_ITERS; ++it) {
-    const int r = it * ST_ROWS + st_r0;
-    st_ok[it] = p.want_dz && (m_warp + r < p.N) && !(p.dbg & 1);
-    st_ptr[it] = reinterpret_cast<uint8_t*>(p.dz) +
-                 (static_cast<long long>(m_warp + r) * p.ldd + col_lo) * ST_ELT + st_ch * 16;
-  }
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (tid == 0) {
+      // ===================== TMA producer =====================
       for (int kb = 0; kb < p.kblocks; ++kb) {
         const int stage = kb % STAGES;
         const uint32_t phase = static_cast<uint32_t>(kb / STAGES) & 1u;
@@ -298,423 +192,282 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
         uint8_t* sb = smem_b + stage * Cfg::B_BYTES;
         tma_load_2d(sa, &tmap_x, &full_bar[stage], k0, m0);
         tma_load_2d(sb, &tmap_w, &full_bar[stage], k0, n0);
-        tma_load_2d(sb + Cfg::UMMA_N * 128, &tmap_w, &full_bar[stage], k0, n0 + Cfg::UMMA_N);
+        tma_load_2d(sb + HALF_N * 128, &tmap_w, &full_bar[stage], k0, n0 + HALF_N);
       }
+    } else if (tid >= 32) {
+      // ===================== row information (+ clear hook) under the mainloop =====================
+      pdl_wait();   // masks / avg come from the preceding sampler kernel (programmatic dependent launch)
+      const int ht = tid - 32;   // 0..95
+      if (p.clear != nullptr) {   // (a write: only after the wait -- the buffer may still be in use by an earlier kernel)
+        const long long stride = static_cast<long long>(gridDim.x) * 96;
+        const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (long long i = static_cast<long long>(blockIdx.x) * 96 + ht; i < p.clear_vecs; i += stride) p.clear[i] = zero4;
+      }
+      for (int row_l = ht; row_l < BLOCK_M; row_l += 96) {
+        const int row = m0 + row_l;
+        long long lab = 0;
+        if (row < p.N) lab = __ldg(p.labels + row);
+        const bool lab_ok = (row < p.N) && lab >= 0 && lab < p.classes;
+        for (int g = 0; g < G; ++g) {
+          int t = lab_ok ? __ldg(p.l2b + g * p.classes + static_cast<int>(lab)) : 0;
+          t = (t >= 0 && t < s_ge[g] - s_gs[g]) ? t : 0;
+          float w = 0.f;
+          if (row < p.N)
+            w = (p.wmask != nullptr)
+                    ? (WF ? __ldg(reinterpret_cast<const float*>(p.wmask) + static_cast<long long>(g) * p.N + row)
+                          : static_cast<float>(__ldg(p.wmask + static_cast<long long>(g) * p.N + row)))
+                    : 1.0f;
+          const float inv_avg = 1.0f / (p.avg != nullptr ? __ldg(p.avg + g) : fmaxf(static_cast<float>(p.N), 1.0f));
+          s_tcol[g * BLOCK_M + row_l] = s_gs[g] + t;
+          s_coef[g * BLOCK_M + row_l] = w * inv_avg;
+        }
+      }
+      named_bar_arrive(1, 96 + 256);
     }
     __syncwarp();
     cluster_wait();
-  } else if (warp == 1) {
-    // ===================== UMMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_instr_desc(TF32 ? 2u : 1u, false, false, BLOCK_M, Cfg::UMMA_N);
-      int stage = 0;
-      uint32_t phase = 0;
-      mbar_wait(bias_bar, 0);   // the accumulators were preset to the bias by the epilogue warps
-      tc_fence_after();
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        if (kb == 0) stamp(p.timing, 2);   // first operands landed
-        const uint32_t sa = smem_u32(smem_a + stage * Cfg::A_BYTES);
-        const uint32_t sb = smem_u32(smem_b + stage * Cfg::B_BYTES);
+    return;
+  }
+
+  // ===================== consumers: mainloop =====================
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1, ctid = threadIdx.x - 128;
+  const int warp = tid >> 5, lane = tid & 31, q = lane & 3;
+  const int row_l0 = cw * 64 + warp * 16 + (lane >> 2);   // rows row_l0 and row_l0 + 8 of the tile
+  float acc0[80], acc1[80];
 #pragma unroll
-        for (int k = 0; k < Cfg::K_STEPS; ++k) {
-          const uint64_t adesc = make_smem_desc(sa + k * 32, 16, 1024);
+  for (int j = 0; j < HALF_N / 8; ++j) {
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            const uint64_t bdesc = make_smem_desc(sb + h * Cfg::UMMA_N * 128 + k * 32, 16, 1024);
-            if (TF32) umma_tf32(tmem_base + h * Cfg::UMMA_N, adesc, bdesc, idesc, 1u);
-            else      umma_bf16(tmem_base + h * Cfg::UMMA_N, adesc, bdesc, idesc, 1u);
-          }
-        }
-        umma_commit(&empty_bar[stage]);
-        if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-      }
-      umma_commit(tfull_bar);
+    for (int e = 0; e < 2; ++e) {
+      const float b0 = s_bias[8 * j + 2 * q + e], b1 = s_bias[HALF_N + 8 * j + 2 * q + e];
+      acc0[4 * j + e] = b0; acc0[4 * j + 2 + e] = b0;
+      acc1[4 * j + e] = b1; acc1[4 * j + 2 + e] = b1;
     }
-    __syncwarp();
-    cluster_wait();
-  } else {
-    // ===================== epilogue, part 0: accumulators := bias, chunk table ===================
-    const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + c_cg;
-    {
-#pragma unroll 1
-      for (int ci = 0; ci < Cfg::CHUNKS; ++ci) {
-        uint32_t bv[CH];
+  }
+  {
+    const uint32_t a_off = cw * 8192;   // this warpgroup's 64 rows of the A tile
+    for (int kb = 0; kb < p.kblocks; ++kb) {
+      const int stage = kb % STAGES;
+      mbar_wait(&full_bar[stage], static_cast<uint32_t>(kb / STAGES) & 1u);
+      const uint32_t sa = smem_u32(smem_a + stage * Cfg::A_BYTES) + a_off;
+      const uint32_t sb = smem_u32(smem_b + stage * Cfg::B_BYTES);
+      fence_regs(acc0);
+      fence_regs(acc1);
+      wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < CH; j += 4) {
-          const float4 b4 = *reinterpret_cast<const float4*>(&s_bias[c_cg + ci * CH + j]);
-          bv[j + 0] = __float_as_uint(b4.x); bv[j + 1] = __float_as_uint(b4.y);
-          bv[j + 2] = __float_as_uint(b4.z); bv[j + 3] = __float_as_uint(b4.w);
-        }
-        tmem_st_32x32b_x16(t_row + ci * CH, bv);
+      for (int k = 0; k < Cfg::K_STEPS; ++k) {
+        const uint64_t adesc = make_smem_desc(sa + k * 32, 16, 1024);
+        const uint64_t bdesc0 = make_smem_desc(sb + k * 32, 16, 1024);
+        const uint64_t bdesc1 = make_smem_desc(sb + HALF_N * 128 + k * 32, 16, 1024);
+        if (TF32) { wgmma_tf32_n160(acc0, adesc, bdesc0, 1u); wgmma_tf32_n160(acc1, adesc, bdesc1, 1u); }
+        else      { wgmma_bf16_n160<0, 0>(acc0, adesc, bdesc0, 1u); wgmma_bf16_n160<0, 0>(acc1, adesc, bdesc1, 1u); }
       }
-      tmem_st_wait();
-      tc_fence_before();
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(acc0);
+      fence_regs(acc1);
       __syncwarp();
-      if (lane == 0) mbar_arrive(bias_bar);
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
     }
-    // per-chunk bin layout of this warp's 80 columns (warp-uniform): columns [0,bpos) of the chunk belong to
-    // bin gA, [bpos,hiB) to bin gB (or to no bin); gA = -1 marks a chunk beyond the last logit column
-    if (lane < Cfg::CHUNKS) {
-      const int col0 = col_lo + lane * CH;
-      int gA = -1, bpos = 0, gB = -1, hiB = 0;
-      if (col0 < p.C) {
-        gA = bin_of(col0);
-        const int endA = bin_end(gA);
-        bpos = (endA - col0 < CH) ? (endA - col0) : CH;
-        hiB = bpos;
-        if (bpos < CH) {
-          gB = bin_of(col0 + bpos);
-          if (gB >= 0) { const int endB = bin_end(gB); hiB = (endB - col0 < CH) ? (endB - col0) : CH; }
+  }
+  pdl_wait();   // every global write below comes after the predecessor grid
+
+  // walk the thread's 160 elements of row slot rr in column order: f(z, local column)
+#define BAGS_WALK(rr, F)                                                                           \
+  do {                                                                                             \
+    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) {                                       \
+      _Pragma("unroll") for (int e = 0; e < 2; ++e) F(acc0[4 * j + 2 * (rr) + e], 8 * j + 2 * q + e); \
+    }                                                                                              \
+    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) {                                       \
+      _Pragma("unroll") for (int e = 0; e < 2; ++e) F(acc1[4 * j + 2 * (rr) + e], HALF_N + 8 * j + 2 * q + e); \
+    }                                                                                              \
+  } while (0)
+
+  float mrow[2][MAXG], srow[2][MAXG];
+#pragma unroll
+  for (int rr = 0; rr < 2; ++rr) {
+    const int row_l = row_l0 + 8 * rr;
+    // ---- pass A: per-bin max over this thread's columns, then over the quad ----
+#pragma unroll
+    for (int g = 0; g < MAXG; ++g) s_part[(g * 2 + rr) * 256 + ctid] = -INFINITY;
+    {
+      int gc = -1;
+      float mc = -INFINITY;
+      auto stepA = [&](float z, int c) {
+        const int b = s_colbin[c];
+        if (b != gc) {
+          if (gc >= 0) s_part[(gc * 2 + rr) * 256 + ctid] = mc;
+          gc = b; mc = -INFINITY;
         }
-      }
-      s_meta[cg * 8 + lane] = make_int4(gA, bpos, gB, hiB);   // the 4 quarters write identical values
+        mc = fmaxf(mc, z);
+      };
+      BAGS_WALK(rr, stepA);
+      if (gc >= 0) s_part[(gc * 2 + rr) * 256 + ctid] = mc;
+    }
+#pragma unroll
+    for (int g = 0; g < MAXG; ++g) {
+      float m = s_part[(g * 2 + rr) * 256 + ctid];
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+      mrow[rr][g] = m;
+      if (q == 0 && g < G) s_mrow[g * BLOCK_M + row_l] = m;
     }
     __syncwarp();
-
-    // ===================== epilogue, part 1: row info (overlaps the mainloop) + pass A ==========
-    pdl_wait();   // masks / avg come from the preceding sampler kernel (programmatic dependent launch)
-    if (p.clear != nullptr) {   // (a write: only after the wait -- the buffer may still be in use by an earlier kernel)
-      const long long stride = static_cast<long long>(gridDim.x) * (32 * Cfg::EPI_WARPS);
-      const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (long long i = static_cast<long long>(blockIdx.x) * (32 * Cfg::EPI_WARPS) + (threadIdx.x - 64); i < p.clear_vecs; i += stride)
-        p.clear[i] = zero4;
-    }
-    if (cg == 0) {
-      long long lab = 0;
-      if (row < p.N) lab = __ldg(p.labels + row);
-      const bool lab_ok = (row < p.N) && lab >= 0 && lab < p.classes;
-      for (int g = 0; g < G; ++g) {
-        int t = lab_ok ? __ldg(p.l2b + g * p.classes + static_cast<int>(lab)) : 0;
-        t = (t >= 0 && t < s_ge[g] - s_gs[g]) ? t : 0;
-        float w = 0.f;
-        if (row < p.N)
-          w = (p.wmask != nullptr)
-                  ? (WF ? __ldg(reinterpret_cast<const float*>(p.wmask) + static_cast<long long>(g) * p.N + row)
-                        : static_cast<float>(__ldg(p.wmask + static_cast<long long>(g) * p.N + row)))
-                  : 1.0f;
-        const float inv_avg = 1.0f / (p.avg != nullptr ? __ldg(p.avg + g) : fmaxf(static_cast<float>(p.N), 1.0f));
-        s_tcol[g * BLOCK_M + row_l] = s_gs[g] + t;
-        s_coef[g * BLOCK_M + row_l] = w * inv_avg;
-      }
-    }
-    // bins this warp does not touch contribute the identity (-inf, 0) to the CTA-local combine
-    for (int g = 0; g < G; ++g)
-      if (s_ge[g] <= col_lo || s_gs[g] >= col_hi) loc[(cg * MAXG + g) * BLOCK_M + row_l] = make_float2(-INFINITY, 0.f);
-
-    named_bar_sync(1, 32 * Cfg::EPI_WARPS);   // s_tcol / s_coef (written by the cg == 0 warps) are visible
-
-    mbar_wait(tfull_bar, 0);
-    tc_fence_after();
-    if (warp == 2 && lane == 0) stamp(p.timing, 3);   // accumulators complete
-    float2* refs = reinterpret_cast<float2*>(smem + Cfg::REF_OFFSET) + (threadIdx.x - 64);   // [chunk][512 threads]
-    float* s_zt = reinterpret_cast<float*>(smem + Cfg::ZT_OFFSET);
+    // ---- pass B: per-bin sum of exp(z - max) ----
+#pragma unroll
+    for (int g = 0; g < MAXG; ++g) s_part[(g * 2 + rr) * 256 + ctid] = 0.f;
     {
-      int g_cur = -2;
-      int tcol_a = -(1 << 30);
-      float m_cur = -INFINITY, s_cur = 0.f;
-      // the logit of the row's target column of bin g, for the loss: saved when this warp walks past it
-      // (most chunks hold no row's target: "others" targets sit in each bin's first column)
-      auto capture = [&](int g, int tcol, const float (&zz)[CH], int col0) {
-        const unsigned tq = static_cast<unsigned>(tcol - col0);
-        if (__any_sync(0xffffffffu, tq < static_cast<unsigned>(CH))) {
-          float zt = 0.f;
-#pragma unroll
-          for (int j = 0; j < CH; ++j) zt = (static_cast<unsigned>(j) == tq) ? zz[j] : zt;
-          if (tq < static_cast<unsigned>(CH)) s_zt[g * BLOCK_M + row_l] = zt;
+      int gc = -1;
+      float mb = 0.f, sc = 0.f;
+      auto stepB = [&](float z, int c) {
+        const int b = s_colbin[c];
+        if (b != gc) {
+          if (gc >= 0) s_part[(gc * 2 + rr) * 256 + ctid] = sc;
+          gc = b; sc = 0.f;
+          mb = (b >= 0) ? s_mrow[b * BLOCK_M + row_l] * kLog2e : 0.f;
         }
+        if (b >= 0) sc += exp2f(fmaf(z, kLog2e, -mb));
       };
-      auto flush = [&]() {
-        if (g_cur >= 0) loc[(cg * MAXG + g_cur) * BLOCK_M + row_l] = make_float2(m_cur, s_cur);
-      };
-      uint32_t v[CH];
-#ifdef BAGS_X_NOTMEMLD
-      for (int j = 0; j < CH; ++j) v[j] = __float_as_uint(0.01f * (lane + j));
-#endif
-      if (col_lo < p.C) BAGS_TMEM_LD16(t_row, v);   // software pipeline: chunk ci+1 is in flight
-#pragma unroll 1                                           // while chunk ci is reduced
-      for (int ci = 0; ci < Cfg::CHUNKS; ++ci) {
-        const int4 md = s_meta[cg * 8 + ci];
-        if (md.x < 0) break;
-        tmem_ld_wait();
-        float z[CH];   // aliases v: the next chunk's load is issued only after the last use of z
-#pragma unroll
-        for (int j = 0; j < CH; ++j) z[j] = __uint_as_float(v[j]);
-        if (md.x != g_cur) {
-          flush();
-          g_cur = md.x; m_cur = -INFINITY; s_cur = 0.f;
-          tcol_a = s_tcol[g_cur * BLOCK_M + row_l];
-        }
-        capture(g_cur, tcol_a, z, col_lo + ci * CH);
-        uint32_t e[CH];
-        float refA, refB = 0.f;
-        if (md.y >= CH) {
-          // fast path: the whole chunk is one bin
-          float c4[4] = {z[0], z[1], z[2], z[3]};
-#pragma unroll
-          for (int j = 4; j < CH; ++j) c4[j & 3] = fmaxf(c4[j & 3], z[j]);
-          const float cm = fmaxf(fmaxf(c4[0], c4[1]), fmaxf(c4[2], c4[3]));
-          const float m_new = fmaxf(m_cur, cm);
-          const float mb = m_new * kLog2e;
-          const float2 k2 = make_float2(kLog2e, kLog2e), nb2 = make_float2(-mb, -mb);
-          float2 a2[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-#pragma unroll
-          for (int j = 0; j < CH; j += 2) {   // packed f32x2 FMA / ADD: half the issue slots
-            const float2 t = __ffma2_rn(make_float2(z[j], z[j + 1]), k2, nb2);
-            const float2 ej = make_float2(fast_exp2(t.x), fast_exp2(t.y));
-            a2[(j >> 1) & 1] = __fadd2_rn(a2[(j >> 1) & 1], ej);
-            e[j] = __float_as_uint(ej.x);
-            e[j + 1] = __float_as_uint(ej.y);
-          }
-          const float2 a1 = __fadd2_rn(a2[0], a2[1]);
-          const float acc = a1.x + a1.y;
-          s_cur = s_cur * fast_exp2((m_cur - m_new) * kLog2e) + acc;   // 2^-inf = 0 on the first chunk of a bin
-          m_cur = m_new;
-          refA = m_new;
-        } else {
-          // two segments: [0,bpos) continues bin gA, [bpos,hiB) opens bin gB.  Branch-free (selects): this chunk
-          // sits on the critical path of its CTA's pass A
-          const int bpos = md.y, hiB = md.w;
-          float cmA = -INFINITY, cmB = -INFINITY;
-#pragma unroll
-          for (int j = 0; j < CH; ++j) {
-            const bool a = j < bpos, b = (j >= bpos) && (j < hiB);
-            cmA = fmaxf(cmA, a ? z[j] : -INFINITY);
-            cmB = fmaxf(cmB, b ? z[j] : -INFINITY);
-          }
-          const float m_newA = fmaxf(m_cur, cmA);
-          const float mbA = m_newA * kLog2e, mbB = cmB * kLog2e;   // mbB = -inf without a second bin: selected away
-          float accA = 0.f, accB = 0.f;
-#pragma unroll
-          for (int j = 0; j < CH; ++j) {
-            const bool a = j < bpos, b = (j >= bpos) && (j < hiB);
-            float ej = fast_exp2(fmaf(z[j], kLog2e, a ? -mbA : -mbB));
-            ej = (a || b) ? ej : 0.f;
-            accA += a ? ej : 0.f;
-            accB += b ? ej : 0.f;
-            e[j] = __float_as_uint(ej);
-          }
-          s_cur = s_cur * fast_exp2((m_cur - m_newA) * kLog2e) + accA;
-          m_cur = m_newA;
-          flush();
-          g_cur = md.z; m_cur = cmB; s_cur = accB;
-          refA = m_newA; refB = cmB;
-          if (g_cur >= 0) {
-            tcol_a = s_tcol[g_cur * BLOCK_M + row_l];
-            capture(g_cur, tcol_a, z, col_lo + ci * CH);
-          }
-        }
-        if (ci + 1 < Cfg::CHUNKS && col_lo + (ci + 1) * CH < p.C) BAGS_TMEM_LD16(t_row + (ci + 1) * CH, v);
-        BAGS_TMEM_ST16(t_row + ci * CH, e);
-        refs[ci * (32 * Cfg::EPI_WARPS)] = make_float2(refA, refB);
-      }
-      if (warp == 2 && lane == 0) stamp2(p.timing, 0);    // chunk loop of pass A done (this warp)
-      if (warp == 17 && lane == 0) stamp2(p.timing, 6);
-      flush();
-      tmem_st_wait();
+      BAGS_WALK(rr, stepB);
+      if (gc >= 0) s_part[(gc * 2 + rr) * 256 + ctid] = sc;
     }
-    // ---- CTA-local combine of the 4 column groups, then publish to the 4 CTAs of the cluster ----
-    // (bins are dealt round-robin to the column groups so that all 16 warps share the work)
-    named_bar_sync(1, 32 * Cfg::EPI_WARPS);
-    cluster_wait();   // (phase 1, arrived during setup) every CTA of the cluster is running: remote smem is live
-    if (warp == 2 && lane == 0) stamp2(p.timing, 1);      // all 16 warps done with pass A
-    for (int g = cg; g < G; g += Cfg::CGROUPS) {
-      float2 q[Cfg::CGROUPS];
 #pragma unroll
-      for (int i = 0; i < Cfg::CGROUPS; ++i) q[i] = loc[(i * MAXG + g) * BLOCK_M + row_l];
-      const float M = fmaxf(fmaxf(q[0].x, q[1].x), fmaxf(q[2].x, q[3].x));
-      float S = 0.f;
-#pragma unroll
-      for (int i = 0; i < Cfg::CGROUPS; ++i) S += (q[i].x == -INFINITY) ? 0.f : q[i].y * fast_exp2((q[i].x - M) * kLog2e);
-      const uint32_t addr = smem_u32(&xch[(static_cast<int>(rank) * MAXG + g) * BLOCK_M + row_l]);
-      const uint32_t baddr = smem_u32(xch_bar);
-#pragma unroll
-      for (uint32_t r = 0; r < 4; ++r) st_async_cluster_f2(addr, baddr, r, M, S);
+    for (int g = 0; g < MAXG; ++g) {
+      float s = s_part[(g * 2 + rr) * 256 + ctid];
+      s += __shfl_xor_sync(0xffffffffu, s, 1);
+      s += __shfl_xor_sync(0xffffffffu, s, 2);
+      srow[rr][g] = s;
     }
   }
 
-  if (warp == 2 && lane == 0) stamp(p.timing, 4);   // pass A done
-
-  if (warp >= 2) {
-    // all partials of all four CTAs have landed once the transaction count of xch_bar is reached; nobody leaves
-    // before that, so no CTA exits while a peer still writes into its shared memory
-    mbar_wait(xch_bar, 0);
-    if (warp == 2 && lane == 0) stamp(p.timing, 5);   // exchange complete
-  }
-
-  if (warp >= 2) {
-    // ===================== epilogue, part 2: combine + pass C =====================================
-    const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + c_cg;
-    uint8_t* buf = smem + ew * Cfg::DZ_BUF_BYTES;   // aliases the (now idle) pipeline stages
-    const float2* refs = reinterpret_cast<const float2*>(smem + Cfg::REF_OFFSET) + (threadIdx.x - 64);
-    tc_fence_after();
-
-    int g_cur = -2;
-    float lb_cur = 0.f, coef_cur = 0.f;
-    int tcol_cur = -1;
-    const float* s_zt = reinterpret_cast<const float*>(smem + Cfg::ZT_OFFSET);
-    // last bin this warp's columns reach: once its loss terms are in, the warp reports to the bookkeeping warp
-    const int g_last = (col_lo < p.C) ? bin_of(((col_hi < p.C) ? col_hi : p.C) - 1) : -1;
-    if (g_last < 0) named_bar_arrive(6, 32 * Cfg::EPI_WARPS + 32);
-    auto start_bin = [&](int g) {
-      g_cur = g;
-      if (g < 0) { lb_cur = 0.f; coef_cur = 0.f; tcol_cur = -1; return; }
-      float2 q[Cfg::CLUSTER];
+  // ---- exchange: publish (max, sum) of every (row, bin) to the four CTAs of the cluster ----
+  cluster_wait();   // (phase 1, arrived during setup) every CTA of the cluster is running: remote smem is live
+  if (q == 0) {
+    const uint32_t baddr = smem_u32(xch_bar);
 #pragma unroll
-      for (int s = 0; s < Cfg::CLUSTER; ++s) q[s] = xch[(s * MAXG + g) * BLOCK_M + row_l];
-      const float M = fmaxf(fmaxf(q[0].x, q[1].x), fmaxf(q[2].x, q[3].x));
-      float S = 0.f;
+    for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
-      for (int s = 0; s < Cfg::CLUSTER; ++s) S += (q[s].x == -INFINITY) ? 0.f : q[s].y * fast_exp2((q[s].x - M) * kLog2e);
-      const float lse_v = M + logf(S);
-      lb_cur = lse_v * kLog2e;
-      coef_cur = s_coef[g * BLOCK_M + row_l];
-      tcol_cur = s_tcol[g * BLOCK_M + row_l];
-      // loss of the bin: rows whose target column lies in this warp's range (its logit was saved in pass A);
-      // one shared-memory atomic per warp instead of 32 contending CAS loops
-      const bool own = (tcol_cur >= col_lo && tcol_cur < col_hi);
-      float term = own ? coef_cur * (lse_v - s_zt[g * BLOCK_M + row_l]) : 0.f;
-      term = warp_sum(term);
-      if (lane == 0) atomicAdd(&s_loss[g], term);
-      if (p.lse != nullptr && row < p.N && s_gs[g] >= col_lo && s_gs[g] < col_hi)
-        p.lse[static_cast<long long>(row) * G + g] = lse_v;
-      if (g == g_last) { __syncwarp(); named_bar_arrive(6, 32 * Cfg::EPI_WARPS + 32); }
-    };
-
-    uint32_t v[CH];
-#ifdef BAGS_X_NOTMEMLD
-    for (int j = 0; j < CH; ++j) v[j] = __float_as_uint(0.01f * (lane + j));
-#endif
-    if (col_lo < p.C) BAGS_TMEM_LD16(t_row, v);
-    if (warp == 2 && lane == 0) stamp2(p.timing, 2);      // pass C starts
-#pragma unroll 1
-    for (int ci = 0; ci < Cfg::CHUNKS; ++ci) {
-      const int4 md = s_meta[cg * 8 + ci];
-      if (md.x < 0) break;
-      const int col0 = col_lo + ci * CH;
-      const float2 rf = refs[ci * (32 * Cfg::EPI_WARPS)];
-      tmem_ld_wait();
-      float d[CH];   // aliases v (e = exp(z - m_chunk) from pass A) until the scaling below
+      for (int g = 0; g < MAXG; ++g) {
+        if (g >= G) break;
+        const uint32_t addr = smem_u32(&xch[(static_cast<int>(rank) * MAXG + g) * BLOCK_M + row_l0 + 8 * rr]);
 #pragma unroll
-      for (int j = 0; j < CH; ++j) d[j] = __uint_as_float(v[j]);
-      if (md.x != g_cur) start_bin(md.x);
-      if (warp == 2 && lane == 0 && ci == 0) stamp_bank(p.timing, 2, 6);
-      if (md.y >= CH) {
-        const float f = fast_exp2(fmaf(rf.x, kLog2e, -lb_cur));   // exp(m_chunk - lse)
-        const float gf = coef_cur * f;
-        const int tq = tcol_cur - col0;
-        // most chunks contain no row's target column ("others" targets sit in each bin's first column):
-        // a warp vote selects the loop without the per-element one-hot handling
-        if (__any_sync(0xffffffffu, tq >= 0 && tq < CH)) {
-#pragma unroll
-          for (int j = 0; j < CH; ++j) {
-            float dj = d[j] * gf;
-            if (j == tq) dj -= coef_cur;
-            d[j] = dj;
-          }
-        } else {
-          const float2 g2 = make_float2(gf, gf);
-#pragma unroll
-          for (int j = 0; j < CH; j += 2) {
-            const float2 r = __fmul2_rn(make_float2(d[j], d[j + 1]), g2);
-            d[j] = r.x;
-            d[j + 1] = r.y;
-          }
-        }
-      } else {
-        // branch-free: e is already zero beyond hiB, so a per-element select of the bin's scale is all it takes
-        const int bpos = md.y;
-        const float fA = fast_exp2(fmaf(rf.x, kLog2e, -lb_cur));
-        const float gfA = coef_cur * fA, coefA = coef_cur;
-        const int tqA = tcol_cur - col0;          // target column of bin A relative to the chunk (maybe outside)
-        start_bin(md.z);
-        const float fB = (md.z >= 0) ? fast_exp2(fmaf(rf.y, kLog2e, -lb_cur)) : 0.f;
-        const float gfB = coef_cur * fB, coefB = coef_cur;
-        const int tqB = tcol_cur - col0;
-#pragma unroll
-        for (int j = 0; j < CH; ++j) {
-          const bool a = j < bpos;
-          float dj = d[j] * (a ? gfA : gfB);
-          if (j == tqA && a) dj -= coefA;
-          if (j == tqB && !a) dj -= coefB;
-          d[j] = dj;
-        }
+        for (uint32_t r = 0; r < 4; ++r) st_async_cluster_f2(addr, baddr, r, mrow[rr][g], srow[rr][g]);
       }
-      // the e values are consumed: the next chunk's TMEM load overlaps the pack / stage / store phase
-      if (ci + 1 < Cfg::CHUNKS && col0 + CH < p.C) BAGS_TMEM_LD16(t_row + (ci + 1) * CH, v);
-      if (p.want_dz) {
-        // stage the 32-row x 16-column tile in (swizzled) shared memory, read it back transposed so that each
-        // warp-wide 16-byte store writes whole 32-byte (bf16) / 64-byte (fp32) row segments
-        if (TF32) {
-          uint4* rowp = reinterpret_cast<uint4*>(buf + lane * 64);
+  }
+  // all partials of all four CTAs have landed once the transaction count of xch_bar is reached; nobody leaves
+  // before that, so no CTA exits while a peer still writes into its shared memory
+  mbar_wait(xch_bar, 0);
+  if (q == 0) {
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float4 r = make_float4(d[4 * j], d[4 * j + 1], d[4 * j + 2], d[4 * j + 3]);
-            rowp[j ^ ((lane >> 1) & 3)] = *reinterpret_cast<uint4*>(&r);
-          }
-          __syncwarp();
+    for (int rr = 0; rr < 2; ++rr) {
+      const int row_l = row_l0 + 8 * rr, row = m0 + row_l;
+      for (int g = 0; g < G; ++g) {
+        float2 v[Cfg::CLUSTER];
 #pragma unroll
-          for (int it = 0; it < ST_ITERS; ++it) {
-            const int r = it * ST_ROWS + st_r0;
-            const uint4 val = *reinterpret_cast<const uint4*>(buf + r * 64 + ((st_ch ^ ((r >> 1) & 3)) << 4));
-            if (st_ok[it]) *reinterpret_cast<uint4*>(st_ptr[it] + ci * (CH * ST_ELT)) = val;
-          }
-        } else {
-          uint4* rowp = reinterpret_cast<uint4*>(buf + lane * 32);
+        for (int s = 0; s < Cfg::CLUSTER; ++s) v[s] = xch[(s * MAXG + g) * BLOCK_M + row_l];
+        const float M = fmaxf(fmaxf(v[0].x, v[1].x), fmaxf(v[2].x, v[3].x));
+        float S = 0.f;
 #pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            uint4 r;
-            r.x = pack_bf16x2(d[8 * j + 0], d[8 * j + 1]); r.y = pack_bf16x2(d[8 * j + 2], d[8 * j + 3]);
-            r.z = pack_bf16x2(d[8 * j + 4], d[8 * j + 5]); r.w = pack_bf16x2(d[8 * j + 6], d[8 * j + 7]);
-            rowp[j ^ ((lane >> 2) & 1)] = r;
-          }
-          __syncwarp();
+        for (int s = 0; s < Cfg::CLUSTER; ++s) S += (v[s].x == -INFINITY) ? 0.f : v[s].y * exp2f((v[s].x - M) * kLog2e);
+        const float lse_v = M + logf(S);
+        s_lse[g * BLOCK_M + row_l] = lse_v;
+        if (p.lse != nullptr && row < p.N && s_gs[g] >= n0 && s_gs[g] < n0 + BLOCK_N)
+          p.lse[static_cast<long long>(row) * G + g] = lse_v;
+      }
+    }
+  }
+  named_bar_sync(1, 96 + 256);   // s_tcol / s_coef from the producer warpgroup; s_lse of the quads
+  // ---- pass C: dz, loss, column sums ----
+  {
+    const bool f32 = TF32;
+    const bool want_cs = p.colsum != nullptr && p.want_dz;
+    int gc = -1;
+    float lb[2] = {0.f, 0.f}, cf[2] = {0.f, 0.f};
+    int tc[2] = {-1, -1};
+    uint8_t* dzrow[2];
+    bool row_ok[2];
 #pragma unroll
-          for (int it = 0; it < ST_ITERS; ++it) {
-            const int r = it * ST_ROWS + st_r0;
-            const uint4 val = *reinterpret_cast<const uint4*>(buf + r * 32 + ((st_ch ^ ((r >> 2) & 1)) << 4));
-            if (st_ok[it]) *reinterpret_cast<uint4*>(st_ptr[it] + ci * (CH * ST_ELT)) = val;
-          }
-        }
-        // optional bias-gradient column sums from the staged tile: lanes l and l+16 share column l % 16
-        if (p.colsum != nullptr && !(p.dbg & 4)) {
-          const int cc = lane & 15, rbase = (lane >> 4) * 16;
-          float cs = 0.f;
+    for (int rr = 0; rr < 2; ++rr) {
+      const int row = m0 + row_l0 + 8 * rr;
+      row_ok[rr] = p.want_dz && row < p.N;
+      dzrow[rr] = reinterpret_cast<uint8_t*>(p.dz) + static_cast<long long>(row) * p.ldd * (f32 ? 4 : 2);
+    }
+    auto stepC = [&](float z0a, float z0b, float z1a, float z1b, int c) {   // rows 0/1 x columns c, c + 1
+      float d[2][2];
+      const float zz[2][2] = {{z0a, z0b}, {z1a, z1b}};
 #pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const int r = rbase + i;
-            if (TF32) {
-              cs += *reinterpret_cast<const float*>(buf + r * 64 + (((cc >> 2) ^ ((r >> 1) & 3)) << 4) + (cc & 3) * 4);
-            } else {
-              const unsigned short h = *reinterpret_cast<const unsigned short*>(buf + r * 32 + (((cc >> 3) ^ ((r >> 2) & 1)) << 4) + (cc & 7) * 2);
-              cs += __uint_as_float(static_cast<uint32_t>(h) << 16);
+      for (int e = 0; e < 2; ++e) {
+        const int b = s_colbin[c + e];
+        if (b != gc) {
+          gc = b;
+          if (b >= 0) {
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+              lb[rr] = s_lse[b * BLOCK_M + row_l0 + 8 * rr];
+              cf[rr] = s_coef[b * BLOCK_M + row_l0 + 8 * rr];
+              tc[rr] = s_tcol[b * BLOCK_M + row_l0 + 8 * rr];
             }
           }
-          cs += __shfl_xor_sync(0xffffffffu, cs, 16);
-          if (lane < 16) atomicAdd(&s_colsum[c_cg + ci * CH + lane], cs);   // 4 quarters share a column
         }
-        __syncwarp();
+        const int col = n0 + c + e;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          float v = 0.f;
+          if (b >= 0) {
+            const float z = zz[rr][e];
+            v = exp2f((z - lb[rr]) * kLog2e) * cf[rr];
+            if (col == tc[rr]) {
+              v -= cf[rr];
+              if (cf[rr] != 0.f) atomicAdd(&s_loss[b], cf[rr] * (lb[rr] - z));
+            }
+          }
+          d[rr][e] = v;
+        }
       }
-      if (warp == 2 && lane == 0) stamp_bank(p.timing, 2, ci);
-    }
-    if (warp == 2 && lane == 0) stamp2(p.timing, 3);      // chunk loop of pass C done (this warp)
-    if (warp == 17 && lane == 0) stamp2(p.timing, 7);
-    if (warp == 2 && lane == 0) stamp(p.timing, 6);   // pass C done
-    tc_fence_before();
-    named_bar_arrive(2, 32 * Cfg::EPI_WARPS + 32);   // this warp is done with TMEM (warp 1 deallocates)
+      const int col = n0 + c;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        if (!f32) {   // the stored (rounded) values feed the column sums
+          d[rr][0] = __bfloat162float(__float2bfloat16_rn(d[rr][0]));
+          d[rr][1] = __bfloat162float(__float2bfloat16_rn(d[rr][1]));
+        }
+        if (row_ok[rr] && col < p.C) {
+          if (col + 1 < p.C) {
+            if (f32) *reinterpret_cast<float2*>(dzrow[rr] + col * 4) = make_float2(d[rr][0], d[rr][1]);
+            else     *reinterpret_cast<uint32_t*>(dzrow[rr] + col * 2) = pack_bf16x2(d[rr][0], d[rr][1]);
+          } else {
+            if (f32) *reinterpret_cast<float*>(dzrow[rr] + col * 4) = d[rr][0];
+            else     *reinterpret_cast<__nv_bfloat16*>(dzrow[rr] + col * 2) = __float2bfloat16_rn(d[rr][0]);
+          }
+        }
+      }
+      if (want_cs) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float cs = d[0][e] + d[1][e];
+          cs += __shfl_xor_sync(0xffffffffu, cs, 4);
+          cs += __shfl_xor_sync(0xffffffffu, cs, 8);
+          cs += __shfl_xor_sync(0xffffffffu, cs, 16);
+          if (lane < 4) atomicAdd(&s_colsum[c + e], cs);
+        }
+      }
+    };
+#pragma unroll
+    for (int j = 0; j < HALF_N / 8; ++j)
+      stepC(acc0[4 * j], acc0[4 * j + 1], acc0[4 * j + 2], acc0[4 * j + 3], 8 * j + 2 * q);
+#pragma unroll
+    for (int j = 0; j < HALF_N / 8; ++j)
+      stepC(acc1[4 * j], acc1[4 * j + 1], acc1[4 * j + 2], acc1[4 * j + 3], HALF_N + 8 * j + 2 * q);
+  }
+#undef BAGS_WALK
+  named_bar_sync(2, 256);   // s_loss / s_colsum complete
 
-    if (p.colsum != nullptr && p.want_dz) {   // optional per-row-tile bias-gradient partials
-      named_bar_sync(3, 32 * Cfg::EPI_WARPS);
-      const int et = threadIdx.x - 64;   // 0..511
-      for (int c = et; c < BLOCK_N; c += 32 * Cfg::EPI_WARPS)
-        if (n0 + c < p.C) p.colsum[static_cast<long long>(row_tile) * p.C + n0 + c] = s_colsum[c];
-    }
-  } else if (warp == 1) {
-    // ---- loss bookkeeping by the (idle) MMA warp, overlapped with pass C: every epilogue warp reports as soon
-    // as the loss terms of its last bin are in shared memory ----
-    named_bar_sync(6, 32 * Cfg::EPI_WARPS + 32);
-    if (lane == 0) stamp2(p.timing, 4);                   // s_loss final
+  if (p.colsum != nullptr && p.want_dz) {   // optional per-row-tile bias-gradient partials
+    for (int c = ctid; c < BLOCK_N; c += 256)
+      if (n0 + c < p.C) p.colsum[static_cast<long long>(row_tile) * p.C + n0 + c] = s_colsum[c];
+  }
+  if (ctid < 32) {
+    // ---- loss bookkeeping: per-CTA partials, the last CTA of the grid sums them in a fixed order ----
     unsigned int last = 0;
     if (lane == 0) {
       float4* dst = reinterpret_cast<float4*>(p.part + static_cast<size_t>(blockIdx.x) * kMaxG);
@@ -723,28 +476,24 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
       last = (atom_add_release_gpu(p.counter, 1u) == gridDim.x - 1) ? 1u : 0u;   // release: the partials first
     }
     last = __shfl_sync(0xffffffffu, last, 0);
-    if (last) {   // the last CTA of the grid sums the per-CTA partials in a fixed order
+    if (last) {
       __threadfence();
-      float acc[kMaxG];
+      float accl[kMaxG];
 #pragma unroll
-      for (int g = 0; g < kMaxG; ++g) acc[g] = 0.f;
+      for (int g = 0; g < kMaxG; ++g) accl[g] = 0.f;
       for (int b = lane; b < static_cast<int>(gridDim.x); b += 32) {
         const float4* src = reinterpret_cast<const float4*>(p.part + static_cast<size_t>(b) * kMaxG);
         const float4 u = __ldcg(src), w = __ldcg(src + 1);
-        acc[0] += u.x; acc[1] += u.y; acc[2] += u.z; acc[3] += u.w;
-        acc[4] += w.x; acc[5] += w.y; acc[6] += w.z; acc[7] += w.w;
+        accl[0] += u.x; accl[1] += u.y; accl[2] += u.z; accl[3] += u.w;
+        accl[4] += w.x; accl[5] += w.y; accl[6] += w.z; accl[7] += w.w;
       }
 #pragma unroll
       for (int g = 0; g < kMaxG; ++g) {
-        const float t = warp_sum(acc[g]);
+        const float t = warp_sum(accl[g]);
         if (lane == 0 && g < G) p.loss[g] = t;   // already divided by avg (coef = w/avg)
       }
       if (lane == 0) *p.counter = 0u;
     }
-    if (lane == 0) stamp2(p.timing, 5);                   // bookkeeping done
-    named_bar_sync(2, 32 * Cfg::EPI_WARPS + 32);          // every epilogue warp has finished reading TMEM
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 

@@ -1,6 +1,6 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// Persistent, warp-specialised wgmma GEMM for sm_90a.
 //
-//   D[M,N] (+)= A[M,K] * B[N,K]^T       fp32 accumulation in TMEM
+//   D[M,N] (+)= A[M,K] * B[N,K]^T       fp32 accumulation in registers
 //
 // A and B are each either "K-major" (contraction index contiguous in HBM, i.e.
 // a row-major [rows,K] matrix) or "MN-major" (row-major [K,rows]: contraction
@@ -11,15 +11,18 @@
 //   backward dX = dz W    : A = dz  [N_roi,C]  K-major , B = W   [C,K]      MN-major
 //   backward dW = dz^T X  : A = dz  [N_roi,C]  MN-major, B = X   [N_roi,K]  MN-major
 //
-// Pipeline (one CTA per SM, 320 threads):
-//   warp 0      : TMA producer   (cp.async.bulk.tensor, 128B swizzle, mbarrier tx)
-//   warp 1      : UMMA issuer    (one thread; tcgen05.mma cta_group::1, M=128)
-//   warps 2..9  : epilogue       (tcgen05.ld 32x32b -> registers -> swizzled smem transpose -> coalesced
-//                                 16-byte st.global / red.global)
-// smem ring of kStages {A tile, B tile}; TMEM holds kAccStages accumulators so
-// the epilogue of tile i overlaps the mainloop of tile i+1.
+// Pipeline (one CTA per SM, 384 threads = 3 warpgroups):
+//   warpgroup 0   : producer.  TMA (cp.async.bulk.tensor, 128B swizzle, mbarrier tx) for every bf16 operand and
+//                   every K-major fp32 operand.  wgmma reads tf32 operands K-major only, so an MN-major fp32
+//                   operand is transposed on the way in: the 128 producer threads load it with coalesced 16-byte
+//                   reads and write it into the K-major swizzled layout.
+//   warpgroups 1,2: consumers.  Each owns 64 rows of the 128 x BLOCK_N tile (wgmma m64nNk16 / k8, accumulators in
+//                   registers) and runs its own epilogue straight from the accumulator fragments.
+// smem ring of STAGES {A tile, B tile}.
 #pragma once
 #include "bags_ptx.cuh"
+#include "bags_kernels.cuh"
+#include "bags_wgmma.cuh"
 
 namespace bags {
 
@@ -48,10 +51,11 @@ struct GemmParams {
   const float* colsum_in;  // optional [colsum_tiles, M]: db_out[m] = rowscale(m) * sum_t colsum_in[t, m]
   int colsum_tiles;
   float* colsum_out;       // written by the (n_tile==0, split==0) unit
-  long long* timing;       // debug timeline [grid][8] (ns, %globaltimer) or nullptr
-  int dbg;                 // test hook: bit0 skip global stores, bit1 skip TMEM loads
   int pdl_wait_producer;   // griddepcontrol.wait before the first operand load (B comes from the previous kernel)
   int pdl_wait_epilogue;   // griddepcontrol.wait before the first output access (output prepared by the previous kernel)
+  // MN-major fp32 operands (loaded without TMA): base pointer, leading dimension (elements), extents
+  const float* a_ptr; long long lda; int a_rows, a_k;
+  const float* b_ptr; long long ldb; int b_rows, b_k;
 };
 
 template <int BLOCK_N, bool A_MN, bool B_MN, int EPI, bool TF32, int STAGES>
@@ -59,38 +63,26 @@ struct GemmCfg {
   static constexpr int BLOCK_M = 128;
   static constexpr int ELT = TF32 ? 4 : 2;
   static constexpr int BLOCK_K = 128 / ELT;          // 64 bf16 / 32 tf32 : one 128B swizzle row
-  static constexpr int UMMA_K = 32 / ELT;            // 16 bf16 / 8 tf32
-  static constexpr int K_STEPS = BLOCK_K / UMMA_K;   // 4
-  static constexpr int N_MMA = (BLOCK_N > 256) ? 2 : 1;
-  static constexpr int UMMA_N = BLOCK_N / N_MMA;
-  static constexpr int ACC_STAGES = (2 * BLOCK_N <= 512) ? 2 : 1;
-  static constexpr int TMEM_COLS_RAW = ACC_STAGES * BLOCK_N;
-  static constexpr int TMEM_COLS = TMEM_COLS_RAW <= 32 ? 32 : TMEM_COLS_RAW <= 64 ? 64 : TMEM_COLS_RAW <= 128 ? 128 : TMEM_COLS_RAW <= 256 ? 256 : 512;
+  static constexpr int K_STEPS = 4;                  // wgmma k16 (bf16) / k8 (tf32): 32 B of K each
   static constexpr int A_BYTES = BLOCK_M * 128;      // 16 KB
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int SLAB = 128 / ELT;             // MN elements per 128B (MN-major slab width)
+  static constexpr bool A_MANUAL = A_MN && TF32;     // transposed by the producer threads
+  static constexpr bool B_MANUAL = B_MN && TF32;
+  static constexpr bool ANY_MANUAL = A_MANUAL || B_MANUAL;
+  static constexpr int TMA_BYTES = (A_MANUAL ? 0 : A_BYTES) + (B_MANUAL ? 0 : B_BYTES);
   // TMA boxes per stage
   static constexpr int A_BOXES = A_MN ? BLOCK_M / SLAB : 1;
   static constexpr int A_BOX_BYTES = A_BYTES / A_BOXES;
-  static constexpr int B_BOXES = B_MN ? BLOCK_N / SLAB : N_MMA;
+  static constexpr int B_BOXES = B_MN ? BLOCK_N / SLAB : 1;
   static constexpr int B_BOX_BYTES = B_BYTES / B_BOXES;
-  // epilogue: 8 warps (two per TMEM lane quarter, each owning half of the tile's columns) so that every
-  // SM sub-partition has two warps to interleave -- a lone warp per scheduler is issue-latency bound.
-  // Each warp has one 32-row x 128-byte swizzled transpose buffer.
-  static constexpr int EPI_WARPS = 8;
-  static constexpr int EPI_BUF_BYTES = 32 * 128;
-  static constexpr int EPI_STAGING_BYTES = EPI_WARPS * EPI_BUF_BYTES;   // 32 KB
-  static constexpr int HALF_N = BLOCK_N / 2;
-  static constexpr int EPI_COLS = (EPI == EPI_STORE_BF16) ? 64 : 32;  // output columns per 128-byte row
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_STAGING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 232448, "exceeds 227 KB of shared memory");
-  static_assert(HALF_N % EPI_COLS == 0, "half tile width must be a multiple of the epilogue chunk");
-  static constexpr int NUM_THREADS = 64 + 32 * EPI_WARPS;
-  static_assert(UMMA_N % 16 == 0 && UMMA_N >= 16 && UMMA_N <= 256, "invalid UMMA N");
-  static_assert(!B_MN || (BLOCK_N % SLAB == 0 && N_MMA == 1), "MN-major B needs slab-aligned single MMA");
-  static_assert((UMMA_N * 128) % 1024 == 0, "B half offset must keep 1024B swizzle alignment");
-  static_assert(TMEM_COLS_RAW <= 512, "accumulators exceed TMEM");
+  static_assert(BLOCK_N == 256, "the consumers issue m64n256 MMAs");
+  static constexpr int NUM_THREADS = 384;
+  static constexpr int STAGES_ = STAGES;
+  static constexpr int BLOCK_N_ = BLOCK_N;
 };
 
 __device__ __forceinline__ float row_group_scale(const GemmParams& p, int m) {
@@ -103,300 +95,338 @@ __device__ __forceinline__ float row_group_scale(const GemmParams& p, int m) {
   return s;
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, int EPI, bool TF32, int STAGES>
-__global__ void __launch_bounds__(64 + 32 * 8, 1)
-bags_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const GemmParams p) {
-  using Cfg = GemmCfg<BLOCK_N, A_MN, B_MN, EPI, TF32, STAGES>;
-  constexpr int BLOCK_M = Cfg::BLOCK_M;
-  constexpr int BLOCK_K = Cfg::BLOCK_K;
-
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment is required by the 128B swizzle atoms.
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1 KB aligned, still a shared-space pointer
-  uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;
-  uint8_t* smem_epi = smem + STAGES * Cfg::STAGE_BYTES;  // 1024-byte aligned (all tile sizes are multiples of 1024)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem_epi + Cfg::EPI_STAGING_BYTES);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + STAGES;
-  uint64_t* tfull_bar = bars + 2 * STAGES;
-  uint64_t* tempty_bar = bars + 2 * STAGES + Cfg::ACC_STAGES;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 2 * Cfg::ACC_STAGES);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) { stamp(p.timing, 0); if (p.timing) p.timing[blockIdx.x * 8 + 7] = sm_id(); }
-  pdl_trigger();   // a dependent kernel may begin its own prologue
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
+// Transposing load of one fp32 tile stored MN-major in HBM ([k][row], row contiguous) into the K-major 128B-swizzled
+// layout wgmma reads: tile element (r, k) goes to r * 128 + (((k >> 2) ^ (r & 7)) << 4) + (k & 3) * 4.
+// A warp covers 8 row quads x 4 k per step: 128-byte coalesced reads, 4-way bank conflicts on the scattered stores.
+// Rows / k outside the matrix are zero (like the TMA's out-of-bounds fill).
+template <int ROWS>
+__device__ __forceinline__ void load_tile_transposed(uint8_t* dst, const float* src, long long ld, int rows, int kdim,
+                                                     int r0, int k0, int tid) {
+  constexpr int STEPS = (ROWS / 32) * 8;   // warp steps of (8 quads x 4 k)
+  const int lane = tid & 31, wid = tid >> 5;
+#pragma unroll 4
+  for (int s = wid; s < STEPS; s += 4) {
+    const int r = ((s % (ROWS / 32)) * 8 + (lane & 7)) * 4;
+    const int k = (s / (ROWS / 32)) * 4 + (lane >> 3);
+    const int gr = r0 + r, gk = k0 + k;
+    float v[4] = {0.f, 0.f, 0.f, 0.f};
+    if (gk < kdim) {
+      const float* g = src + static_cast<long long>(gk) * ld + gr;
+      if (gr + 3 < rows) {
+        const float4 q = __ldg(reinterpret_cast<const float4*>(g));
+        v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+      } else {
 #pragma unroll
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+        for (int e = 0; e < 4; ++e) if (gr + e < rows) v[e] = __ldg(g + e);
+      }
     }
 #pragma unroll
-    for (int a = 0; a < Cfg::ACC_STAGES; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], Cfg::EPI_WARPS);
+    for (int e = 0; e < 4; ++e) {
+      const int rr = r + e;
+      *reinterpret_cast<float*>(dst + rr * 128 + (((k >> 2) ^ (rr & 7)) << 4) + (k & 3) * 4) = v[e];
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Pieces shared by the GEMM kernel and the merged backward kernel.  Every problem a kernel runs has the same stage
+// layout (128 x 256 tiles of 128-byte rows), so one shared-memory ring and one set of barriers serve all of them.
+// ---------------------------------------------------------------------------------------------------------------------
+struct Pipe {
+  uint8_t* smem_a;
+  uint8_t* smem_b;
+  uint64_t* full_bar;
+  uint64_t* empty_bar;
+  int stage;
+  uint32_t phase;
+};
+
+// balanced k-block range of split `split`
+__device__ __forceinline__ void split_range(const GemmParams& p, int split, int& kb0, int& kb1) {
+  const int base = p.kblocks_total / p.num_splits, rem = p.kblocks_total % p.num_splits;
+  kb0 = split * base + (split < rem ? split : rem);
+  kb1 = kb0 + base + (split < rem ? 1 : 0);
+}
+
+// Producer side of one unit: k-blocks [kb0, kb1) of the tile at (m0, n0).  Thread 0 issues the TMA loads; with an
+// MN-major fp32 operand all 128 producer threads take part (b_ptr: the B matrix that operand path reads).
+template <class Cfg, bool A_MN, bool B_MN>
+__device__ __forceinline__ void produce_unit(const CUtensorMap* tmap_a, const CUtensorMap* tmap_b, const GemmParams& p,
+                                             const float* b_ptr, int m0, int n0, int kb0, int kb1, Pipe& pp, int tid) {
+  constexpr int STAGES = Cfg::STAGES_;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&pp.empty_bar[pp.stage], pp.phase ^ 1u);
+    const int k0 = kb * Cfg::BLOCK_K;
+    uint8_t* sa = pp.smem_a + pp.stage * Cfg::A_BYTES;
+    uint8_t* sb = pp.smem_b + pp.stage * Cfg::B_BYTES;
+    uint64_t* fb = &pp.full_bar[pp.stage];
+    if (tid == 0 && Cfg::TMA_BYTES > 0) {
+      if (Cfg::ANY_MANUAL) mbar_expect_tx(fb, Cfg::TMA_BYTES);
+      else                 mbar_arrive_expect_tx(fb, Cfg::TMA_BYTES);
+      if (!Cfg::A_MANUAL) {
+#pragma unroll
+        for (int i = 0; i < Cfg::A_BOXES; ++i) {
+          if (A_MN) tma_load_2d(sa + i * Cfg::A_BOX_BYTES, tmap_a, fb, m0 + i * Cfg::SLAB, k0);
+          else      tma_load_2d(sa + i * Cfg::A_BOX_BYTES, tmap_a, fb, k0, m0);
+        }
+      }
+      if (!Cfg::B_MANUAL) {
+#pragma unroll
+        for (int i = 0; i < Cfg::B_BOXES; ++i) {
+          if (B_MN) tma_load_2d(sb + i * Cfg::B_BOX_BYTES, tmap_b, fb, n0 + i * Cfg::SLAB, k0);
+          else      tma_load_2d(sb + i * Cfg::B_BOX_BYTES, tmap_b, fb, k0, n0);
+        }
+      }
+    }
+    if (Cfg::ANY_MANUAL) {
+      if (Cfg::A_MANUAL) load_tile_transposed<Cfg::BLOCK_M>(sa, p.a_ptr, p.lda, p.a_rows, p.a_k, m0, k0, tid);
+      if (Cfg::B_MANUAL) load_tile_transposed<Cfg::BLOCK_N_>(sb, b_ptr, p.ldb, p.b_rows, p.b_k, n0, k0, tid);
+      fence_proxy_async_smem();   // generic-proxy stores -> visible to the wgmma (async proxy) reads
+      mbar_arrive(fb);
+    }
+    if (++pp.stage == STAGES) { pp.stage = 0; pp.phase ^= 1u; }
+  }
+}
+
+// Consumer side of one unit: the mainloop of warpgroup `cw` (rows 64 cw .. 64 cw + 63 of the tile).
+template <class Cfg, bool A_MN, bool B_MN, bool TF32>
+__device__ __forceinline__ void consume_unit(float (&acc)[128], int cw, int kb0, int kb1, Pipe& pp, int lane) {
+  constexpr int STAGES = Cfg::STAGES_;
+  // K-major: 8-row atoms 1024 B apart, K step 32 B.  MN-major (bf16): slabs of 64 elements, K step 16 rows = 2048 B.
+  constexpr bool A_T = A_MN && !TF32, B_T = B_MN && !TF32;
+  constexpr uint32_t A_LBO = A_T ? Cfg::BLOCK_K * 128 : 16, B_LBO = B_T ? Cfg::BLOCK_K * 128 : 16;
+  constexpr uint32_t A_KSTEP = A_T ? 2048 : 32, B_KSTEP = B_T ? 2048 : 32;
+  // this warpgroup's 64 A rows: the second MN slab (MN-major) / rows 64..127 (K-major) -- 8 KB either way
+  const uint32_t a_off = cw * 8192;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&pp.full_bar[pp.stage], pp.phase);
+    const uint32_t sa = smem_u32(pp.smem_a + pp.stage * Cfg::A_BYTES) + a_off;
+    const uint32_t sb = smem_u32(pp.smem_b + pp.stage * Cfg::B_BYTES);
+    fence_regs(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < Cfg::K_STEPS; ++k) {
+      const uint64_t adesc = make_smem_desc(sa + k * A_KSTEP, A_LBO, 1024);
+      const uint64_t bdesc = make_smem_desc(sb + k * B_KSTEP, B_LBO, 1024);
+      const uint32_t accum = (kb > kb0 || k > 0) ? 1u : 0u;
+      if (TF32) wgmma_tf32_n256(acc, adesc, bdesc, accum);
+      else      wgmma_bf16_n256<A_T ? 1 : 0, B_T ? 1 : 0>(acc, adesc, bdesc, accum);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&pp.empty_bar[pp.stage]);   // frees the smem slot
+    if (++pp.stage == STAGES) { pp.stage = 0; pp.phase ^= 1u; }
+  }
+}
+
+// Epilogue from the fragments: thread holds rows r and r + 8, column pairs 8j + 2 (lane & 3).
+// EPI_STORE_*: out = act(oscale * acc + bias);  EPI_RED_F32: out += rowscale(m) * acc.
+template <int BLOCK_N, int EPI>
+__device__ __forceinline__ void epilogue_unit(const float (&acc)[128], const GemmParams& p, int m_tile, int n_tile,
+                                              int split, int cw, int warp, int lane, float oscale) {
+  const bool pair_ok = ((p.ldo & 1) == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 7) == 0);
+  const int r_a = m_tile * 128 + cw * 64 + warp * 16 + (lane >> 2);
+  const int c_base = n_tile * BLOCK_N + 2 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int m = r_a + 8 * h;
+    if (m >= p.M) continue;
+    float scale = oscale;
+    if (EPI == EPI_RED_F32) {
+      scale = row_group_scale(p, m);
+      if (p.colsum_out != nullptr && n_tile == 0 && split == 0 && (lane & 3) == 0) {
+        float cs = 0.f;
+        for (int tt = 0; tt < p.colsum_tiles; ++tt) cs += __ldg(p.colsum_in + static_cast<long long>(tt) * p.M + m);
+        p.colsum_out[m] = scale * cs;
+      }
+    }
+    uint8_t* orow = reinterpret_cast<uint8_t*>(p.out) + static_cast<long long>(m) * p.ldo * (EPI == EPI_STORE_BF16 ? 2 : 4);
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      const int n = c_base + 8 * j;
+      if (n >= p.N) continue;
+      float v0 = acc[4 * j + 2 * h] * scale, v1 = acc[4 * j + 2 * h + 1] * scale;
+      const bool two = n + 1 < p.N;
+      if (EPI == EPI_RED_F32) {
+        float* o = reinterpret_cast<float*>(orow) + n;
+        if (two && pair_ok) {
+          asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(o), "f"(v0), "f"(v1) : "memory");
+        } else {
+          red_add_f32(o, v0);
+          if (two) red_add_f32(o + 1, v1);
+        }
+      } else {
+        if (p.bias != nullptr) { v0 += __ldg(p.bias + n); if (two) v1 += __ldg(p.bias + n + 1); }
+        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (EPI == EPI_STORE_BF16) {
+          __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(orow) + n;
+          if (two && pair_ok) *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(v0, v1);
+          else { o[0] = __float2bfloat16_rn(v0); if (two) o[1] = __float2bfloat16_rn(v1); }
+        } else {
+          float* o = reinterpret_cast<float*>(orow) + n;
+          if (two && pair_ok) *reinterpret_cast<float2*>(o) = make_float2(v0, v1);
+          else { o[0] = v0; if (two) o[1] = v1; }
+        }
+      }
+    }
+  }
+}
+
+__device__ __forceinline__ Pipe setup_pipe(uint8_t* smem_raw, int stages, int a_bytes, int stage_bytes, bool manual) {
+  // 1024-byte alignment is required by the 128B swizzle atoms.
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  Pipe pp;
+  pp.smem_a = smem;
+  pp.smem_b = smem + stages * a_bytes;
+  pp.full_bar = reinterpret_cast<uint64_t*>(smem + stages * stage_bytes);
+  pp.empty_bar = pp.full_bar + stages;
+  pp.stage = 0;
+  pp.phase = 0;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < stages; ++s) {
+      mbar_init(&pp.full_bar[s], manual ? 128 : 1);
+      mbar_init(&pp.empty_bar[s], 8);   // one arrival per consumer warp
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_holder, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_holder;
-  if (threadIdx.x == 0) stamp(p.timing, 1);   // setup done
+  return pp;
+}
+
+template <int BLOCK_N, bool A_MN, bool B_MN, int EPI, bool TF32, int STAGES>
+__global__ void __launch_bounds__(384, 1)
+bags_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                 const GemmParams p) {
+  using Cfg = GemmCfg<BLOCK_N, A_MN, B_MN, EPI, TF32, STAGES>;
+  extern __shared__ uint8_t smem_raw[];
+  const int wg = threadIdx.x >> 7;
+  const int tid = threadIdx.x & 127;
+  pdl_trigger();   // a dependent kernel may begin its own prologue
+  if (threadIdx.x == 0) { tma_prefetch_desc(&tmap_a); tma_prefetch_desc(&tmap_b); }
+  Pipe pp = setup_pipe(smem_raw, STAGES, Cfg::A_BYTES, Cfg::STAGE_BYTES, Cfg::ANY_MANUAL);
 
   const int units_per_split = p.num_m_tiles * p.num_n_tiles;
   const int num_units = units_per_split * p.num_splits;
-  // balanced k-block ranges per split
-  auto split_range = [&](int split, int& kb0, int& kb1) {
-    const int base = p.kblocks_total / p.num_splits, rem = p.kblocks_total % p.num_splits;
-    kb0 = split * base + (split < rem ? split : rem);
-    kb1 = kb0 + base + (split < rem ? 1 : 0);
-  };
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (lane == 0) {
+  if (wg == 0) {
+    // ===================== producer =====================
+    setmaxnreg_dec<40>();
+    if (Cfg::ANY_MANUAL || tid == 0) {
       if (p.pdl_wait_producer) pdl_wait();
-      int stage = 0;
-      uint32_t phase = 0;
       for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
         const int split = u / units_per_split;
         const int t = u - split * units_per_split;
         const int m_tile = t / p.num_n_tiles, n_tile = t - m_tile * p.num_n_tiles;
-        const int m0 = m_tile * BLOCK_M, n0 = n_tile * BLOCK_N;
         int kb0, kb1;
-        split_range(split, kb0, kb1);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u);
-          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          const int k0 = kb * BLOCK_K;
-          uint8_t* sa = smem_a + stage * Cfg::A_BYTES;
-          uint8_t* sb = smem_b + stage * Cfg::B_BYTES;
-#pragma unroll
-          for (int i = 0; i < Cfg::A_BOXES; ++i) {
-            if (A_MN) tma_load_2d(sa + i * Cfg::A_BOX_BYTES, &tmap_a, &full_bar[stage], m0 + i * Cfg::SLAB, k0);
-            else      tma_load_2d(sa + i * Cfg::A_BOX_BYTES, &tmap_a, &full_bar[stage], k0, m0);
-          }
-#pragma unroll
-          for (int i = 0; i < Cfg::B_BOXES; ++i) {
-            if (B_MN) tma_load_2d(sb + i * Cfg::B_BOX_BYTES, &tmap_b, &full_bar[stage], n0 + i * Cfg::SLAB, k0);
-            else      tma_load_2d(sb + i * Cfg::B_BOX_BYTES, &tmap_b, &full_bar[stage], k0, n0 + i * Cfg::UMMA_N);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== UMMA issuer (single thread) =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_instr_desc(TF32 ? 2u : 1u, A_MN, B_MN, BLOCK_M, Cfg::UMMA_N);
-      // K-major (128B swizzle): rows are 128 B, 8-row atoms are 1024 B apart (SBO);
-      //   a K step of UMMA_K elements advances the start address by 32 B.
-      // MN-major (128B swizzle): 64(bf16)-wide MN slabs, each K row is 128 B, 8-row
-      //   K groups 1024 B apart (SBO), slabs BLOCK_K*128 B apart (LBO);
-      //   a K step advances UMMA_K rows = UMMA_K*128 B.
-      // MN-major tf32 must use the 32B-atom swizzle: K atoms are 4 rows (512 B) instead of 8.
-      constexpr uint64_t A_LAYOUT = (A_MN && TF32) ? kSwizzle128B_Base32B : kSwizzle128B;
-      constexpr uint64_t B_LAYOUT = (B_MN && TF32) ? kSwizzle128B_Base32B : kSwizzle128B;
-      constexpr uint32_t A_LBO = A_MN ? BLOCK_K * 128 : 16, A_SBO = (A_MN && TF32) ? 512 : 1024;
-      constexpr uint32_t B_LBO = B_MN ? BLOCK_K * 128 : 16, B_SBO = (B_MN && TF32) ? 512 : 1024;
-      constexpr uint32_t A_KSTEP = A_MN ? Cfg::UMMA_K * 128 : 32;
-      constexpr uint32_t B_KSTEP = B_MN ? Cfg::UMMA_K * 128 : 32;
-      int stage = 0;
-      uint32_t phase = 0;
-      int local = 0;
-      for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++local) {
-        const int split = u / units_per_split;
-        int kb0, kb1;
-        split_range(split, kb0, kb1);
-        const int acc = local % Cfg::ACC_STAGES;
-        const uint32_t acc_phase = (local / Cfg::ACC_STAGES) & 1u;
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (local == 0 && kb == kb0) stamp(p.timing, 2);   // first operands landed
-          const uint32_t sa = smem_u32(smem_a + stage * Cfg::A_BYTES);
-          const uint32_t sb = smem_u32(smem_b + stage * Cfg::B_BYTES);
-#pragma unroll
-          for (int k = 0; k < Cfg::K_STEPS; ++k) {
-            const uint64_t adesc = make_smem_desc(sa + k * A_KSTEP, A_LBO, A_SBO, A_LAYOUT);
-#pragma unroll
-            for (int h = 0; h < Cfg::N_MMA; ++h) {
-              const uint64_t bdesc = make_smem_desc(sb + h * Cfg::UMMA_N * 128 + k * B_KSTEP, B_LBO, B_SBO, B_LAYOUT);
-              const uint32_t accum = (kb > kb0 || k > 0) ? 1u : 0u;
-              if (TF32) umma_tf32(d_tmem + h * Cfg::UMMA_N, adesc, bdesc, idesc, accum);
-              else      umma_bf16(d_tmem + h * Cfg::UMMA_N, adesc, bdesc, idesc, accum);
-            }
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs retire
-          if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-        }
-        umma_commit(&tfull_bar[acc]);      // accumulator complete -> epilogue
-        if (local == 0) stamp(p.timing, 3);   // all MMAs of the first tile issued
+        split_range(p, split, kb0, kb1);
+        produce_unit<Cfg, A_MN, B_MN>(&tmap_a, &tmap_b, p, p.b_ptr, m_tile * 128, n_tile * BLOCK_N, kb0, kb1, pp, tid);
       }
     }
   } else {
-    // ===================== epilogue warps =====================
-    // TMEM -> registers (thread = accumulator row) -> bias / row scale / bf16 pack -> 128B-swizzled smem
-    // tile (conflict-free 16 B writes) -> read back transposed so that every warp-wide 16 B store /
-    // reduction covers 4 complete 128-byte output rows (fully coalesced).
-    const int quarter = warp & 3;  // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;   // which half of the tile's columns
-    uint8_t* buf = smem_epi + (warp - 2) * Cfg::EPI_BUF_BYTES;
+    // ===================== consumers =====================
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1, warp = tid >> 5, lane = tid & 31;
     if (p.pdl_wait_epilogue) pdl_wait();
-    constexpr int OUT_ELT = (EPI == EPI_STORE_BF16) ? 2 : 4;
-    constexpr int VEC = 16 / OUT_ELT;  // output elements per 16-byte vector
-    const bool vec_ok = ((p.ldo * OUT_ELT) % 16 == 0) && ((reinterpret_cast<uintptr_t>(p.out) & 15) == 0);
-    int local = 0;
-    for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++local) {
+    float acc[128];
+    for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
       const int split = u / units_per_split;
       const int t = u - split * units_per_split;
       const int m_tile = t / p.num_n_tiles, n_tile = t - m_tile * p.num_n_tiles;
-      const int m_warp = m_tile * BLOCK_M + quarter * 32;
-      const int m = m_warp + lane;
-      const int n0 = n_tile * BLOCK_N;
-      const int acc = local % Cfg::ACC_STAGES;
-      const uint32_t acc_phase = (local / Cfg::ACC_STAGES) & 1u;
-
-      float scale = 1.0f;
-      if (EPI == EPI_RED_F32) {
-        scale = (m < p.M) ? row_group_scale(p, m) : 0.0f;
-        if (p.colsum_out != nullptr && n_tile == 0 && split == 0 && half == 0 && m < p.M) {
-          float cs = 0.f;
-          for (int tt = 0; tt < p.colsum_tiles; ++tt) cs += __ldg(p.colsum_in + static_cast<long long>(tt) * p.M + m);
-          p.colsum_out[m] = scale * cs;
-        }
-      }
-
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      if (local == 0 && warp == 2 && lane == 0) stamp(p.timing, 4);   // first accumulator complete
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BLOCK_N;
-#pragma unroll 1
-      for (int c = half * Cfg::HALF_N; c < (half + 1) * Cfg::HALF_N; c += Cfg::EPI_COLS) {
-        const int n = n0 + c;
-        if (n >= p.N) break;  // warp-uniform: nothing of this chunk is inside the output
-        uint32_t v[32];
-        uint32_t v2[32];
-        if (!(p.dbg & 2)) {
-          tmem_ld_32x32b_x32(t_row + c, v);
-          if (EPI == EPI_STORE_BF16) tmem_ld_32x32b_x32(t_row + c + 32, v2);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) { v[j] = c + j; v2[j] = lane + j; }
-        }
-        uint4* rowp = reinterpret_cast<uint4*>(buf + lane * 128);
-        if (EPI == EPI_STORE_BF16) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {  // 16-byte chunk j = 8 bf16 = columns 8j..8j+7
-            const uint32_t* src = (j < 4) ? (v + 8 * j) : (v2 + 8 * (j - 4));
-            float f[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(src[e]);
-            if (p.bias != nullptr) {   // (all rows of the warp read the same addresses: one broadcast transaction each)
-#pragma unroll
-              for (int e = 0; e < 8; ++e)
-                if (n + 8 * j + e < p.N) f[e] += __ldg(p.bias + n + 8 * j + e);
-            }
-            if (p.relu) {
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = fmaxf(f[e], 0.f);
-            }
-            uint4 r;
-            r.x = pack_bf16x2(f[0], f[1]);
-            r.y = pack_bf16x2(f[2], f[3]);
-            r.z = pack_bf16x2(f[4], f[5]);
-            r.w = pack_bf16x2(f[6], f[7]);
-            rowp[j ^ (lane & 7)] = r;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {  // 16-byte chunk j = 4 fp32 = columns 4j..4j+3
-            float4 r;
-            r.x = __uint_as_float(v[4 * j + 0]); r.y = __uint_as_float(v[4 * j + 1]);
-            r.z = __uint_as_float(v[4 * j + 2]); r.w = __uint_as_float(v[4 * j + 3]);
-            if (EPI == EPI_STORE_F32) {
-              if (p.bias != nullptr && n + 4 * j + 3 < p.N) {
-                const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + n + 4 * j));
-                r.x += b.x; r.y += b.y; r.z += b.z; r.w += b.w;
-              } else if (p.bias != nullptr) {
-                if (n + 4 * j + 0 < p.N) r.x += __ldg(p.bias + n + 4 * j + 0);
-                if (n + 4 * j + 1 < p.N) r.y += __ldg(p.bias + n + 4 * j + 1);
-                if (n + 4 * j + 2 < p.N) r.z += __ldg(p.bias + n + 4 * j + 2);
-              }
-              if (p.relu) { r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); r.z = fmaxf(r.z, 0.f); r.w = fmaxf(r.w, 0.f); }
-            } else {
-              r.x *= scale; r.y *= scale; r.z *= scale; r.w *= scale;
-            }
-            rowp[j ^ (lane & 7)] = *reinterpret_cast<uint4*>(&r);
-          }
-        }
-        __syncwarp();
-        // read back: iteration it covers tile rows 4*it .. 4*it+3, lane -> (row, 16-byte chunk)
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int r = it * 4 + (lane >> 3);
-          const int ch = lane & 7;
-          const uint4 val = *reinterpret_cast<const uint4*>(buf + r * 128 + ((ch ^ (r & 7)) << 4));
-          const int gm = m_warp + r;
-          const int gn = n + ch * VEC;
-          if (gm < p.M && gn < p.N && !(p.dbg & 1)) {
-            uint8_t* gp = reinterpret_cast<uint8_t*>(p.out) + (static_cast<long long>(gm) * p.ldo + gn) * OUT_ELT;
-            if (vec_ok && gn + VEC <= p.N) {
-              if (EPI == EPI_RED_F32)
-                red_add_v4_f32(reinterpret_cast<float*>(gp), __uint_as_float(val.x), __uint_as_float(val.y),
-                               __uint_as_float(val.z), __uint_as_float(val.w));
-              else
-                *reinterpret_cast<uint4*>(gp) = val;
-            } else {
-              const uint32_t w4[4] = {val.x, val.y, val.z, val.w};
-#pragma unroll
-              for (int e = 0; e < VEC; ++e) {
-                if (gn + e < p.N) {
-                  if (EPI == EPI_STORE_BF16) {
-                    const uint32_t word = w4[e >> 1];
-                    reinterpret_cast<unsigned short*>(gp)[e] = static_cast<unsigned short>((e & 1) ? (word >> 16) : (word & 0xffffu));
-                  } else if (EPI == EPI_RED_F32) {
-                    red_add_f32(reinterpret_cast<float*>(gp) + e, __uint_as_float(w4[e]));
-                  } else {
-                    reinterpret_cast<float*>(gp)[e] = __uint_as_float(w4[e]);
-                  }
-                }
-              }
-            }
-          }
-        }
-        __syncwarp();   // buffer is rewritten by the next chunk
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+      int kb0, kb1;
+      split_range(p, split, kb0, kb1);
+      consume_unit<Cfg, A_MN, B_MN, TF32>(acc, cw, kb0, kb1, pp, lane);
+      epilogue_unit<BLOCK_N, EPI>(acc, p, m_tile, n_tile, split, cw, warp, lane, 1.0f);
     }
-    if (warp == 2 && lane == 0) stamp(p.timing, 5);   // epilogue done
   }
+}
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+// ---------------------------------------------------------------------------------------------------------------------
+// Merged backward: both contractions of the BAGS head's backward in ONE persistent launch.
+//
+//   dW units : dW[C,K]  += gout(bin(c)) * dz^T x       (A = dz MN-major, B = x MN-major, split-K, red.add)
+//   dX units : dX[N,K]   = dz W'                       (A = dz K-major,  B = W' MN-major, plain stores)
+//
+// The units form one work list (dW first: their split-K partials are the longer tail), dealt round-robin to the
+// CTAs, so the SMs that finish their dW share early take dX tiles instead of idling at a kernel boundary.  When all
+// gout[g] are equal (the reference's setting) the dX units read W itself and scale their output by gout[0]: the
+// preparation kernel then skips the scaled copy W' (it makes the same device-side decision).
+// ---------------------------------------------------------------------------------------------------------------------
+struct BwdMergedParams {
+  GemmParams dw;     // tile counts, splits and epilogue fields of the dW problem
+  GemmParams dx;     // ... of the dX problem (b_ptr: W')
+  int dw_units, dx_units;
+  const float* w;    // W (B of the dX units when gout is uniform)
+  const float* gout; // [G] per-bin upstream gradients, or nullptr (dX reads b_ptr unscaled)
+  int G;
+};
+
+template <bool TF32>
+using BwdDwCfg = GemmCfg<256, true, true, EPI_RED_F32, TF32, 4>;
+template <bool TF32>
+using BwdDxCfg = GemmCfg<256, false, true, TF32 ? EPI_STORE_F32 : EPI_STORE_BF16, TF32, 4>;
+
+template <bool TF32>
+__global__ void __launch_bounds__(384, 1)
+bags_bwd_merged_kernel(const __grid_constant__ CUtensorMap t_dzT, const __grid_constant__ CUtensorMap t_xT,
+                       const __grid_constant__ CUtensorMap t_dz, const __grid_constant__ CUtensorMap t_w,
+                       const __grid_constant__ CUtensorMap t_wp, const BwdMergedParams p) {
+  using CW = BwdDwCfg<TF32>;
+  using CX = BwdDxCfg<TF32>;
+  static_assert(CW::STAGE_BYTES == CX::STAGE_BYTES && CW::A_BYTES == CX::A_BYTES, "one ring serves both problems");
+  static_assert(CW::ANY_MANUAL == CX::ANY_MANUAL, "one barrier arrival count serves both problems");
+  extern __shared__ uint8_t smem_raw[];
+  const int wg = threadIdx.x >> 7;
+  const int tid = threadIdx.x & 127;
+  pdl_trigger();
+  Pipe pp = setup_pipe(smem_raw, 4, CW::A_BYTES, CW::STAGE_BYTES, CW::ANY_MANUAL);
+  // dz, the zeroed dW, W' and the bias-gradient partials all come from the preceding kernels
+  pdl_wait();
+  float g0 = 1.0f;
+  const bool uniform = p.gout != nullptr && gout_uniform(p.gout, p.G, g0);
+  const float* xb = uniform ? p.w : p.dx.b_ptr;
+  const CUtensorMap* txb = uniform ? &t_w : &t_wp;
+  const float xscale = uniform ? g0 : 1.0f;
+
+  const int dw_per_split = p.dw.num_m_tiles * p.dw.num_n_tiles;
+  const int num_units = p.dw_units + p.dx_units;
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (CW::ANY_MANUAL || tid == 0) {
+      for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+        if (u < p.dw_units) {
+          const int split = u / dw_per_split, t = u - split * dw_per_split;
+          const int m_tile = t / p.dw.num_n_tiles, n_tile = t - m_tile * p.dw.num_n_tiles;
+          int kb0, kb1;
+          split_range(p.dw, split, kb0, kb1);
+          produce_unit<CW, true, true>(&t_dzT, &t_xT, p.dw, p.dw.b_ptr, m_tile * 128, n_tile * 256, kb0, kb1, pp, tid);
+        } else {
+          const int t = u - p.dw_units;
+          const int m_tile = t / p.dx.num_n_tiles, n_tile = t - m_tile * p.dx.num_n_tiles;
+          produce_unit<CX, false, true>(&t_dz, txb, p.dx, xb, m_tile * 128, n_tile * 256, 0, p.dx.kblocks_total, pp, tid);
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1, warp = tid >> 5, lane = tid & 31;
+    float acc[128];
+    for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+      if (u < p.dw_units) {
+        const int split = u / dw_per_split, t = u - split * dw_per_split;
+        const int m_tile = t / p.dw.num_n_tiles, n_tile = t - m_tile * p.dw.num_n_tiles;
+        int kb0, kb1;
+        split_range(p.dw, split, kb0, kb1);
+        consume_unit<CW, true, true, TF32>(acc, cw, kb0, kb1, pp, lane);
+        epilogue_unit<256, EPI_RED_F32>(acc, p.dw, m_tile, n_tile, split, cw, warp, lane, 1.0f);
+      } else {
+        const int t = u - p.dw_units;
+        const int m_tile = t / p.dx.num_n_tiles, n_tile = t - m_tile * p.dx.num_n_tiles;
+        consume_unit<CX, false, true, TF32>(acc, cw, 0, p.dx.kblocks_total, pp, lane);
+        epilogue_unit<256, TF32 ? EPI_STORE_F32 : EPI_STORE_BF16>(acc, p.dx, m_tile, n_tile, 0, cw, warp, lane, xscale);
+      }
+    }
   }
-  if (threadIdx.x == 0) stamp(p.timing, 6);
 }
 
 }  // namespace bags

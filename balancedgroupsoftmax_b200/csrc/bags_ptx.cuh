@@ -1,10 +1,9 @@
-// Thin inline-PTX wrappers for the sm_100a features the BAGS kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and
-// a few cache-hinted global accesses.  No CUTLASS/CuTe dependency.
+// Thin inline-PTX wrappers for the sm_90a features the BAGS kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (fences, groups, shared-memory descriptors),
+// setmaxnreg and a few cache-hinted global accesses.  No CUTLASS/CuTe dependency.
 //
-// Descriptor bit layouts follow the PTX ISA "tcgen05 matrix descriptor" /
-// "instruction descriptor" tables (same fields CUTLASS names
-// UMMA::SmemDescriptor / UMMA::InstrDescriptor).
+// The wgmma descriptor bit layout follows the PTX ISA "matrix descriptor" table for
+// wgmma.mma_async (the fields CUTLASS names GMMA::DescriptorIterator / GmmaDescriptor).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -94,19 +93,16 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   return ok != 0;
 }
 
-// Bounded wait: a broken pipeline must never hang the GPU box.  After ~2^28
-// failed probes (seconds) the kernel raises a flag in global memory and traps.
+// Bounded wait: a broken pipeline must never hang the GPU.  After ~2^28
+// failed probes (seconds) the kernel traps.
 #ifndef BAGS_WAIT_LIMIT
 #define BAGS_WAIT_LIMIT (1u << 28)
 #endif
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  // (no printf here: a call inside the mainloop makes ptxas serialise the wgmma pipeline)
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > BAGS_WAIT_LIMIT) {
-      printf("bags: mbarrier wait timed out (block %d thread %d bar %u parity %u)\n",
-             (int)blockIdx.x, (int)threadIdx.x, smem_u32(bar), parity);
-      __trap();
-    }
+    if (++spins > BAGS_WAIT_LIMIT) __trap();
   }
 }
 
@@ -127,89 +123,45 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, ui
       : "memory");
 }
 
-// Multicast variant: the box is written to the same shared-memory offset of every CTA in `cta_mask` of the
-// cluster, and each destination's mbarrier (same offset) receives the complete_tx.
-__device__ __forceinline__ void tma_load_2d_mc(void* smem_dst, const void* tmap, uint64_t* bar,
-                                               int32_t c_inner, int32_t c_outer, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)),
-        "r"(c_inner), "r"(c_outer), "h"(cta_mask)
-      : "memory");
-}
-// commit that arrives on the mbarrier at the same offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
+
+// expect `bytes` more transaction bytes on `bar` without arriving (the arrivals come from other threads)
+__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 
-// pull one box of a tiled tensor map into L2 ahead of the TMA load that will need it (no smem, no barrier)
-__device__ __forceinline__ void tma_prefetch_l2_2d(const void* tmap, int32_t c_inner, int32_t c_outer) {
-  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
-               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(c_inner), "r"(c_outer)
-               : "memory");
+// ----------------------------------------------------------------------------
+// wgmma : fences, groups, descriptors
+// ----------------------------------------------------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- CTA-pair (cta_group::2) variants: two CTAs of a cluster (ranks 2i, 2i+1) act as one 256-row MMA unit ----
-// shared::cluster addresses carry the CTA rank above bit 24; clearing bit 24 of one of our own shared addresses
-// yields the same offset in the even ("leader") CTA of the pair.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-// load into THIS CTA's shared memory, but count the bytes on the LEADER CTA's mbarrier
-__device__ __forceinline__ void tma_load_2d_2sm(void* smem_dst, const void* tmap, uint64_t* bar,
-                                                int32_t c_inner, int32_t c_outer) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask),
-        "r"(c_inner), "r"(c_outer)
-      : "memory");
-}
-// arrive on the leader CTA's copy of `bar`
-__device__ __forceinline__ void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_holder, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_2sm() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs, 256 rows] (+)= A[smem of both CTAs] * B[smem halves of both CTAs]; issued by the leader
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32_2sm(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                              uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once the pair's MMAs retire) on the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_2sm_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// Shared-memory matrix descriptor (64 bit), 128-byte swizzle (the layout TMA SWIZZLE_128B writes):
+//   [ 0,14) start address >> 4      [16,30) leading-dim byte offset >> 4
+//   [32,46) stride-dim byte offset >> 4      [49,52) base offset (0: tiles are 1024 B aligned)
+//   [62,64) swizzle mode (1 = 128B)
+// K-major: rows of 128 B, 8-row atoms SBO = 1024 B apart (LBO unused); a K step of 32 B advances the start address.
+// MN-major (bf16 only): 64-element MN slabs LBO apart, 8-row K groups SBO = 1024 B apart; a K step of 16 rows
+// advances the start address by 2048 B.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
+  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
+  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
 }
 
 // 2-D tiled store shared::cta -> global (bulk async group); out-of-bounds parts of the box are clipped.
@@ -232,140 +184,6 @@ __device__ __forceinline__ void tma_store_wait_read() {
   asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
 }
 __device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------
-// tcgen05 : TMEM allocation
-// ----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_holder, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_holder)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-// ----------------------------------------------------------------------------
-// tcgen05 : descriptors
-// ----------------------------------------------------------------------------
-// Shared-memory matrix descriptor (64 bit):
-//   [ 0,14) start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1 (sm_100)
-//   [49,52) base offset (0: tiles are 1024 B aligned)   [61,64) swizzle mode
-// Swizzle mode 2 = 128-byte swizzle of 16 B chunks (TMA SWIZZLE_128B); mode 1 = 128-byte swizzle of
-// 32 B chunks (TMA SWIZZLE_128B_ATOM_32B), the only layout tcgen05 accepts for MN-major 32-bit (tf32)
-// operands.  The mode must match the TMA tensor map that filled the tile.
-constexpr uint64_t kSwizzle128B = 2;
-constexpr uint64_t kSwizzle128B_Base32B = 1;
-
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                                   uint32_t sbo_bytes,
-                                                   uint64_t layout = kSwizzle128B) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= layout << 61;
-  return d;
-}
-
-// Instruction descriptor (32 bit) for kind::f16 / kind::tf32, fp32 accumulate:
-//   [4,6) D format (1 = f32)  [7,10) A format  [10,13) B format
-//   (kind::f16: 0 = f16, 1 = bf16 ; kind::tf32: 2 = tf32)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_instr_desc(uint32_t ab_format, bool a_mn, bool b_mn,
-                                                       uint32_t m, uint32_t n) {
-  return (1u << 4) | (ab_format << 7) | (ab_format << 10) | ((a_mn ? 1u : 0u) << 15) |
-         ((b_mn ? 1u : 0u) << 16) | ((n >> 3) << 17) | ((m >> 4) << 24);
-}
-
-// ----------------------------------------------------------------------------
-// tcgen05 : MMA issue / commit
-// ----------------------------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc,
-                                          uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once all previously issued MMAs of this thread retire.
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
-// ----------------------------------------------------------------------------
-// tcgen05 : TMEM -> registers (32 lanes x 32 columns of 32-bit per warp)
-// ----------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// registers -> TMEM: thread l of the warp writes 16 consecutive 32-bit columns of lane (quarter*32 + l)
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() {
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
 
 // ----------------------------------------------------------------------------
 // global memory helpers

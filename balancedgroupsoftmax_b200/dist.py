@@ -106,7 +106,7 @@ def flat_grad_bucket(shapes: List[Tuple[int, ...]], device, dtype=torch.float32)
 
 
 # ---------------------------------------------------------------------------------------------------
-# NVLink peer-memory exchange (libbags_b200.so: bags_grad_allreduce) -- the B200 path
+# NVLink peer-memory exchange (libbags_b200.so: bags_grad_allreduce) -- the NVSwitch path
 # ---------------------------------------------------------------------------------------------------
 class PeerGradBucket(object):
     """Flat fp32 gradient bucket in symmetric (peer-mapped) memory + its one-kernel all-reduce.
@@ -237,8 +237,7 @@ def _exchange_overlapped(self, side_stream=None):
     cur = torch.cuda.current_stream(dev)
     if isinstance(self, PeerGradBucket) and self.max_blocks == 0:
         # An exchange that shares the GPU with the dX GEMM wants a SMALL grid: its blocks then live on the SMs the GEMM
-        # leaves free instead of competing with GEMM CTAs for issue slots (measured at 2 / 4 / 8 ranks,
-        # profiles/r02_bench_*gpu_matrix.log: 8 ranks 67.0 us/step on 16 blocks vs 74.7 on 39), but large enough to keep
+        # leaves free instead of competing with GEMM CTAs for issue slots, but large enough to keep
         # this rank's slice in flight: one block per 2048 16-byte vectors of the slice, between 16 and 48.
         per_rank = (self.count // 4 + self.world - 1) // self.world
         self.max_blocks = max(16, min(48, (per_rank + 2047) // 2048))
@@ -284,8 +283,7 @@ def make_grad_bucket(shapes: List[Tuple[int, ...]], device, prefer_peer: bool = 
             b = PeerGradBucket(shapes, device, max_blocks=max_blocks)
             if not b.mc_ptr and b.world > 4 and os.environ.get('BAGS_ALLREDUCE') != 'peer':
                 # without an NVSwitch multicast object the kernel falls back to plain peer loads / stores, which read every
-                # element from all ranks: fine at 2 ranks (18.5 us vs 25), slower than NCCL at 8 (163 vs 102 us per step
-                # with the exchange inside the step; profiles/r02_bench_8gpu_matrix.log)
+                # element from all ranks: fine at 2 ranks, slower than NCCL at 8
                 import warnings
                 warnings.warn('no multicast (NVLS) mapping at %d ranks: using NCCL all-reduce for the gradient bucket' % b.world)
             elif b.self_test():

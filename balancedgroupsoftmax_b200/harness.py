@@ -1,4 +1,4 @@
-"""Synthetic-image detector harness around the BAGS head (SURVEY.md §8f-1) -- the CALLER of the hot path.
+"""Synthetic-image detector harness around the BAGS head -- the CALLER of the hot path.
 
 The reference's detectors (``TwoStageDetector.forward_train`` mmdet/models/detectors/two_stage.py:134-265,
 ``CascadeRCNN`` cascade_rcnn.py:152-298) feed the head like this, per image batch:
@@ -133,7 +133,7 @@ class BagsDetectorHarness(nn.Module):
         self.stage_loss_weights = [float(w) for w in stage_loss_weights]
         self.stage_iou_thrs = [float(t) for t in stage_iou_thrs]
         self.rois_per_image, self.pos_fraction = rois_per_image, pos_fraction
-        # shared FCs / fc_reg under bf16 autocast (cuBLAS; 11x the fc_cls FLOPs, SURVEY.md 8f-3): the BAGS part takes the
+        # shared FCs / fc_reg under bf16 autocast (cuBLAS; 11x the fc_cls FLOPs): the BAGS part takes the
         # bf16 activations as they come
         self.amp = bool(amp)
         # several stages regress class-agnostically, like the cascade configs (configs/bags/gs_cascade_*.py)

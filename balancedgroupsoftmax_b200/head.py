@@ -8,9 +8,9 @@ signatures and returned dict keys are identical so configs/bags/*.py blocks buil
     SharedFCBBoxHead    mmdet/models/bbox_heads/convfc_bbox_head.py:171-185
     GSBBoxHeadWith0     mmdet/models/bbox_heads/gs_bbox_head_with0.py:14-380
 
-What differs is the execution of the hot path (SURVEY.md §8a):
+What differs is the execution of the hot path:
 
-  * ``fc_cls`` (convfc_bbox_head.py:166) runs on tcgen05 tensor cores through the C ABI
+  * ``fc_cls`` (convfc_bbox_head.py:166) runs on wgmma tensor cores through the C ABI
     (``bags_linear_fwd``) instead of cuBLAS SGEMM;
   * ``_remap_labels`` + ``_sample_others`` + ``_slice_preds`` + 5x ``CrossEntropyLoss``
     (gs_bbox_head_with0.py:63-171) -- ~70 small kernels and >=15 host syncs per call in the
@@ -21,7 +21,7 @@ What differs is the execution of the hot path (SURVEY.md §8a):
   * ``_merge_score`` (gs_bbox_head_with0.py:239-273) is one kernel (``bags_merge_scores``).
 
 The shared FCs, ``fc_reg`` and the SmoothL1 box loss are neighbours of the path and stay
-plain ``nn.Linear`` / PyTorch, exactly as SURVEY.md §2.1 scopes them.
+plain ``nn.Linear`` / PyTorch, exactly as scopes them.
 """
 from __future__ import annotations
 
@@ -133,7 +133,7 @@ class ClsScoreHandle(object):
     It records the fc_cls input instead of launching the projection, so that ``loss`` can run
     the fused forward (GEMM + grouped softmax-CE) without a logits round trip through autograd.
     ``tensor()`` (or any tensor attribute access) materialises real logits with the same
-    tcgen05 kernel, autograd-connected, so every other consumer keeps working.
+    wgmma kernel, autograd-connected, so every other consumer keeps working.
     """
 
     def __init__(self, head: 'GSBBoxHeadWith0', x_cls: torch.Tensor):
@@ -184,7 +184,7 @@ class ClsScoreHandle(object):
 
 
 class FcClsFunction(torch.autograd.Function):
-    """Materialised logits = x W^T + b on tcgen05 (bags_linear_fwd); backward reuses bags_bwd."""
+    """Materialised logits = x W^T + b on the wgmma GEMM (bags_linear_fwd); backward reuses bags_bwd."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, compute_dtype):
@@ -422,7 +422,7 @@ def _cfg_get(cfg, key, default=None):
 
 
 class GSBBoxHeadWith0(SharedFCBBoxHead):
-    """Balanced Group Softmax head (gs_bbox_head_with0.py:14-380), fused B200 execution.
+    """Balanced Group Softmax head (gs_bbox_head_with0.py:14-380), fused H100 execution.
 
     Extra, optional ``gs_config`` keys (all default to reference behaviour where one exists):
         tables            a ``GroupTables`` object instead of the three file paths
@@ -433,7 +433,7 @@ class GSBBoxHeadWith0(SharedFCBBoxHead):
         fuse_loss         True (default): training forward returns a ClsScoreHandle
         graph_cache       False (default).  True: ``loss`` replays two CUDA graphs per recurring RoI count
                           (``api.GraphCachedHeadLoss``) -- graph-replay host cost with a data-dependent N
-        native_trunk      True (default): shared FCs / fc_reg on this library's tcgen05 GEMMs
+        native_trunk      True (default): shared FCs / fc_reg on this library's wgmma GEMMs
         eval_compute_dtype 'fp32' (default) / 'bf16' for the test-time logits
     """
 
@@ -479,7 +479,7 @@ class GSBBoxHeadWith0(SharedFCBBoxHead):
         ed = _cfg_get(gs_config, 'eval_compute_dtype', os.environ.get('BAGS_EVAL_COMPUTE_DTYPE', 'fp32'))
         self.eval_compute_dtype = {'bf16': torch.bfloat16, 'bfloat16': torch.bfloat16, 'fp32': torch.float32,
                                    'float32': torch.float32, 'tf32': torch.float32}[str(ed).lower()]
-        # shared FCs + fc_reg on this library's tcgen05 GEMMs (bias + ReLU in the epilogue) instead of nn.Linear / cuBLAS
+        # shared FCs + fc_reg on this library's wgmma GEMMs (bias + ReLU in the epilogue) instead of nn.Linear / cuBLAS
         self.native_trunk = bool(_cfg_get(gs_config, 'native_trunk', os.environ.get('BAGS_NATIVE_TRUNK', '1') != '0'))
         # opt-in: CUDA-graph replay per recurring RoI count behind loss() (api.GraphCachedHeadLoss)
         self.graph_cache = bool(_cfg_get(gs_config, 'graph_cache', os.environ.get('BAGS_GRAPH_CACHE', '0') == '1'))
@@ -518,7 +518,7 @@ class GSBBoxHeadWith0(SharedFCBBoxHead):
         device = torch.device(device)
         if device.type != 'cuda':
             raise ops.nat.BagsNativeError(
-                'the BAGS head hot path runs on a B200 GPU only (tensor on %s); there is no CPU fallback' % device)
+                'the BAGS head hot path runs on an H100 GPU only (tensor on %s); there is no CPU fallback' % device)
         idx = device.index if device.index is not None else torch.cuda.current_device()
         dt = self._device_tables.get(idx)
         if dt is None:
@@ -539,7 +539,7 @@ class GSBBoxHeadWith0(SharedFCBBoxHead):
 
     def _trunk(self, x):
         """convfc_bbox_head.py:132-160 for the FC-only configuration the BAGS configs use: flatten -> (Linear + ReLU) x
-        num_shared_fcs, each one LinearActFunction (tcgen05 GEMM, bias + ReLU in its epilogue; the activations travel
+        num_shared_fcs, each one LinearActFunction (wgmma GEMM, bias + ReLU in its epilogue; the activations travel
         in the operand dtype)."""
         if not self._use_native_trunk(x):
             return super()._trunk(x)
@@ -617,7 +617,7 @@ class GSBBoxHeadWith0(SharedFCBBoxHead):
                     and reduction_override in (None, 'mean') and isinstance(cls_score, ClsScoreHandle)
                     and cls_score._logits is None and torch.is_grad_enabled()):
                 # opt-in (gs_config['graph_cache']): recurring RoI counts replay two CUDA graphs (sampler + fused forward;
-                # merged backward) instead of paying ~220 us of host work per call; new counts run eagerly first
+                # preparation + merged backward) instead of paying the host work of every call; new counts run eagerly first
                 if self._graph_loss is None:
                     from .api import GraphCachedHeadLoss
                     self._graph_loss = GraphCachedHeadLoss(dt, self.others_sample_ratio, compute_dtype=self.compute_dtype,

@@ -1,8 +1,7 @@
 """NUMA-aware pinned staging buffers for the host -> device leg of the head's inputs.
 
-On the 2-socket hosts of the B200 boxes the H2D rate of one step's inputs (8.4 MB of bf16 RoI features) measured
-between 20 and 55 GB/s depending on where the pinned pages live and which cores last wrote them
-(profiles/r01_probe_h2d_*.json).  ``pinned_like`` allocates and first-touches the staging buffer from ONE thread
+On a multi-socket host the H2D rate of one step's inputs (8.4 MB of bf16 RoI features) depends on where the pinned
+pages live and which cores last wrote them.  ``pinned_like`` allocates and first-touches the staging buffer from ONE thread
 bound to the GPU's own NUMA node (``/sys/bus/pci/devices/<bdf>/local_cpulist``), which is what a data-loader
 worker pinned next to its GPU would do.  Pure host plumbing: no effect on results.
 """

@@ -10,7 +10,7 @@ They are NOT the hot path: inside ``GSBBoxHeadWith0.loss`` the five per-bin
 ``CrossEntropyLoss`` calls of the reference (gs_bbox_head_with0.py:164-171) are
 replaced by one fused CUDA call (ops.GroupSoftmaxFunction); the per-bin modules
 only contribute their ``loss_weight``.  ``SmoothL1Loss`` (<= 128x4 values per
-image) stays plain PyTorch, as SURVEY.md §2.1 #11 scopes it.
+image) stays plain PyTorch, as scopes it.
 """
 from __future__ import annotations
 

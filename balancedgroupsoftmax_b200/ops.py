@@ -6,7 +6,7 @@ whose forward/backward call a compiled ``forward``/``backward``):
 
     GroupSoftmaxFunction.forward/backward      <- torch.autograd.Function
         -> bags_fwd / bags_bwd                 <- C ABI (include/bags_b200.h), ctypes
-            -> sm_100a kernels                 <- csrc/*.cuh
+            -> sm_90a kernels                  <- csrc/*.cuh
 
 Nothing in this file computes on the CPU or with torch math ops; torch is used
 for device memory, streams and autograd bookkeeping only.  Every entry point
@@ -35,7 +35,7 @@ def _require_cuda(*tensors) -> None:
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise nat.BagsNativeError(
-                'BAGS ops run on a B200 GPU only (got a %s tensor); there is no CPU fallback' % t.device)
+                'BAGS ops run on an H100 GPU only (got a %s tensor); there is no CPU fallback' % t.device)
 
 
 def _dtype_code(dt: torch.dtype) -> int:
@@ -215,7 +215,7 @@ def group_ce(logits: torch.Tensor, labels: torch.Tensor, dt: DeviceTables,
 
 
 def fused_eligible(dt: DeviceTables) -> bool:
-    """True when bags_fwd can keep the logits in tensor memory (fused GEMM + grouped CE kernel)."""
+    """True when bags_fwd can keep the logits on chip (fused GEMM + grouped CE kernel)."""
     return bool(nat.lib().bags_fused_eligible(dt.slices_host, dt.G, dt.num_logits))
 
 
@@ -396,7 +396,7 @@ def multiclass_nms(multi_bboxes: torch.Tensor, multi_scores: torch.Tensor, score
 
 def gemm_probe(a, a_mn: bool, b, b_mn: bool, M: int, N: int, K: int, block_n: int = 256, splits: int = 1,
                epi: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Test hook for one tcgen05 GEMM (see bags_gemm_probe)."""
+    """Test hook for one wgmma GEMM (see bags_gemm_probe)."""
     _require_cuda(a, b)
     dev = a.device
     if out is None:
@@ -408,10 +408,10 @@ def gemm_probe(a, a_mn: bool, b, b_mn: bool, M: int, N: int, K: int, block_n: in
     return out
 
 
-# --------------------------------------------------------------------------- the trunk's linear layers (SURVEY.md 8f-3)
+# --------------------------------------------------------------------------- the trunk's linear layers
 def linear_act(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], relu: bool,
                out_dtype: Optional[torch.dtype] = None, out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[N,C] = act(x @ w^T + bias), act = ReLU or identity, on the tcgen05 GEMM (convfc_bbox_head.py:138-143,167).
+    """out[N,C] = act(x @ w^T + bias), act = ReLU or identity, on the wgmma GEMM (convfc_bbox_head.py:138-143,167).
     x and w share the operand dtype (bf16, or fp32 = TF32 products); out is fp32 or (bf16 operands) bf16."""
     _require_cuda(x, w, bias)
     x, w = _row_major(x), _row_major(w)
@@ -488,10 +488,10 @@ def _single_slice_tables(cols: int, device) -> DeviceTables:
 
 class LinearActFunction(torch.autograd.Function):
     """y = act(x W^T + b) for the head's shared FCs (ReLU) and fc_reg (identity) -- nn.Linear (+ nn.ReLU) of the
-    reference (convfc_bbox_head.py:138-143,167) on this library's tcgen05 GEMMs, forward and backward:
+    reference (convfc_bbox_head.py:138-143,167) on this library's wgmma GEMMs, forward and backward:
 
     forward : bags_linear_act_fwd (bias + activation in the GEMM epilogue; bf16 output feeds the next layer)
-    backward: bags_act_bwd (ReLU mask + cast) -> bags_bwd (dW = g^T x, db, dX = g W in one merged launch)"""
+    backward: bags_act_bwd (ReLU mask + cast) -> bags_bwd (dW = g^T x, db, dX = g W: preparation + one merged launch)"""
 
     @staticmethod
     def forward(ctx, x, weight, bias, relu, compute_dtype, out_dtype):
@@ -526,10 +526,10 @@ class LinearActFunction(torch.autograd.Function):
 
 
 # --------------------------------------------------------------------------- autograd
-# where the backward's preparation work runs: 1 = dW is zeroed by the fused forward kernel (idle epilogue warps)
+# where the backward's preparation work runs: 1 = dW is zeroed by the fused forward kernel (idle producer warps)
 PREP_IN_FORWARD = os.environ.get('BAGS_PREP_IN_FORWARD', '1') != '0'
-# 1 = the bias-gradient column sums come from the forward's epilogue as well (otherwise a job of the backward kernel).
-# Costs the forward ~1.2 us and is a loss for the merged backward (one GPU); with a grad_bucket (data-parallel schedule)
+# 1 = the bias-gradient column sums come from the forward's epilogue as well (otherwise a job of the backward's
+# preparation kernel).  Off by default on one GPU; with a grad_bucket (data-parallel schedule)
 # it is always on: the dW + db launch -- on the critical path before the exchange -- then has nothing to prepare.
 FWD_COLSUM = os.environ.get('BAGS_FWD_COLSUM', '0') == '1'
 
@@ -537,9 +537,9 @@ FWD_COLSUM = os.environ.get('BAGS_FWD_COLSUM', '0') == '1'
 class GroupSoftmaxFunction(torch.autograd.Function):
     """losses[G] = BAGS(fc_cls(x)) with a fused backward.
 
-    forward : bags_fwd  (fused kernel: tcgen05 fc_cls GEMM with the grouped softmax-CE in its epilogue;
-              logits stay in tensor memory unless a ``logits_out`` buffer is given; saves dz~ and its column sums)
-    backward: bags_bwd  (dW = dz^T x, db, dX = dz W on tcgen05; per-bin upstream gradients applied
+    forward : bags_fwd  (fused kernel: wgmma fc_cls GEMM with the grouped softmax-CE in its epilogue;
+              logits stay on chip unless a ``logits_out`` buffer is given; saves dz~ and its column sums)
+    backward: bags_bwd  (dW = dz^T x, db, dX = dz W on wgmma; per-bin upstream gradients applied
               in the GEMM epilogue / on a scaled copy of W)
 
     compute_dtype torch.bfloat16: x and W are used as bf16 operands (fp32 masters are cast by
@@ -552,7 +552,7 @@ class GroupSoftmaxFunction(torch.autograd.Function):
         """``grad_bucket`` (optional, data-parallel training): an object with ``views = (dW [C,K] fp32, db [C] fp32)`` living
         in the ranks' exchange bucket and ``exchange_overlapped()`` -- e.g. ``dist.PeerGradBucket``.  The backward then
         writes dW / db straight into the bucket, starts the exchange as soon as they are complete and computes dX while
-        the gradients travel (SURVEY.md 8e; the reference exchanges after the whole backward, dist_utils.py:51-58);
+        the gradients travel (the reference exchanges after the whole backward, dist_utils.py:51-58);
         the returned weight / bias gradients ARE the bucket views, holding the mean over ranks."""
         _require_cuda(x, weight, bias, labels)
         # (autograd does not record inside Function.forward: the inputs are used as they are, no detach() round trips)

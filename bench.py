@@ -13,7 +13,7 @@ One "step" = one pass of the hot path over one batch of 4096 synthetic RoIs per 
 `value`  : whole-job RoIs/s with inputs resident in HBM, K steps replayed from a CUDA graph
            (launch-bound inner loop), timed with CUDA events on the launching stream, max over
            ranks.  Each step uses a different member of a rotating pool of buffer sets larger than
-           the 126 MB L2, so no step finds its inputs in cache.
+           the 50 MB L2, so no step finds its inputs in cache.
 `e2e`    : the same metric through the public autograd API (GroupSoftmaxFunction behind
            balancedgroupsoftmax_b200.bags_head_loss) with HOST (pinned) features/labels copied
            H2D and the per-bin losses read back D2H inside the timed region.
@@ -57,17 +57,8 @@ def peaks():
                         source='measured')
         except Exception:
             pass
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source='fallback')
-
-
-def ncu_traffic(kernel):
-    """DRAM bytes per launch of `kernel` from the committed ncu --set full capture (profiles/ncu_traffic.json)."""
-    try:
-        d = json.load(open(os.path.join(ROOT, 'profiles', 'ncu_traffic.json')))
-        k = d.get(kernel)
-        return None if k is None else int(k['dram_read'] + k['dram_write'])
-    except Exception:
-        return None
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- not reached figures
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source='H100 SXM data sheet')
 
 
 def make_labels(torch, n, num_classes, gen):
@@ -251,8 +242,8 @@ def cpu_baseline(n, steps=10):
 
 
 def gpu_library_baseline(torch, tables, dev, n, iters=20):
-    """The on-device bar SURVEY.md 2.2 names: the reference's own formulation through the vendor libraries on the SAME
-    B200 -- F.linear (cuBLAS) + 5 x F.cross_entropy on column slices (ATen) + autograd backward (dW, db, dX).  The
+    """The on-device bar: the reference's own formulation through the vendor libraries on the SAME
+    H100 -- F.linear (cuBLAS) + 5 x F.cross_entropy on column slices (ATen) + autograd backward (dW, db, dX).  The
     reference's host-synchronising sampler (gs_bbox_head_with0.py:63-89) is left OUT (masks are precomputed device
     tensors), which only flatters the library arm.  Timed eagerly (how the reference runs) and from a CUDA graph."""
     import torch.nn.functional as F
@@ -328,6 +319,27 @@ def gpu_library_baseline(torch, tables, dev, n, iters=20):
 
 
 # ======================================================================================= our arm
+DUMP_ARRAY_BYTES = 24 << 20   # per array: dW (5 MB) + dX + the small ones stay below 64 MB
+
+
+def dump_outputs(out_dir, s):
+    """What the last timed step handed its caller: the per-bin losses and the fc_cls gradients dW, db and the input
+    gradient dX, as float32 .npy files (about 22 MB at the default size).  The inputs come from fixed seeds, so two
+    builds can be compared output for output.  An array larger than DUMP_ARRAY_BYTES (dX beyond 6144 RoIs) is stored
+    as a fixed, seeded sample of its rows; <name>_rows.npy (float64) then lists the sampled row indices."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for name in ('loss', 'dW', 'db', 'dX'):
+        a = s[name].detach().float()
+        if a.numel() * 4 > DUMP_ARRAY_BYTES:
+            keep = DUMP_ARRAY_BYTES // (4 * a[0].numel())
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=keep, replace=False))
+            a = a[torch.from_numpy(rows).to(a.device)]
+            np.save(os.path.join(out_dir, name + '_rows.npy'), rows.astype(np.float64))
+        np.save(os.path.join(out_dir, name + '.npy'), a.cpu().numpy())
+
+
 def run_ours(args):
     import numpy as np
     import torch
@@ -341,7 +353,7 @@ def run_ours(args):
     rank = int(os.environ.get('RANK', '0'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py needs a B200 GPU (no CPU fallback); use --impl reference for the CPU arm')
+        raise SystemExit('bench.py needs an H100 GPU (no CPU fallback); use --impl reference for the CPU arm')
     torch.cuda.set_device(local_rank)
     dev = torch.device('cuda', local_rank)
     if world > 1:
@@ -359,7 +371,7 @@ def run_ours(args):
     elt = 2 if dtype == torch.bfloat16 else 4
     ldd = ops.pad_cols(C)
     per_set = n * K_FEAT * elt * 2 + n * C * 4 + n * ldd * elt + C * K_FEAT * 4 + C * K_FEAT * elt * 2
-    pool = max(2, int(np.ceil(2.2 * 126e6 / per_set)))
+    pool = max(2, int(np.ceil(2.2 * 50e6 / per_set)))
     if args.pool:
         pool = max(2, args.pool)
     elif world > 1 and args.exchange == 'overlap-next-step':
@@ -429,9 +441,8 @@ def run_ours(args):
                                                clear=(s['dW'] if prez else None),
                                                want_colsum=(args.prep == 'fwd-zero-colsum' and not args.unfused))
         if split_bwd:
-            # in-step schedule with overlap (SURVEY.md 8e: "launch as soon as the dW epilogue finishes, overlap with the dX
-            # GEMM"): dW + db first, then the exchange on a side stream WHILE dX runs; joined before the step ends, so the
-            # reduced gradients are complete before the next forward starts
+            # in-step schedule with overlap: dW + db first, then the exchange on a side stream WHILE dX runs; joined
+            # before the step ends, so the reduced gradients are complete before the next forward starts
             ops.fused_bwd(dz, s['x'], s['w'], gout, dt, colsum, need_dx=False, dW=s['dW'], wscratch=s['wscratch'], db=s['db'],
                           dw_prezeroed=prez)
             ev = torch.cuda.Event()
@@ -456,7 +467,7 @@ def run_ours(args):
                     do_exchange(side_stream)
                 do_dx()
             torch.cuda.current_stream(dev).wait_stream(side_stream)
-            last['loss'] = loss
+            last['loss'] = s['loss'] = loss
             return loss
         ops.fused_bwd(dz, s['x'], s['w'], gout, dt, colsum, dW=s['dW'], dX=s['dX'], wscratch=s['wscratch'],
                       db=s['db'], dw_prezeroed=prez)
@@ -477,12 +488,13 @@ def run_ours(args):
             ev.record(torch.cuda.current_stream(dev))
             comm_stream.wait_event(ev)
             nat.check(nat.lib().bags_debug_spin(fake[0], fake[1], fake[2], comm_stream.cuda_stream), 'bags_debug_spin')
-        last['loss'] = loss
+        last['loss'] = s['loss'] = loss
         return loss
 
-    # sampler, fused fwd (or GEMM + grouped CE), merged backward (preparation jobs + dW + dX units in one launch)
-    kernels_per_step = (4 if args.unfused else 3) + (1 if world > 1 and sets[0].get('bucket') is not None else 0) + (
-        1 if args.exchange == 'instep-overlap-dx' else 0)   # split schedule: the backward is two launches (dW+db, dX)
+    # sampler, fused fwd (or GEMM + grouped CE), backward preparation, merged backward (dW + dX units in one launch).
+    # Split schedule: dW + db alone (nothing left to prepare with the forward's column sums), then preparation + dX.
+    kernels_per_step = (5 if args.unfused else 4) + (1 if world > 1 and sets[0].get('bucket') is not None else 0) + (
+        1 if args.exchange == 'instep-overlap-dx' else 0)
 
     stream = torch.cuda.Stream(device=dev)
     comm_stream = torch.cuda.Stream(device=dev) if (world > 1 and args.exchange == 'overlap-next-step') else None
@@ -547,6 +559,8 @@ def run_ours(args):
             dist.barrier()
         ms_total = e0.elapsed_time(e1)
         ms_step = ms_total / args.steps
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, sets[(args.steps - 1) % pool])
         if world > 1:
             t = torch.tensor([ms_step], device=dev)
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -853,15 +867,26 @@ def run_ours(args):
             kernel_us['bwd_dX_only'] = graphed(lambda s: ops.fused_bwd(dzs[idx[id(s)]], s['x'], s['w'], gout, dt, None,
                                                                        need_dw=False, need_db=False, dX=s['dX'],
                                                                        wscratch=s['wscratch2']))
-            kernel_us['bwd_merged(prep+dW+dX)'] = graphed(lambda s: ops.fused_bwd(dzs[idx[id(s)]], s['x'], s['w'], gout, dt,
-                                                                                  None, dW=s['dW'], dX=s['dX'],
-                                                                                  wscratch=s['wscratch'], db=s['db']))
+            def full_bwd(s):
+                ops.fused_bwd(dzs[idx[id(s)]], s['x'], s['w'], gout, dt, None, dW=s['dW'], dX=s['dX'],
+                              wscratch=s['wscratch'], db=s['db'])
+            kernel_us['bwd(prep+merged)'] = graphed(full_bwd)
+            # the same backward as three launches (preparation, split-K dW, dX): what the merged kernel replaces
+            from balancedgroupsoftmax_b200 import _native as nat_
+            os.environ['BAGS_BWD_MERGED'] = '0'
+            nat_.reload_env()
+            try:
+                kernel_us['bwd(prep+dW+dX)'] = graphed(full_bwd)
+            finally:
+                os.environ.pop('BAGS_BWD_MERGED')
+                nat_.reload_env()
             kernel_us['sample_others'] = graphed(lambda s: ops.sample_others(s['labels'], dt, RATIO, 7))
         except Exception as ex:  # pragma: no cover
             log('per-kernel timing failed: %r' % (ex,))
         TF = dtype != torch.bfloat16
         flops = {'fc_cls_gemm': 2.0 * n * K_FEAT * C, 'fused_fwd': 2.0 * n * K_FEAT * C, 'bwd_dW_db_only': 2.0 * n * K_FEAT * C,
-                 'bwd_dX_only': 2.0 * n * K_FEAT * C, 'bwd_merged(prep+dW+dX)': 4.0 * n * K_FEAT * C}
+                 'bwd_dX_only': 2.0 * n * K_FEAT * C, 'bwd(prep+merged)': 4.0 * n * K_FEAT * C,
+                 'bwd(prep+dW+dX)': 4.0 * n * K_FEAT * C}
         bytes_ce = n * C * 4 + n * C * elt + n * 8 + dt.G * n   # read fp32 logits, write dz, labels, masks
         # Isolated kernel timings (a few hundred microseconds of launches at full clocks) are judged against the BURST
         # cuBLAS figure of MEASURED_PEAKS.json; the whole step, timed inside a seconds-long loop, against the SUSTAINED
@@ -876,16 +901,15 @@ def run_ours(args):
                 return {'kernel': name, 'bound': 'tensor', 'achieved': ach, 'peak': pk_burst, 'unit': 'TFLOP/s',
                         'frac': ach / pk_burst, 'frac_of_sustained_peak': ach / pk_sust, 'peak_sustained': pk_sust,
                         'kernel_us': kernel_us[name], 'algorithmic_flops': flops[name],
-                        'traffic': (ncu_traffic(name) if n == N_ROIS and not TF else None),
-                        'peak_source': psrc + ' (burst: the kernel is timed alone)'}
-            step_kernels = [k_ for k_ in ('fused_fwd', 'fc_cls_gemm', 'group_ce', 'bwd_merged(prep+dW+dX)') if k_ in kernel_us]
+                                                'peak_source': psrc + ' (burst: the kernel is timed alone)'}
+            step_kernels = [k_ for k_ in ('fused_fwd', 'fc_cls_gemm', 'group_ce', 'bwd(prep+merged)') if k_ in kernel_us]
             dom = max(step_kernels, key=lambda k_: kernel_us[k_])
             if dom in flops:
                 roof = tensor_roof(dom)
             else:
                 ach = bytes_ce / (kernel_us[dom] * 1e-6) / 1e9
                 roof = {'kernel': dom, 'bound': 'hbm', 'achieved': ach, 'peak': pk['hbm_gbs'], 'unit': 'GB/s',
-                        'frac': ach / pk['hbm_gbs'], 'traffic': ncu_traffic(dom), 'peak_source': pk['source'],
+                        'frac': ach / pk['hbm_gbs'], 'peak_source': pk['source'],
                         'algorithmic_bytes': bytes_ce}
             cands = [tensor_roof(k_) for k_ in step_kernels if k_ in flops]
             if cands:
@@ -915,7 +939,7 @@ def run_ours(args):
                             '5 bins, %s operands, dW+db+dX, device sampler, %s forward' % (n, K_FEAT, NUM_CLASSES, C, args.dtype,
                                                                                     'unfused' if args.unfused else 'fused'),
                 'rois_per_gpu': n, 'parallelism': 'dp%d' % world,
-                'l2': 'rotating pool of %d buffer sets (%.0f MB > 126 MB L2); no step re-reads cached inputs'
+                'l2': 'rotating pool of %d buffer sets (%.0f MB > 50 MB L2); no step re-reads cached inputs'
                       % (pool, pool * per_set / 1e6),
                 'launch': 'cuda-graph replay' if graph is not None else 'eager',
                 'collective': 'none' if world == 1 else (
@@ -985,7 +1009,9 @@ def main():
     ap.add_argument('--e2e-eager-only', action='store_true', help='e2e leg: eager autograd calls only (no CUDA-graph step)')
     ap.add_argument('--unfused', action='store_true', help='GEMM -> fp32 logits -> grouped CE instead of the fused kernel')
     ap.add_argument('--no-library-baseline', action='store_true', help='skip the torch/cuBLAS same-GPU baseline leg')
-    ap.add_argument('--profile', action='store_true', help='timed loop only (for ncu): skip e2e / cpu / per-kernel legs')
+    ap.add_argument('--profile', action='store_true', help='timed loop only: skip e2e / cpu / per-kernel legs')
+    ap.add_argument('--dump-outputs', default='', metavar='DIR',
+                    help='after the timed steps, write the last step\'s losses, dW, db and dX to DIR/<name>.npy (float32)')
     args = ap.parse_args()
     if args.impl == 'reference':
         args.steps = args.steps or 20
@@ -995,7 +1021,7 @@ def main():
     args.warmup = 20 if args.warmup is None else args.warmup
     if args.exchange is None:
         # N > 1: the exchange inside the step, overlapped by the dX contraction (the product's data-parallel schedule);
-        # one GPU: the merged backward (nothing to exchange)
+        # one GPU: preparation + the merged backward (nothing to exchange)
         args.exchange = 'instep-overlap-dx' if int(os.environ.get('WORLD_SIZE', '1')) > 1 else 'instep'
     if args.prep is None:
         # split schedule: the dW + db launch sits on the critical path before the exchange -> nothing left to prepare there

@@ -1,5 +1,5 @@
 /*
- * bags_b200.h -- C ABI of the B200-native Balanced Group Softmax (BAGS) RoI
+ * bags_b200.h -- C ABI of the H100-native Balanced Group Softmax (BAGS) RoI
  * classification head hot path.
  *
  * This is the drop-in boundary for the reference's fc_cls -> grouped softmax /
@@ -42,7 +42,7 @@
  *   - `stream` is a cudaStream_t passed as void*
  *   - slices_host is int32 [G,2] = (start, len) per bin, ascending and non-overlapping
  *     (tools/lvis_analyse.py:45-50), G <= BAGS_MAX_BINS
- *   - requires an sm_100 (B200) device; there is no CPU or other-arch fallback
+ *   - requires an sm_90 (H100) device; there is no CPU or other-arch fallback
  */
 #ifndef BAGS_B200_H_
 #define BAGS_B200_H_
@@ -62,7 +62,7 @@ extern "C" {
 #define BAGS_OK 0
 #define BAGS_ERR_INVALID (-1)   /* bad argument / unsupported shape */
 #define BAGS_ERR_CUDA (-2)      /* CUDA runtime / driver error */
-#define BAGS_ERR_ARCH (-3)      /* device is not sm_100 */
+#define BAGS_ERR_ARCH (-3)      /* device is not sm_90 */
 
 int bags_abi_version(void);
 const char* bags_last_error(void);
@@ -102,11 +102,11 @@ int bags_group_ce(const float* logits, long long ldz, const int64_t* labels,
                   size_t workspace_bytes, void* stream);
 
 /* 1 if bags_fwd can run its fused kernel (logits == NULL) for this bin table: C <= 1280, G <= 6, C % 4 == 0,
- * bins tile [0, C) contiguously and no 16-column chunk intersects more than two bins. */
+ * bins tile [0, C) contiguously. */
 int bags_fused_eligible(const int32_t* slices_host, int G, int C);
 
 /* fc_cls + grouped softmax-CE (+ dz, colsum) in one call.
- *   logits == NULL : fused kernel -- the logits stay in tensor memory and never reach HBM
+ *   logits == NULL : fused kernel -- the logits stay in registers and never reach HBM
  *                    (requires bags_fused_eligible); ldz is ignored.
  *   logits != NULL : bags_linear_fwd into `logits` followed by bags_group_ce (same arguments).
  * colsum (optional) is [colsum_tiles, C] with colsum_tiles = ceil(N/128): per-128-row-tile partial column sums
@@ -222,7 +222,7 @@ int bags_debug_spin(int blocks, int threads, int micros, void* stream);
 int bags_debug_max_clusters(int cluster, int threads, int smem_bytes);
 
 /* The head's trunk, the step before the path (SURVEY.md 8f-3; convfc_bbox_head.py:138-143 shared FCs + ReLU, :167 fc_reg):
- * out[N,C] = act(x[N,K] W[C,K]^T + bias), act = ReLU when relu != 0, on the tcgen05 GEMM of bags_linear_fwd.
+ * out[N,C] = act(x[N,K] W[C,K]^T + bias), act = ReLU when relu != 0, on the wgmma GEMM of bags_linear_fwd.
  * dtype = operand dtype of x and W; out_dtype: BAGS_DTYPE_F32, or BAGS_DTYPE_BF16 (bf16 operands only: feeds the next layer). */
 int bags_linear_act_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
                         void* out, long long ldo, int N, int K, int C, int dtype, int out_dtype, int relu,
@@ -245,16 +245,15 @@ int bags_act_bwd(const void* dy, long long lddy, int dy_dtype, const void* y, lo
 int bags_cast_bf16(const float* src, long long lds, void* dst, long long ldd, int rows, int cols,
                    void* stream);
 
-/* Test hook: one tcgen05 GEMM, out[M,N] = A * B^T with either operand K-major ([rows,K]) or
- * MN-major ([K,rows]).  epi: 0 = fp32 store, 1 = bf16 store, 2 = fp32 reduce-add (split-K).
- * block_n in {256, 320}; 320 only with K-major B and epi 0. */
+/* Test hook: one wgmma GEMM, out[M,N] = A * B^T with either operand K-major ([rows,K]) or
+ * MN-major ([K,rows]).  epi: 0 = fp32 store, 1 = bf16 store, 2 = fp32 reduce-add (split-K).  block_n = 256. */
 int bags_gemm_probe(const void* a, long long lda, int a_mn, const void* b, long long ldb, int b_mn,
                     void* out, long long ldo, int M, int N, int K, int dtype, int block_n,
                     int splits, int epi, void* stream);
 
-/* Test hook: point the tcgen05 kernels at a device buffer of [ctas][8] int64 that they stamp with
- * %globaltimer values (0 start, 1 setup done, 2 first operands landed, 3..6 phase ends, 7 SM id).
- * NULL (the default) disables it.  Not thread-safe; for profiling only. */
+/* Test hook: point the gradient-exchange kernel (bags_grad_allreduce) at a device buffer of int64 %globaltimer
+ * stamps; it writes [blocks][8] slots starting at row 4096 of the buffer.  The GEMM and fused-forward kernels do
+ * not stamp it.  NULL (the default) disables it.  Not thread-safe; for profiling only. */
 int bags_debug_set_timing(void* dev_ptr);
 
 /* The library reads its tuning / experiment switches (BAGS_* environment variables) once per name and caches them;

@@ -15,10 +15,10 @@ algorithm for the path, function by function:
   weight_reduce_loss      mmdet/models/losses/utils.py:26-53
   bags_loss               gs_bbox_head_with0.py:147-171
   merge_score             gs_bbox_head_with0.py:239-273
-  closed_form_grads       what autograd produces for the above (SURVEY.md appendix A)
+  closed_form_grads       what autograd produces for the above
 
 Parity pinning: the reference ships no tests / golden vectors for this path
-(SURVEY.md §4, §8c), so the oracle is pinned against the reference's OWN source
+(, §8c), so the oracle is pinned against the reference's OWN source
 executed in place on CPU through ``oracle/ref_shim.py`` (tests/test_oracle_vs_reference.py,
 run wherever /root/reference is reachable) and against the committed fixtures in
 ``tests/golden/`` that the same shim generated (tests/golden/make_golden.py).
@@ -212,7 +212,7 @@ def head_step(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, labels:
 
 
 # ---------------------------------------------------------------------------------------------------
-# test-time consumer of the merged scores (SURVEY.md 8f-2): per-class NMS
+# test-time consumer of the merged scores: per-class NMS
 # ---------------------------------------------------------------------------------------------------
 def nms_plus1(dets: torch.Tensor, iou_thr: float) -> Tuple[torch.Tensor, torch.Tensor]:
     """Greedy NMS with the reference op's conventions (mmdet/ops/nms/src/nms_kernel.cu:13-21,60,76-78): boxes visited

@@ -3,7 +3,7 @@ oracle/ref_shim.py) on CPU.  Run in the build container where /root/reference ex
 
     python tests/golden/make_golden.py
 
-The reference ships no golden vectors for this path (SURVEY.md §4/§8c); these fixtures are the
+The reference ships no golden vectors for this path; these fixtures are the
 pinning: inputs + the reference's outputs (per-bin losses, sampled masks, avg factors, grads,
 merged scores).  They travel to the GPU box, where /root/reference does not exist.
 

@@ -195,7 +195,7 @@ def case_fused(name):
 
 
 def case_fusedk(name):
-    """fused forward kernel (logits stay in TMEM) vs the oracle, incl. ragged N and lse output"""
+    """fused forward kernel (logits stay on chip) vs the oracle, incl. ragged N and lse output"""
     np, torch, ops, _, O = _setup()
     _, dts = name.split('.')
     cdt = torch.bfloat16 if dts == 'bf16' else torch.float32
@@ -232,173 +232,6 @@ def case_fusedk(name):
         for k_, v in res.items():
             assert v < tol[k_], (N, k_, v, tol[k_])
     return out
-
-
-def case_timeline(name):
-    """per-CTA %globaltimer stamps of the tcgen05 kernels at the benchmark shape"""
-    np, torch, ops, _, O = _setup()
-    from balancedgroupsoftmax_b200 import _native as nat
-    N = 4096
-    t, x, W, b, labels, l2b, ps, remapped = _problem(N)
-    dt = ops.DeviceTables.from_tables(t, 'cuda')
-    xc, wc = x.cuda().bfloat16(), W.cuda().bfloat16()
-    bc, lc = b.cuda(), labels.cuda()
-    wmask, avg = ops.sample_others(lc, dt, 8.0, 1)
-    logits = torch.empty(N, t.num_logits, device='cuda')
-    tbuf = torch.zeros(4096, 8, dtype=torch.int64, device='cuda')
-    res = {}
-
-    def run(label, fn, nctas):
-        for _ in range(3):
-            fn()
-        torch.cuda.synchronize()
-        tbuf.zero_()
-        nat.check(nat.lib().bags_debug_set_timing(tbuf.data_ptr()), 'set_timing')
-        fn()
-        torch.cuda.synchronize()
-        nat.check(nat.lib().bags_debug_set_timing(None), 'set_timing')
-        off = 2048 if 'bwd_merged' in label else 0   # the merged backward stamps rows [2048, ..)
-        tb = tbuf[off:off + nctas].cpu().double()
-        tb = tb[tb[:, 0] > 0]   # the grid may be smaller than nctas (e.g. 144 units of 256 x 256)
-        if 'bwd_merged' in label and os.environ.get('BAGS_BWD_PAIR') == '1':
-            tb = tb[0::2]   # only the leader CTA of a pair stamps the MMA slots
-        t0 = tb[:, 0].min()
-        end = tb[:, 6].max()
-        d = {}
-        d['kernel_span_us'] = float((end - t0) / 1e3)
-        d['cta_start_skew_us'] = float((tb[:, 0].max() - t0) / 1e3)
-        names = ['start', 'setup', 'first_data', 's3', 's4', 's5', 'end']
-        for i in range(1, 7):
-            seg = (tb[:, i] - tb[:, i - 1]) / 1e3
-            d['%s->%s_us(mean,max)' % (names[i - 1], names[i])] = [round(float(seg.mean()), 2), round(float(seg.max()), 2)]
-        d['cta_life_us(mean,max)'] = [round(float(((tb[:, 6] - tb[:, 0]) / 1e3).mean()), 2),
-                                      round(float(((tb[:, 6] - tb[:, 0]) / 1e3).max()), 2)]
-        d['distinct_sms'] = int(tb[:, 7].unique().numel())
-        d['ctas'] = int(tb.shape[0])
-        if 'bwd_merged' in label and tb.shape[0] > 64 and os.environ.get('BAGS_BWD_PAIR') != '1':
-            # 256 x 256 units, one per CTA: the last 64 CTAs run dX units (20 k-blocks), the others dW units
-            ndw = tb.shape[0] - 64
-            for kind, sub in (('dW', tb[:ndw]), ('dX', tb[ndw:])):
-                d['%s_units' % kind] = {
-                    'ctas': int(sub.shape[0]),
-                    'start->first_data': round(float(((sub[:, 2] - sub[:, 0]) / 1e3).mean()), 2),
-                    'mainloop(first_data->acc_done)': [round(float(((sub[:, 4] - sub[:, 2]) / 1e3).mean()), 2),
-                                                       round(float(((sub[:, 4] - sub[:, 2]) / 1e3).max()), 2)],
-                    'epilogue(acc_done->epi_done)': [round(float(((sub[:, 5] - sub[:, 4]) / 1e3).mean()), 2),
-                                                     round(float(((sub[:, 5] - sub[:, 4]) / 1e3).max()), 2)],
-                    'end_after_kernel_start': [round(float(((sub[:, 6] - t0) / 1e3).mean()), 2),
-                                               round(float(((sub[:, 6] - t0) / 1e3).max()), 2)]}
-        if 'fused' in label:   # second stamp bank: finer epilogue phases (us after 'acc done')
-            t2 = tbuf[nctas:2 * nctas].cpu().double()
-            base = tb[:, 3]
-            nm = ['A_loop(w2)', 'A_allwarps', 'C_start', 'C_loop(w2)', 'C_allwarps', 'cta_done', 'A_loop(w17)', 'C_loop(w17)']
-            d['fine_us_after_acc_done(mean)'] = {nm[i]: round(float(((t2[:, i] - base) / 1e3).mean()), 2) for i in range(8)}
-            d['coarse_us_after_acc_done(mean)'] = {'passA(s4)': round(float(((tb[:, 4] - base) / 1e3).mean()), 2),
-                                                   'xchg(s5)': round(float(((tb[:, 5] - base) / 1e3).mean()), 2),
-                                                   'passC(s6)': round(float(((tb[:, 6] - base) / 1e3).mean()), 2)}
-            t3 = tbuf[2 * nctas:3 * nctas].cpu().double()
-            c0 = t2[:, 2]   # pass C start
-            for r in (0, 2):
-                d['passC_w2_rank%d_us_after_C_start' % r] = {
-                    'start_bin0': round(float(((t3[r::4, 6] - c0[r::4]) / 1e3).mean()), 2),
-                    **{'chunk%d' % i: round(float(((t3[r::4, i] - c0[r::4]) / 1e3).mean()), 2) for i in range(5)}}
-            for r in range(4):
-                d['fine_rank%d' % r] = {nm[i]: round(float(((t2[r::4, i] - base[r::4]) / 1e3).mean()), 2) for i in range(8)}
-        if 'fused' in label:   # per cluster-rank means of pass A / barrier / pass C
-            for r in range(4):
-                sub = tb[r::4]
-                d['rank%d(passA,bar,passC)' % r] = [round(float(((sub[:, 4] - sub[:, 3]) / 1e3).mean()), 2),
-                                                    round(float(((sub[:, 5] - sub[:, 4]) / 1e3).mean()), 2),
-                                                    round(float(((sub[:, 6] - sub[:, 5]) / 1e3).mean()), 2)]
-        res[label] = d
-
-    run('gemm_fwd_320 (s3=mma issued, s4=acc done, s5=epi done)',
-        lambda: ops.linear_fwd(xc, wc, bc, out=logits), 128)
-    loss, _, _, dz, colsum = ops.fused_fwd(xc, wc, bc, lc, dt, wmask, avg, logits=logits)
-    dW = torch.empty(t.num_logits, 1024, device='cuda')
-    dX = torch.empty(N, 1024, device='cuda', dtype=torch.bfloat16)
-    run('gemm_dX_256', lambda: ops.fused_bwd(dz, xc, wc, None, dt, colsum, need_dw=False, need_db=False, dX=dX), 128)
-    run('gemm_dW_256_split3', lambda: ops.fused_bwd(dz, xc, wc, None, dt, colsum, need_dx=False, dW=dW), 120)
-    ws = ops.bwd_scratch(wc)
-    gout = torch.ones(5, device='cuda')
-    run('bwd_merged (s2=first data, s3=unit0 mma issued, s4=unit0 acc done, s5=unit0 epi done)',
-        lambda: ops.fused_bwd(dz, xc, wc, gout, dt, colsum, dW=dW, dX=dX, wscratch=ws), 148)
-    run('fused_fwd (s3=acc done, s4=passA, s5=xchg barrier, end=passC...)',
-        lambda: ops.fused_fwd(xc, wc, bc, lc, dt, wmask, avg), 128)
-    return res
-
-
-def case_steptimeline(name):
-    """absolute %globaltimer picture of consecutive training steps replayed from one CUDA graph (bench.py's loop):
-    when do the forward / backward CTAs of step i start and end relative to each other"""
-    np, torch, ops, _, O = _setup()
-    from balancedgroupsoftmax_b200 import _native as nat
-    N, POOL = 4096, 5
-    t, x, W, b, labels, l2b, ps, remapped = _problem(N)
-    dt = ops.DeviceTables.from_tables(t, 'cuda')
-    g = torch.Generator().manual_seed(1)
-    sets = []
-    for i in range(POOL):
-        s = dict(x=torch.relu(torch.randn(N, 1024, generator=g)).cuda().bfloat16(), w=W.cuda().bfloat16(), bias=b.cuda(),
-                 labels=labels.cuda(), dW=torch.empty(t.num_logits, 1024, device='cuda'),
-                 db=torch.empty(t.num_logits, device='cuda'), dX=torch.empty(N, 1024, device='cuda', dtype=torch.bfloat16),
-                 tb=torch.zeros(4096, 8, dtype=torch.int64, device='cuda'))
-        s['ws'] = ops.bwd_scratch(s['w'])
-        sets.append(s)
-    gout = torch.ones(5, device='cuda')
-    seed = [0]
-
-    def step(s, timed):
-        seed[0] += 1
-        if timed:
-            nat.check(nat.lib().bags_debug_set_timing(s['tb'].data_ptr()), 'set_timing')
-        wmask, avg = ops.sample_others(s['labels'], dt, 8.0, seed[0])
-        loss, _, _, dz, colsum = ops.fused_fwd(s['x'], s['w'], s['bias'], s['labels'], dt, wmask, avg)
-        ops.fused_bwd(dz, s['x'], s['w'], gout, dt, colsum, dW=s['dW'], dX=s['dX'], wscratch=s['ws'], db=s['db'])
-
-    stream = torch.cuda.Stream()
-    with torch.cuda.stream(stream):
-        for s in sets[:2]:
-            step(s, False)
-        stream.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph, stream=stream):
-            for s in sets:
-                step(s, True)    # every step's launches capture their own stamp buffer
-        nat.check(nat.lib().bags_debug_set_timing(None), 'set_timing')
-        for _ in range(6):
-            graph.replay()
-        stream.synchronize()
-    res = {}
-    t0 = None
-    rows = []
-    for i, s in enumerate(sets):
-        tb = s['tb'].cpu().double()
-        f = tb[:128]
-        bw = tb[2048:2048 + 148]
-        bw = bw[bw[:, 0] > 0]
-        if t0 is None:
-            t0 = f[:, 0].min()
-        us = lambda v: round(float((v - t0) / 1e3), 2)
-        rows.append(dict(step=i,
-                         fwd_first_cta_start=us(f[:, 0].min()), fwd_median_cta_start=us(f[:, 0].median()),
-                         fwd_last_cta_start=us(f[:, 0].max()),
-                         fwd_first_acc_done=us(f[:, 3].min()), fwd_last_acc_done=us(f[:, 3].max()),
-                         fwd_first_exchange_done=us(f[:, 5].min()), fwd_last_exchange_done=us(f[:, 5].max()),
-                         fwd_first_end=us(f[:, 6].min()), fwd_last_end=us(f[:, 6].max()),
-                         bwd_first_cta_start=us(bw[:, 0].min()), bwd_last_cta_start=us(bw[:, 0].max()),
-                         bwd_median_first_data=us(bw[:, 2].median()), bwd_last_first_data=us(bw[:, 2].max()),
-                         bwd_first_end=us(bw[:, 6].min()), bwd_median_end=us(bw[:, 6].median()), bwd_last_end=us(bw[:, 6].max())))
-    res['steps'] = rows
-    res['period_us(bwd_last_end deltas)'] = [round(rows[i + 1]['bwd_last_end'] - rows[i]['bwd_last_end'], 2) for i in range(POOL - 1)]
-    # how many forward CTAs of step i+1 started before the backward of step i had finished
-    early = []
-    for i in range(POOL - 1):
-        fe = sets[i + 1]['tb'][:128, 0].cpu().double()
-        be = sets[i]['tb'][2048:2048 + 148, 6].cpu().double().max()   # (unused rows are zero)
-        early.append(int((fe < be).sum()))
-    res['fwd_ctas_started_before_prev_bwd_end'] = early
-    return res
 
 
 def case_timing(name):
@@ -474,11 +307,11 @@ def case_timing(name):
 
 CASES = {
     'group_ce': case_group_ce, 'sampler': case_sampler, 'merge': case_merge,
-    'gemm.kk256.bf16': case_gemm, 'gemm.kk320.bf16': case_gemm, 'gemm.kmn.bf16': case_gemm,
+    'gemm.kk256.bf16': case_gemm, 'gemm.kmn.bf16': case_gemm,
     'gemm.mnmn.bf16': case_gemm,
-    'gemm.kk256.f32': case_gemm, 'gemm.kk320.f32': case_gemm, 'gemm.kmn.f32': case_gemm, 'gemm.mnmn.f32': case_gemm,
+    'gemm.kk256.f32': case_gemm, 'gemm.kmn.f32': case_gemm, 'gemm.mnmn.f32': case_gemm,
     'fused.bf16': case_fused, 'fused.f32': case_fused, 'fusedk.bf16': case_fusedk, 'fusedk.f32': case_fusedk,
-    'timeline': case_timeline, 'steptimeline': case_steptimeline, 'timing': case_timing,
+    'timing': case_timing,
 }
 
 

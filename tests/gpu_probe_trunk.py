@@ -1,4 +1,4 @@
-"""Timing of the head's trunk layers (SURVEY.md 8f-3) on this library's tcgen05 GEMMs vs torch (cuBLAS) on the same GPU:
+"""Timing of the head's trunk layers on this library's tcgen05 GEMMs vs torch (cuBLAS) on the same GPU:
 python tests/gpu_probe_trunk.py    -> one JSON line (CUDA events, rotating buffers > L2 are not needed: the 25 MB weight of
 shared_fcs.0 plus activations are re-read from L2 / HBM alike in both arms)."""
 import json

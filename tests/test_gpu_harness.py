@@ -1,4 +1,4 @@
-"""GPU: the detector harness end to end (SURVEY.md §8f-1) -- frozen torchvision trunk -> RoI sampling -> BAGS head(s)
+"""GPU: the detector harness end to end -- frozen torchvision trunk -> RoI sampling -> BAGS head(s)
 forward / get_target / loss / backward -> SGD step, at a small image size; losses finite, head gradients non-zero."""
 import math
 

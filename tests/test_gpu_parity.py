@@ -1,11 +1,11 @@
-"""GPU parity tests (run with ``-m gpu`` on a B200): the CUDA path, called through the C ABI
+"""GPU parity tests (run with ``-m gpu`` on an H100): the CUDA path, called through the C ABI
 (balancedgroupsoftmax_b200.ops -> ctypes -> libbags_b200.so), against
 
   * the committed golden fixtures produced by the reference's own code (tests/golden/),
   * the CPU oracle on the same seeded inputs at sizes the oracle finishes in seconds,
   * size-independent properties at the full benchmark size (4096 RoIs).
 
-Tolerances (stated per SURVEY.md §8c / BASELINE.json north_star):
+Tolerances:
   integer outputs (in-bin labels, masks given as input, avg factors, argmax ids) .. bit-exact
   fp32 mode (fp32 operands, TF32 tensor-core products, fp32 accumulate) ........... loss rel <= 1e-3,
                                                               dW/db/dX Frobenius-rel <= 1e-3 vs the fp32 reference
@@ -71,7 +71,7 @@ def test_golden_fixture_through_c_abi(env, path, mode):
     tol = TOL[mode]
     ref_loss = d['losses']
     assert ops.fused_eligible(dt)
-    # route 1: fused kernel (logits never leave tensor memory); route 2: GEMM -> fp32 logits -> grouped CE
+    # route 1: fused kernel (logits never leave the chip); route 2: GEMM -> fp32 logits -> grouped CE
     for materialize in (False, True):
         loss, logits, lse, dz, colsum = ops.fused_fwd(x, W, b, labels, dt, wmask, avg, want_lse=True,
                                                       materialize=materialize)
@@ -161,7 +161,7 @@ def test_uniform_upstream_gradients_skip_the_scaled_weight_copy(env, mode, gval)
     avg = ops.mask_avg(wmask)
     xc, wc = x.cuda().to(mode), W.cuda().to(mode)
     loss, _, _, dz, _ = ops.fused_fwd(xc, wc, b.cuda(), labels.cuda(), dt, wmask, avg)
-    for _ in range(2):   # twice: the in-kernel grid counters must be left re-armed
+    for _ in range(2):   # twice: the second call must not depend on state the first one left
         dW, db, dX = ops.fused_bwd(dz, xc, wc, torch.tensor(gout, device='cuda'), dt, None)
     torch.cuda.synchronize()
     tol = TOL[mode]
@@ -388,15 +388,15 @@ def test_device_sampler_module_path_and_cascade_weights(env):
 
 
 # --------------------------------------------------------------------------------------------------------------
-# BASELINE config 2 (4096 RoIs x 1024 x 1236) against the oracle itself -- the shape bench.py times, i.e. the
-# 256 x 256-unit (MT = 2) instantiation of the merged backward, plus the unit-size switch boundary and a ragged N.
+# The benchmark configuration (4096 RoIs x 1024 x 1236) against the oracle itself -- the shape bench.py times -- plus
+# neighbouring and ragged N.
 # Reference to match: gs_bbox_head_with0.py:147-171 + autograd (dist_utils.py:53).
 # --------------------------------------------------------------------------------------------------------------
 GOUTS = {'uniform': [1.0] * 5, 'cascade': [0.5] * 5, 'nonuniform': [1.0, 0.5, 0.25, 2.0, 1.5]}
 
 
 def _check_vs_oracle(ops, dt, l2b, ps, x, W, b, labels, remapped, mode, gout, loss, dW, db, dX):
-    """fp32 mode: the SURVEY 8c tolerances vs the fp32 oracle.  bf16 mode: those of TOL vs the fp32 oracle AND the tight
+    """fp32 mode: the TOL tolerances vs the fp32 oracle.  bf16 mode: those of TOL vs the fp32 oracle AND the tight
     ones vs the oracle fed the same bf16-rounded operands."""
     tol = TOL[mode]
     ref = O.bags_loss(O.fc_cls(x, W, b), labels, l2b, ps, remapped=remapped)
@@ -444,13 +444,14 @@ def test_config2_full_size_vs_oracle(env, N, mode, gname):
     _check_vs_oracle(ops, dt, l2b, ps, x, W, b, labels, remapped, mode, gout, loss, dW, db, dX)
 
 
-@pytest.mark.parametrize('mt', ['1', '2'])
+@pytest.mark.parametrize('splits', ['1', '5'])
 @pytest.mark.parametrize('N', [512, 4096])
-def test_backward_unit_size_forced(env, monkeypatch, N, mt):
-    """Both unit sizes of the merged backward (BAGS_BWD_MT) at a small and at the benchmark size."""
+def test_backward_dw_splits_forced(env, monkeypatch, N, splits):
+    """The merged backward with its dW units forced to one split (plain red.add of whole-K tiles) and to five (more dW
+    than dX units in the work list), at a small and at the benchmark size."""
     ops, t, dt, l2b, ps = env
     from balancedgroupsoftmax_b200 import _native
-    monkeypatch.setenv('BAGS_BWD_MT', mt)
+    monkeypatch.setenv('BAGS_DW_SPLITS', splits)
     _native.reload_env()
     try:
         x, W, b, labels, remapped = _problem(N, seed=7 + N)
@@ -463,7 +464,7 @@ def test_backward_unit_size_forced(env, monkeypatch, N, mt):
         torch.cuda.synchronize()
         _check_vs_oracle(ops, dt, l2b, ps, x, W, b, labels, remapped, torch.bfloat16, gout, loss, dW, db, dX)
     finally:
-        monkeypatch.delenv('BAGS_BWD_MT')
+        monkeypatch.delenv('BAGS_DW_SPLITS')
         _native.reload_env()
 
 
@@ -506,7 +507,7 @@ def test_graphed_step_config2_vs_oracle(env, need_dx):
 @pytest.mark.parametrize('N', [512, 4096])
 def test_split_backward_matches_oracle(env, N, mode, gname):
     """The two launches of the in-step exchange schedule (dW + db first, then dX while the gradients travel): each half
-    alone runs on the merged kernel (no dX units / no dW units) and must give the oracle's gradients."""
+    alone runs as a plain GEMM (with the preparation kernel where it has work) and must give the oracle's gradients."""
     ops, t, dt, l2b, ps = env
     x, W, b, labels, remapped = _problem(N, seed=55 + N)
     gout = GOUTS[gname]
@@ -515,7 +516,7 @@ def test_split_backward_matches_oracle(env, N, mode, gname):
     xc, wc = x.cuda().to(mode), W.cuda().to(mode)
     loss, _, _, dz, _ = ops.fused_fwd(xc, wc, b.cuda(), labels.cuda(), dt, wmask, avg)
     g = torch.tensor(gout, device='cuda')
-    for _ in range(2):   # twice: the library-owned grid counters must be left re-armed by either half
+    for _ in range(2):   # twice: the second call must not depend on state the first one left
         dW, db, none_dx = ops.fused_bwd(dz, xc, wc, g, dt, None, need_dx=False)
         none_dw, none_db, dX = ops.fused_bwd(dz, xc, wc, g, dt, None, need_dw=False, need_db=False)
     torch.cuda.synchronize()

@@ -1,4 +1,4 @@
-"""GPU: the head's trunk on this library's tcgen05 GEMMs (SURVEY.md §8f-3) -- shared FCs (Linear + ReLU) and fc_reg
+"""GPU: the head's trunk on this library's wgmma GEMMs -- shared FCs (Linear + ReLU) and fc_reg
 (convfc_bbox_head.py:138-143,167) through LinearActFunction, forward and backward, against plain torch fp32 (the numerics
 reference for a floating-point kernel: fp32 nn.Linear + ReLU + autograd on the CPU)."""
 import pytest

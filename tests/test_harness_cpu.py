@@ -1,5 +1,5 @@
-"""CPU: the detector harness (SURVEY.md §8f-1) up to the head's inputs -- trunk (torchvision, frozen), RoI assignment +
-sampling, RoIAlign features, targets -- i.e. the caller side of the hot path.  The head's loss itself needs a B200."""
+"""CPU: the detector harness up to the head's inputs -- trunk (torchvision, frozen), RoI assignment +
+sampling, RoIAlign features, targets -- i.e. the caller side of the hot path.  The head's loss itself needs an H100."""
 import pytest
 import torch
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Full-detector harness bench (SURVEY.md §8f-1; BASELINE.json configs[2..3] shapes) -- NOT the headline bench.py.
+"""Full-detector harness bench -- NOT the headline bench.py.
 
     python tools/bench_detector.py [--stages 1|3] [--imgs-per-gpu 2] [--steps 20] [--warmup 5]
     python -m torch.distributed.run --nproc-per-node N tools/bench_detector.py ...      (one rank per GPU)
@@ -47,7 +47,7 @@ def main() -> int:
     rank = int(os.environ.get('RANK', '0'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
     if not torch.cuda.is_available():
-        raise SystemExit('bench_detector.py needs a B200 GPU (the BAGS head has no CPU fallback)')
+        raise SystemExit('bench_detector.py needs an H100 GPU (the BAGS head has no CPU fallback)')
     torch.cuda.set_device(local)
     dev = torch.device('cuda', local)
     if world > 1:

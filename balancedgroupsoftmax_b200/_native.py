@@ -15,9 +15,11 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # BAGS_LIB: development hook to A/B two builds of the same ABI inside one GPU session
 LIB_PATH = os.environ.get('BAGS_LIB') or os.path.join(_HERE, 'libbags_b200.so')
 
-ABI_VERSION = 1
+ABI_VERSION = 2
 DTYPE_F32 = 0
 DTYPE_BF16 = 1
+WEIGHTS_U8 = 0
+WEIGHTS_F32 = 1
 MAX_BINS = 8
 
 _lib = None
@@ -30,34 +32,23 @@ SIGNATURES = {
     'bags_abi_version': (_i, []),
     'bags_last_error': (C.c_char_p, []),
     'bags_workspace_bytes': (_sz, []),
-    'bags_linear_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _ll, _i, _i, _i, _i, _vp]),
-    'bags_sample_others': (_i, [_vp, _vp, _i, _i, _i, C.c_double, C.c_uint64, _vp, _vp, _vp]),
-    'bags_sample_others_step': (_i, [_vp, _vp, _i, _i, _i, C.c_double, C.c_uint64, _vp, _vp, _vp, _vp]),
+    'bags_sample_others': (_i, [_vp, _vp, _i, _i, _i, C.c_double, C.c_uint64, _vp, _vp, _vp, _vp]),
     'bags_mask_avg': (_i, [_vp, _i, _i, _vp, _vp]),
-    'bags_group_ce': (_i, [_vp, _ll, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _ll, _i, _vp,
+    'bags_group_ce': (_i, [_vp, _ll, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _ll, _i, _vp,
                            _vp, _sz, _vp]),
     'bags_fused_eligible': (_i, [_vp, _i, _i]),
-    'bags_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _ll,
-                      _vp, _vp, _vp, _ll, _vp, _i, _vp, _sz, _vp]),
-    'bags_fwd_ex': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _ll,
-                         _vp, _vp, _vp, _ll, _vp, _i, _vp, _sz, _vp, _sz, _vp]),
-    'bags_bwd_ex': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _ll, _vp, _sz, _i, _i,
-                         _i, _i, _i, _i, _vp]),
+    'bags_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _ll,
+                      _vp, _vp, _vp, _ll, _vp, _i, _vp, _sz, _vp, _sz, _vp]),
     'bags_reweight': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
-    'bags_fwd_w': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _ll,
-                        _vp, _vp, _vp, _ll, _vp, _i, _vp, _sz, _vp]),
-    'bags_group_ce_w': (_i, [_vp, _ll, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _ll, _i, _vp,
-                             _vp, _sz, _vp]),
     'bags_bwd_scratch_bytes': (_sz, [_i, _ll, _i]),
     'bags_bwd': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _ll, _vp, _sz, _i, _i,
-                      _i, _i, _i, _vp]),
+                      _i, _i, _i, _i, _vp]),
     'bags_merge_scores': (_i, [_vp, _ll, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp]),
     'bags_grad_allreduce_flag_bytes': (_sz, [_i]),
     'bags_grad_allreduce_status_offset': (_ll, [_i]),
     'bags_grad_allreduce': (_i, [_vp, _vp, _ll, _ll, _i, _i, C.c_float, _i, _vp]),
     'bags_class_nms_dense': (_i, [_vp, _i, _vp, _vp, _i, _i, C.c_float, _vp, _vp, _vp]),
     'bags_debug_spin': (_i, [_i, _i, _i, _vp]),
-    'bags_debug_max_clusters': (_i, [_i, _i, _i]),
     'bags_cast_bf16': (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp]),
     'bags_linear_act_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _vp]),
     'bags_linear_act_splits': (_i, [_i, _i, _i, _i]),

@@ -167,12 +167,13 @@ extern "C" int bags_reload_env(void) {
   return BAGS_OK;
 }
 
-// Launch with the programmatic-stream-serialization attribute (PDL): the kernel may begin while its predecessor
-// in the stream is still running; every kernel of this library guards its first access to predecessor-produced
-// data (and its first write) with griddepcontrol.wait, so stream semantics are preserved.
+// Kernel launch.  pdl: with the programmatic-stream-serialization attribute (PDL; BAGS_PDL=0 turns it off), so the
+// kernel may begin while its predecessor in the stream is still running; every kernel of this library guards its
+// first access to predecessor-produced data (and its first write) with griddepcontrol.wait, so stream semantics are
+// preserved.
 template <typename... KArgs, typename... Args>
-static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
-                              Args&&... args) {
+static cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl,
+                          Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -182,7 +183,7 @@ static cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = env_int("BAGS_PDL", 1) ? 1 : 0;
+  cfg.numAttrs = (pdl && env_int("BAGS_PDL", 1)) ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
@@ -228,23 +229,8 @@ static int launch_gemm(const GemmArgs& ga, const DeviceInfo& di, cudaStream_t st
   const int grid = units < di.num_sms ? units : di.num_sms;
 
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(Cfg::NUM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = (pdl && env_int("BAGS_PDL", 1)) ? 1 : 0;
-  BAGS_CUDA(cudaLaunchKernelEx(&cfg, kernel, ta, tb, p));
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, pdl, ta, tb, p));
   return BAGS_OK;
-}
-
-template <int BLOCK_N, bool A_MN, bool B_MN, int EPI, bool TF32, int STAGES>
-static int launch_gemm_pdl(const GemmArgs& ga, const DeviceInfo& di, cudaStream_t stream) {
-  return launch_gemm<BLOCK_N, A_MN, B_MN, EPI, TF32, STAGES>(ga, di, stream, true);
 }
 
 static int pick_splits(int tiles, int kblocks, int num_sms) {
@@ -259,31 +245,8 @@ static int pick_splits(int tiles, int kblocks, int num_sms) {
 // ----------------------------------------------------------------------------
 extern "C" size_t bags_workspace_bytes(void) { return 256 + 4096 * kMaxG * sizeof(float); }
 
-extern "C" int bags_linear_fwd(const void* x, long long ldx, const void* w, long long ldw,
-                               const float* bias, float* out, long long ldo, int N, int K, int C,
-                               int dtype, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  BAGS_REQUIRE(N >= 0 && K >= 1 && C >= 1, "bags_linear_fwd: bad shape N=%d K=%d C=%d", N, K, C);
-  BAGS_REQUIRE(N == 0 || (x && w && out), "bags_linear_fwd: NULL operand");
-  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "bags_linear_fwd: bad dtype %d", dtype);
-  BAGS_REQUIRE(ldx >= K && ldw >= K && ldo >= C, "bags_linear_fwd: leading dimension smaller than row");
-  if (N == 0) return BAGS_OK;
-  DeviceInfo di;
-  if (int rc = device_info(di)) return rc;
-  if (bias != nullptr) BAGS_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "bias must be 16-byte aligned");
-  BAGS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "out must be 16-byte aligned");
-  GemmArgs ga{};
-  ga.a = x; ga.lda = ldx; ga.a_mn = false;
-  ga.b = w; ga.ldb = ldw; ga.b_mn = false;
-  ga.M = N; ga.N = C; ga.K = K; ga.dtype = dtype; ga.splits = 1;
-  ga.p.out = out; ga.p.ldo = ldo; ga.p.bias = bias; ga.p.gscale = nullptr; ga.p.G = 0;
-  ga.p.colsum_in = nullptr; ga.p.colsum_out = nullptr;
-  if (dtype == BAGS_DTYPE_BF16) return launch_gemm<256, false, false, EPI_STORE_F32, false, 4>(ga, di, stream);
-  return launch_gemm<256, false, false, EPI_STORE_F32, true, 4>(ga, di, stream);
-}
-
-// y = act(x W^T + b): the head's shared FCs (ReLU) and fc_reg (identity) on the same wgmma pipeline
-// (convfc_bbox_head.py:138-143,167: nn.Linear + ReLU through cuBLAS / ATen in the reference)
+// y = act(x W^T + b): the head's shared FCs (ReLU), fc_reg and fc_cls (identity) on the same wgmma pipeline
+// (convfc_bbox_head.py:138-143,166-167: nn.Linear + ReLU through cuBLAS / ATen in the reference)
 extern "C" int bags_linear_act_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
                                    void* out, long long ldo, int N, int K, int C, int dtype, int out_dtype, int relu,
                                    void* stream_) {
@@ -297,8 +260,11 @@ extern "C" int bags_linear_act_fwd(const void* x, long long ldx, const void* w, 
   if (N == 0) return BAGS_OK;
   DeviceInfo di;
   if (int rc = device_info(di)) return rc;
-  if (bias != nullptr && out_dtype == BAGS_DTYPE_F32)
-    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "bags_linear_act_fwd: bias must be 16-byte aligned");
+  if (out_dtype == BAGS_DTYPE_F32) {
+    BAGS_REQUIRE(bias == nullptr || (reinterpret_cast<uintptr_t>(bias) & 15) == 0,
+                 "bags_linear_act_fwd: bias must be 16-byte aligned");
+    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "bags_linear_act_fwd: out must be 16-byte aligned");
+  }
   GemmArgs ga{};
   ga.a = x; ga.lda = ldx; ga.a_mn = false;
   ga.b = w; ga.ldb = ldw; ga.b_mn = false;
@@ -389,9 +355,9 @@ extern "C" int bags_act_bwd(const void* dy, long long lddy, int dy_dtype, const 
   return BAGS_OK;
 }
 
-extern "C" int bags_sample_others_step(const int64_t* labels, const int32_t* label2bin, int N, int G,
-                                       int classes, double ratio, uint64_t seed, const uint64_t* seed_step,
-                                       uint8_t* wmask, float* avg, void* stream_) {
+extern "C" int bags_sample_others(const int64_t* labels, const int32_t* label2bin, int N, int G,
+                                  int classes, double ratio, uint64_t seed, const uint64_t* seed_step,
+                                  uint8_t* wmask, float* avg, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   BAGS_REQUIRE(labels && label2bin && wmask && avg, "bags_sample_others: NULL argument");
   BAGS_REQUIRE(G >= 1 && G <= kMaxG && classes >= 1 && N >= 0, "bags_sample_others: bad shape");
@@ -399,16 +365,9 @@ extern "C" int bags_sample_others_step(const int64_t* labels, const int32_t* lab
   const long long* lab = reinterpret_cast<const long long*>(labels);
   const unsigned long long sd = static_cast<unsigned long long>(seed);
   const unsigned long long* st = reinterpret_cast<const unsigned long long*>(seed_step);
-  if (N <= 4096)       BAGS_CUDA(launch_pdl(sample_others_kernel<4>, dim3(G), dim3(1024), 0, stream, lab, label2bin, classes, G, N, ratio, sd, wmask, avg, st));
-  else if (N <= 16384) BAGS_CUDA(launch_pdl(sample_others_kernel<16>, dim3(G), dim3(1024), 0, stream, lab, label2bin, classes, G, N, ratio, sd, wmask, avg, st));
-  else                 BAGS_CUDA(launch_pdl(sample_others_kernel<0>, dim3(G), dim3(1024), 0, stream, lab, label2bin, classes, G, N, ratio, sd, wmask, avg, st));
+  auto kernel = N <= 4096 ? sample_others_kernel<4> : N <= 16384 ? sample_others_kernel<16> : sample_others_kernel<0>;
+  BAGS_CUDA(launch(kernel, dim3(G), dim3(1024), 0, stream, true, lab, label2bin, classes, G, N, ratio, sd, wmask, avg, st));
   return BAGS_OK;
-}
-
-extern "C" int bags_sample_others(const int64_t* labels, const int32_t* label2bin, int N, int G,
-                                  int classes, double ratio, uint64_t seed, uint8_t* wmask,
-                                  float* avg, void* stream_) {
-  return bags_sample_others_step(labels, label2bin, N, G, classes, ratio, seed, nullptr, wmask, avg, stream_);
 }
 
 extern "C" int bags_mask_avg(const uint8_t* wmask, int N, int G, float* avg, void* stream_) {
@@ -422,10 +381,10 @@ extern "C" int bags_mask_avg(const uint8_t* wmask, int N, int G, float* avg, voi
 
 template <int NV>
 static int launch_group_ce(const float* logits, long long ldz, const int64_t* labels,
-                           const int32_t* label2bin, const GroupTable& gt, const uint8_t* wmask,
+                           const int32_t* label2bin, const GroupTable& gt, const uint8_t* wmask, bool wf,
                            const float* avg, int N, int C, int classes, float* loss, float* lse,
                            void* dz, long long ldd, int dz_dtype, float* colsum, void* workspace,
-                           int num_sms, cudaStream_t stream, bool wf = false) {
+                           int num_sms, cudaStream_t stream) {
   const int smem = 8 * NV * 128 * (int)sizeof(float);
   // persistent CTAs (2 per SM: 126 regs x 256 threads): every CTA walks several row octets so the
   // bias-gradient column sums are reduced in registers/smem and hit global atomics once per CTA
@@ -439,34 +398,25 @@ static int launch_group_ce(const float* logits, long long ldz, const int64_t* la
   unsigned int* counter = reinterpret_cast<unsigned int*>(workspace);
   float* part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
   const long long* lab = reinterpret_cast<const long long*>(labels);
-  if (wf) {   // fp32 per-RoI weights (reweight head variant)
-    auto k = (dz_dtype == BAGS_DTYPE_F32) ? group_ce_kernel<NV, true, true> : group_ce_kernel<NV, false, true>;
-    BAGS_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    k<<<grid, 256, smem, stream>>>(logits, ldz, lab, label2bin, classes, gt, wmask, avg, N, C, loss, lse, dz, ldd,
-                                   colsum, part, counter);
-  } else if (dz_dtype == BAGS_DTYPE_F32) {
-    auto k = group_ce_kernel<NV, true>;
-    BAGS_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    k<<<grid, 256, smem, stream>>>(logits, ldz, lab, label2bin, classes, gt, wmask, avg, N, C, loss, lse, dz, ldd,
-                                   colsum, part, counter);
-  } else {
-    auto k = group_ce_kernel<NV, false>;
-    BAGS_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    k<<<grid, 256, smem, stream>>>(logits, ldz, lab, label2bin, classes, gt, wmask, avg, N, C, loss, lse, dz, ldd,
-                                   colsum, part, counter);
-  }
+  const bool dz_f32 = dz_dtype == BAGS_DTYPE_F32;
+  auto k = wf ? (dz_f32 ? group_ce_kernel<NV, true, true> : group_ce_kernel<NV, false, true>)
+              : (dz_f32 ? group_ce_kernel<NV, true> : group_ce_kernel<NV, false>);
+  BAGS_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  k<<<grid, 256, smem, stream>>>(logits, ldz, lab, label2bin, classes, gt, wmask, avg, N, C, loss, lse, dz, ldd,
+                                 colsum, part, counter);
   BAGS_CUDA(cudaGetLastError());
   return BAGS_OK;
 }
 
-static int group_ce_impl(const float* logits, long long ldz, const int64_t* labels,
-                         const int32_t* label2bin, const int32_t* slices_host,
-                         const uint8_t* wmask, bool wf, const float* avg, int N, int C, int G,
-                         int classes, float* loss, float* lse, void* dz, long long ldd,
-                         int dz_dtype, float* colsum, void* workspace, size_t workspace_bytes,
-                         void* stream_) {
+extern "C" int bags_group_ce(const float* logits, long long ldz, const int64_t* labels,
+                             const int32_t* label2bin, const int32_t* slices_host, const void* weights,
+                             int weights_dtype, const float* avg, int N, int C, int G, int classes, float* loss,
+                             float* lse, void* dz, long long ldd, int dz_dtype, float* colsum, void* workspace,
+                             size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   BAGS_REQUIRE(label2bin && loss && workspace && (N == 0 || (logits && labels)), "bags_group_ce: NULL argument");
+  BAGS_REQUIRE(weights_dtype == BAGS_WEIGHTS_U8 || weights_dtype == BAGS_WEIGHTS_F32,
+               "bags_group_ce: bad weights dtype %d", weights_dtype);
   BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "bags_group_ce: workspace too small (%zu < %zu)",
                workspace_bytes, bags_workspace_bytes());
   BAGS_REQUIRE(N >= 0 && C >= 4 && (C % 4) == 0 && C <= 4096, "bags_group_ce: C=%d must be a multiple of 4 in [4,4096]", C);
@@ -489,36 +439,17 @@ static int group_ce_impl(const float* logits, long long ldz, const int64_t* labe
     BAGS_CUDA(cudaMemsetAsync(loss, 0, sizeof(float) * G, stream));
     return BAGS_OK;
   }
+  const uint8_t* wmask = static_cast<const uint8_t*>(weights);
+  const bool wf = weights_dtype == BAGS_WEIGHTS_F32;
   const int nv = (C / 4 + 31) / 32;
   if (nv <= 10)
-    return launch_group_ce<10>(logits, ldz, labels, label2bin, gt, wmask, avg, N, C, classes, loss, lse, dz, ldd,
-                               dz_dtype, colsum, workspace, di.num_sms, stream, wf);
+    return launch_group_ce<10>(logits, ldz, labels, label2bin, gt, wmask, wf, avg, N, C, classes, loss, lse, dz, ldd,
+                               dz_dtype, colsum, workspace, di.num_sms, stream);
   if (nv <= 16)
-    return launch_group_ce<16>(logits, ldz, labels, label2bin, gt, wmask, avg, N, C, classes, loss, lse, dz, ldd,
-                               dz_dtype, colsum, workspace, di.num_sms, stream, wf);
-  return launch_group_ce<32>(logits, ldz, labels, label2bin, gt, wmask, avg, N, C, classes, loss, lse, dz, ldd,
-                             dz_dtype, colsum, workspace, di.num_sms, stream, wf);
-}
-
-extern "C" int bags_group_ce(const float* logits, long long ldz, const int64_t* labels,
-                             const int32_t* label2bin, const int32_t* slices_host,
-                             const uint8_t* wmask, const float* avg, int N, int C, int G,
-                             int classes, float* loss, float* lse, void* dz, long long ldd,
-                             int dz_dtype, float* colsum, void* workspace, size_t workspace_bytes,
-                             void* stream_) {
-  return group_ce_impl(logits, ldz, labels, label2bin, slices_host, wmask, false, avg, N, C, G, classes, loss, lse, dz,
-                       ldd, dz_dtype, colsum, workspace, workspace_bytes, stream_);
-}
-
-extern "C" int bags_group_ce_w(const float* logits, long long ldz, const int64_t* labels,
-                               const int32_t* label2bin, const int32_t* slices_host,
-                               const float* wfloat, const float* avg, int N, int C, int G,
-                               int classes, float* loss, float* lse, void* dz, long long ldd,
-                               int dz_dtype, float* colsum, void* workspace, size_t workspace_bytes,
-                               void* stream_) {
-  return group_ce_impl(logits, ldz, labels, label2bin, slices_host, reinterpret_cast<const uint8_t*>(wfloat),
-                       wfloat != nullptr, avg, N, C, G, classes, loss, lse, dz, ldd, dz_dtype, colsum, workspace,
-                       workspace_bytes, stream_);
+    return launch_group_ce<16>(logits, ldz, labels, label2bin, gt, wmask, wf, avg, N, C, classes, loss, lse, dz, ldd,
+                               dz_dtype, colsum, workspace, di.num_sms, stream);
+  return launch_group_ce<32>(logits, ldz, labels, label2bin, gt, wmask, wf, avg, N, C, classes, loss, lse, dz, ldd,
+                             dz_dtype, colsum, workspace, di.num_sms, stream);
 }
 
 
@@ -533,8 +464,7 @@ static bool fused_eligible(const int32_t* slices_host, int G, int C) {
     if (slices_host[2 * g] != end || slices_host[2 * g + 1] < 1) return false;
     end += slices_host[2 * g + 1];
   }
-  if (end != C) return false;
-  return env_int("BAGS_FUSED", 1) != 0;
+  return end == C;
 }
 
 extern "C" int bags_fused_eligible(const int32_t* slices_host, int G, int C) {
@@ -543,7 +473,7 @@ extern "C" int bags_fused_eligible(const int32_t* slices_host, int G, int C) {
 
 template <bool TF32>
 static int launch_fused_fwd(const void* x, long long ldx, const void* w, long long ldw, const FusedFwdParams& p0,
-                            void* dz, long long ldd, const DeviceInfo& di, cudaStream_t stream, bool wf = false) {
+                            void* dz, long long ldd, cudaStream_t stream, bool wf) {
   using Cfg = FusedCfg<TF32>;
   const int dtype = TF32 ? BAGS_DTYPE_F32 : BAGS_DTYPE_BF16;
   CUtensorMap tx, tw;
@@ -561,39 +491,31 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   auto kernel = wf ? bags_fwd_fused_kernel<TF32, true> : bags_fwd_fused_kernel<TF32, false>;
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   const int grid = Cfg::CLUSTER * ((p.N + Cfg::BLOCK_M - 1) / Cfg::BLOCK_M);
-  (void)di;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(Cfg::NUM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
   // PDL INVARIANT (also the sampler's): this kernel reads x, W, bias and labels BEFORE its griddepcontrol.wait (only the
   // sampler's masks / avg and every global write come after it).  That is correct as long as those tensors are not
   // produced by the immediately preceding kernel of the stream with an early launch_dependents trigger -- true for torch
   // kernels (they never trigger early) and for this library's own chain (the predecessor is the sampler / the previous
   // step's backward or exchange, none of which writes them).  A future producer that triggers early must be followed by
   // a non-PDL launch (BAGS_PDL=0) or move these reads behind the wait.
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // overlap with the sampler (pdl_wait in-kernel)
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = env_int("BAGS_PDL", 1) ? 1 : 0;
-  BAGS_CUDA(cudaLaunchKernelEx(&cfg, kernel, tx, tw, p));
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, true, tx, tw, p));
   return BAGS_OK;
 }
 
-static int fwd_impl(const void* x, long long ldx, const void* w, long long ldw,
-                    const float* bias, const int64_t* labels, const int32_t* label2bin,
-                    const int32_t* slices_host, const uint8_t* wmask, bool wf, const float* avg, int N,
-                        int K, int C, int G, int classes, int dtype, float* logits, long long ldz,
+extern "C" int bags_fwd(const void* x, long long ldx, const void* w, long long ldw,
+                        const float* bias, const int64_t* labels, const int32_t* label2bin,
+                        const int32_t* slices_host, const void* weights, int weights_dtype, const float* avg,
+                        int N, int K, int C, int G, int classes, int dtype, float* logits, long long ldz,
                         float* loss, float* lse, void* dz, long long ldd, float* colsum,
-                        int colsum_tiles, void* workspace, size_t workspace_bytes, void* stream_,
-                        void* clear = nullptr, size_t clear_bytes = 0) {
+                        int colsum_tiles, void* workspace, size_t workspace_bytes, void* clear, size_t clear_bytes,
+                        void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  BAGS_REQUIRE(weights_dtype == BAGS_WEIGHTS_U8 || weights_dtype == BAGS_WEIGHTS_F32,
+               "bags_fwd: bad weights dtype %d", weights_dtype);
   if (clear != nullptr) {
     BAGS_REQUIRE((reinterpret_cast<uintptr_t>(clear) & 15) == 0 && (clear_bytes % 16) == 0,
-                 "bags_fwd_ex: the buffer to clear must be 16-byte aligned and a multiple of 16 bytes");
+                 "bags_fwd: the buffer to clear must be 16-byte aligned and a multiple of 16 bytes");
     if (logits != nullptr || N == 0) {   // not the fused kernel: a plain memset
-      BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, static_cast<cudaStream_t>(stream_)));
+      BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, stream));
       clear = nullptr;
     }
   }
@@ -604,13 +526,13 @@ static int fwd_impl(const void* x, long long ldx, const void* w, long long ldw,
     // caller wants materialised logits: GEMM with fp32 store, then the stand-alone grouped CE (tile 0 holds
     // the column sums, the other tiles are zero)
     if (colsum != nullptr && colsum_tiles > 1)
-      BAGS_CUDA(cudaMemsetAsync(colsum, 0, sizeof(float) * C * colsum_tiles, static_cast<cudaStream_t>(stream_)));
-    if (int rc = bags_linear_fwd(x, ldx, w, ldw, bias, logits, ldz, N, K, C, dtype, stream_)) return rc;
-    return group_ce_impl(logits, ldz, labels, label2bin, slices_host, wmask, wf, avg, N, C, G, classes, loss,
-                         lse, dz, ldd, dtype, colsum, workspace, workspace_bytes, stream_);
+      BAGS_CUDA(cudaMemsetAsync(colsum, 0, sizeof(float) * C * colsum_tiles, stream));
+    if (int rc = bags_linear_act_fwd(x, ldx, w, ldw, bias, logits, ldz, N, K, C, dtype, BAGS_DTYPE_F32, 0, stream_))
+      return rc;
+    return bags_group_ce(logits, ldz, labels, label2bin, slices_host, weights, weights_dtype, avg, N, C, G, classes,
+                         loss, lse, dz, ldd, dtype, colsum, workspace, workspace_bytes, stream_);
   }
   // fused path: logits stay in registers
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   BAGS_REQUIRE(fused_eligible(slices_host, G, C),
                "bags_fwd: logits == NULL requests the fused kernel, but this bin table / C=%d / G=%d is not eligible "
                "(see bags_fused_eligible); pass a logits workspace", C, G);
@@ -634,48 +556,15 @@ static int fwd_impl(const void* x, long long ldx, const void* w, long long ldw,
   FusedFwdParams p{};
   p.N = N; p.C = C; p.K = K; p.gt = gt; p.bias = bias;
   p.labels = reinterpret_cast<const long long*>(labels);
-  p.l2b = label2bin; p.classes = classes; p.wmask = wmask; p.avg = avg;
+  p.l2b = label2bin; p.classes = classes; p.wmask = static_cast<const uint8_t*>(weights); p.avg = avg;
   p.loss = loss; p.lse = lse; p.colsum = colsum;
   p.counter = reinterpret_cast<unsigned int*>(workspace);
   p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  if (N == 0) dz = nullptr;
   p.clear = reinterpret_cast<float4*>(clear);
   p.clear_vecs = static_cast<long long>(clear_bytes / 16);
-  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di, stream, wf)
-                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di, stream, wf);
-}
-
-extern "C" int bags_fwd(const void* x, long long ldx, const void* w, long long ldw,
-                        const float* bias, const int64_t* labels, const int32_t* label2bin,
-                        const int32_t* slices_host, const uint8_t* wmask, const float* avg, int N,
-                        int K, int C, int G, int classes, int dtype, float* logits, long long ldz,
-                        float* loss, float* lse, void* dz, long long ldd, float* colsum,
-                        int colsum_tiles, void* workspace, size_t workspace_bytes, void* stream_) {
-  return fwd_impl(x, ldx, w, ldw, bias, labels, label2bin, slices_host, wmask, false, avg, N, K, C, G, classes, dtype,
-                  logits, ldz, loss, lse, dz, ldd, colsum, colsum_tiles, workspace, workspace_bytes, stream_);
-}
-
-extern "C" int bags_fwd_ex(const void* x, long long ldx, const void* w, long long ldw,
-                           const float* bias, const int64_t* labels, const int32_t* label2bin,
-                           const int32_t* slices_host, const uint8_t* wmask, const float* avg, int N,
-                           int K, int C, int G, int classes, int dtype, float* logits, long long ldz,
-                           float* loss, float* lse, void* dz, long long ldd, float* colsum,
-                           int colsum_tiles, void* workspace, size_t workspace_bytes, void* clear, size_t clear_bytes,
-                           void* stream_) {
-  return fwd_impl(x, ldx, w, ldw, bias, labels, label2bin, slices_host, wmask, false, avg, N, K, C, G, classes, dtype,
-                  logits, ldz, loss, lse, dz, ldd, colsum, colsum_tiles, workspace, workspace_bytes, stream_, clear,
-                  clear_bytes);
-}
-
-extern "C" int bags_fwd_w(const void* x, long long ldx, const void* w, long long ldw,
-                          const float* bias, const int64_t* labels, const int32_t* label2bin,
-                          const int32_t* slices_host, const float* wfloat, const float* avg, int N,
-                          int K, int C, int G, int classes, int dtype, float* logits, long long ldz,
-                          float* loss, float* lse, void* dz, long long ldd, float* colsum,
-                          int colsum_tiles, void* workspace, size_t workspace_bytes, void* stream_) {
-  return fwd_impl(x, ldx, w, ldw, bias, labels, label2bin, slices_host, reinterpret_cast<const uint8_t*>(wfloat),
-                  wfloat != nullptr, avg, N, K, C, G, classes, dtype, logits, ldz, loss, lse, dz, ldd, colsum,
-                  colsum_tiles, workspace, workspace_bytes, stream_);
+  const bool wf = weights_dtype == BAGS_WEIGHTS_F32;
+  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, stream, wf)
+                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, stream, wf);
 }
 
 extern "C" int bags_reweight(const int64_t* labels, const int32_t* label2bin, const uint8_t* wmask,
@@ -723,40 +612,29 @@ static int launch_bwd_merged(const void* dz, long long ldd, const void* x, long 
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CW::SMEM_BYTES));
   const int units = bp.dw_units + bp.dx_units;
   const int grid = units < di.num_sms ? units : di.num_sms;
-  BAGS_CUDA(launch_pdl(kernel, dim3(grid), dim3(CW::NUM_THREADS), CW::SMEM_BYTES, stream, t_dzT, t_xT, t_dz, t_w, t_wp, bp));
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(CW::NUM_THREADS), CW::SMEM_BYTES, stream, true, t_dzT, t_xT, t_dz, t_w, t_wp, bp));
   return BAGS_OK;
 }
 
 static constexpr int kColsumTiles = 8;   // row groups of the bias-gradient partial sums made by bwd_prep
 
-extern "C" size_t bags_bwd_scratch_bytes(int C, long long ldw, int dtype) {
+// bytes of the gout-scaled copy W' at the start of wscratch; the bias-gradient partials follow it
+static size_t wprime_bytes(int C, long long ldw, int dtype) {
   const size_t elt = (dtype == BAGS_DTYPE_BF16) ? 2 : 4;
-  const size_t wbytes = (static_cast<size_t>(C) * static_cast<size_t>(ldw) * elt + 255) & ~static_cast<size_t>(255);
-  return wbytes + static_cast<size_t>(kColsumTiles) * C * sizeof(float);
+  return (static_cast<size_t>(C) * static_cast<size_t>(ldw) * elt + 255) & ~static_cast<size_t>(255);
 }
 
-extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long long ldx, const void* w,
-                           long long ldw, const float* gout, const int32_t* slices_host,
-                           const float* colsum, int colsum_tiles, float* dW, long long lddw, float* db, void* dX,
-                           long long lddx, void* wscratch, size_t wscratch_bytes, int N, int K, int C, int G,
-                           int dtype, int flags, void* stream_);
+extern "C" size_t bags_bwd_scratch_bytes(int C, long long ldw, int dtype) {
+  return wprime_bytes(C, ldw, dtype) + static_cast<size_t>(kColsumTiles) * C * sizeof(float);
+}
 
 extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long ldx, const void* w,
                         long long ldw, const float* gout, const int32_t* slices_host,
                         const float* colsum, int colsum_tiles, float* dW, long long lddw, float* db, void* dX,
                         long long lddx, void* wscratch, size_t wscratch_bytes, int N, int K, int C, int G,
-                        int dtype, void* stream_) {
-  return bags_bwd_ex(dz, ldd, x, ldx, w, ldw, gout, slices_host, colsum, colsum_tiles, dW, lddw, db, dX, lddx, wscratch,
-                     wscratch_bytes, N, K, C, G, dtype, 0, stream_);
-}
-
-extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long long ldx, const void* w,
-                           long long ldw, const float* gout, const int32_t* slices_host,
-                           const float* colsum, int colsum_tiles, float* dW, long long lddw, float* db, void* dX,
-                           long long lddx, void* wscratch, size_t wscratch_bytes, int N, int K, int C, int G,
-                           int dtype, int flags, void* stream_) {
+                        int dtype, int flags, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  const bool prezeroed = (flags & BAGS_BWD_DW_PREZEROED) != 0;   // the caller (bags_fwd_ex's clear hook) zeroed dW
+  const bool prezeroed = (flags & BAGS_BWD_DW_PREZEROED) != 0;   // the caller (bags_fwd's clear hook) zeroed dW
   BAGS_REQUIRE(dz != nullptr || N == 0, "bags_bwd: dz is NULL");
   BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "bags_bwd: bad dtype %d", dtype);
   BAGS_REQUIRE(N >= 0 && K >= 1 && C >= 1, "bags_bwd: bad shape");
@@ -779,12 +657,8 @@ extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long lo
                  bags_bwd_scratch_bytes(C, ldw, dtype), wscratch_bytes);
     BAGS_REQUIRE((reinterpret_cast<uintptr_t>(wscratch) & 255) == 0, "bags_bwd: wscratch must be 256-byte aligned");
   }
-  float* colpart = nullptr;
-  if (wscratch != nullptr) {
-    const size_t elt = bf ? 2 : 4;
-    const size_t wbytes = (static_cast<size_t>(C) * static_cast<size_t>(ldw) * elt + 255) & ~static_cast<size_t>(255);
-    colpart = reinterpret_cast<float*>(reinterpret_cast<char*>(wscratch) + wbytes);
-  }
+  float* colpart = (wscratch == nullptr) ? nullptr
+                   : reinterpret_cast<float*>(reinterpret_cast<char*>(wscratch) + wprime_bytes(C, ldw, dtype));
   if (dW != nullptr)
     BAGS_REQUIRE((x != nullptr || N == 0) && lddw >= K && (lddw % 4) == 0 && (K % 4) == 0 &&
                      (reinterpret_cast<uintptr_t>(dW) & 15) == 0,
@@ -811,9 +685,10 @@ extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long lo
     pp.c_ctas = want_colpart ? ((C + 63) / 64) * kColsumTiles : 0;
     pp.skip_scale_if_uniform = merged ? 1 : 0;   // the merged kernel reads W itself when all gout[g] are equal
     const int grid = pp.z_ctas + pp.s_ctas + pp.c_ctas;
-    if (grid == 0) { /* nothing to prepare */ }
-    else if (bf) { BAGS_CUDA(launch_pdl(bwd_prep_kernel<false>, dim3(grid), dim3(256), 0, stream, pp)); prep_launched = true; }
-    else         { BAGS_CUDA(launch_pdl(bwd_prep_kernel<true>, dim3(grid), dim3(256), 0, stream, pp)); prep_launched = true; }
+    if (grid > 0) {
+      BAGS_CUDA(launch(bf ? bwd_prep_kernel<false> : bwd_prep_kernel<true>, dim3(grid), dim3(256), 0, stream, true, pp));
+      prep_launched = true;
+    }
   }
   const float* cs_in = (colsum != nullptr) ? colsum : colpart;
   const int cs_tiles = (colsum != nullptr) ? colsum_tiles : kColsumTiles;
@@ -881,8 +756,8 @@ extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long lo
     ga.p.colsum_out = (db != nullptr) ? db : nullptr;
     ga.p.pdl_wait_epilogue = 1;   // dW zeroing + column-sum partials come from bwd_prep; the mainloop overlaps it
     ga.p.pdl_wait_producer = prep_launched ? 0 : 1;   // no preparation kernel in between: dz comes from the preceding kernel
-    int rc = bf ? launch_gemm_pdl<256, true, true, EPI_RED_F32, false, 4>(ga, di, stream)
-                : launch_gemm_pdl<256, true, true, EPI_RED_F32, true, 4>(ga, di, stream);
+    int rc = bf ? launch_gemm<256, true, true, EPI_RED_F32, false, 4>(ga, di, stream, true)
+                : launch_gemm<256, true, true, EPI_RED_F32, true, 4>(ga, di, stream, true);
     if (rc) return rc;
   } else if (db != nullptr) {
     scale_colsum_kernel<<<(C + 255) / 256, 256, 0, stream>>>(cs_in, cs_tiles, db, C, gt, gout);
@@ -899,8 +774,8 @@ extern "C" int bags_bwd_ex(const void* dz, long long ldd, const void* x, long lo
     ga.p.out = dX; ga.p.ldo = lddx; ga.p.bias = nullptr; ga.p.gscale = nullptr; ga.p.G = 0;
     ga.p.colsum_in = nullptr; ga.p.colsum_out = nullptr;
     ga.p.pdl_wait_producer = 1;   // W' is produced by bwd_prep (two kernels back; the chain of waits covers it)
-    int rc = bf ? launch_gemm_pdl<256, false, true, EPI_STORE_BF16, false, 4>(ga, di, stream)
-                : launch_gemm_pdl<256, false, true, EPI_STORE_F32, true, 4>(ga, di, stream);
+    int rc = bf ? launch_gemm<256, false, true, EPI_STORE_BF16, false, 4>(ga, di, stream, true)
+                : launch_gemm<256, false, true, EPI_STORE_F32, true, 4>(ga, di, stream, true);
     if (rc) return rc;
   }
   return BAGS_OK;
@@ -967,10 +842,9 @@ extern "C" int bags_grad_allreduce(void* const* peer_bufs_host, void* mc_buf, lo
   if (blocks > max_blocks) blocks = max_blocks;
   const bool epoch = env_int("BAGS_AR_EPOCH", 1) != 0;
   const dim3 grid(static_cast<unsigned>(blocks)), block(static_cast<unsigned>(threads));
-  if (mm && epoch)       BAGS_CUDA(launch_pdl(bags_grad_allreduce_kernel<true, true>, grid, block, 0, stream, p));
-  else if (mm)           BAGS_CUDA(launch_pdl(bags_grad_allreduce_kernel<true, false>, grid, block, 0, stream, p));
-  else if (epoch)        BAGS_CUDA(launch_pdl(bags_grad_allreduce_kernel<false, true>, grid, block, 0, stream, p));
-  else                   BAGS_CUDA(launch_pdl(bags_grad_allreduce_kernel<false, false>, grid, block, 0, stream, p));
+  auto kernel = mm ? (epoch ? bags_grad_allreduce_kernel<true, true> : bags_grad_allreduce_kernel<true, false>)
+                  : (epoch ? bags_grad_allreduce_kernel<false, true> : bags_grad_allreduce_kernel<false, false>);
+  BAGS_CUDA(launch(kernel, grid, block, 0, stream, true, p));
   return BAGS_OK;
 }
 
@@ -1008,31 +882,6 @@ extern "C" int bags_debug_spin(int blocks, int threads, int micros, void* stream
   bags_debug_spin_kernel<<<blocks, threads, 0, static_cast<cudaStream_t>(stream_)>>>(1000LL * micros);
   BAGS_CUDA(cudaGetLastError());
   return BAGS_OK;
-}
-
-// test hook: how many clusters of `cluster` CTAs (each `threads` threads + `smem_bytes` dynamic shared memory, i.e. one CTA
-// per SM for the GEMM-sized value) can be resident at once -- the GPC layout decides (an SM count such as 132 does not split evenly)
-extern "C" int bags_debug_max_clusters(int cluster, int threads, int smem_bytes) {
-  if (cluster < 1 || cluster > 16 || threads < 32 || threads > 1024 || smem_bytes < 0) return -1;
-  DeviceInfo di;
-  if (device_info(di)) return -1;
-  if (cudaFuncSetAttribute(bags_debug_spin_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes) != cudaSuccess) {
-    (void)cudaGetLastError();
-    return -1;
-  }
-  if (cluster > 8) (void)cudaFuncSetAttribute(bags_debug_spin_kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(cluster * ((2 * di.num_sms) / cluster)));
-  cfg.blockDim = dim3(static_cast<unsigned>(threads));
-  cfg.dynamicSmemBytes = static_cast<size_t>(smem_bytes);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = static_cast<unsigned>(cluster); attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  int n = -1;
-  if (cudaOccupancyMaxActiveClusters(&n, bags_debug_spin_kernel, &cfg) != cudaSuccess) { (void)cudaGetLastError(); return -1; }
-  return n;
 }
 
 extern "C" int bags_merge_scores(const float* logits, long long ldz, const int32_t* slices_host,

@@ -11,7 +11,7 @@ signatures and returned dict keys are identical so configs/bags/*.py blocks buil
 What differs is the execution of the hot path:
 
   * ``fc_cls`` (convfc_bbox_head.py:166) runs on wgmma tensor cores through the C ABI
-    (``bags_linear_fwd``) instead of cuBLAS SGEMM;
+    (``bags_linear_act_fwd``) instead of cuBLAS SGEMM;
   * ``_remap_labels`` + ``_sample_others`` + ``_slice_preds`` + 5x ``CrossEntropyLoss``
     (gs_bbox_head_with0.py:63-171) -- ~70 small kernels and >=15 host syncs per call in the
     reference -- become one sampler launch plus ONE fused forward call and ONE fused backward
@@ -184,7 +184,7 @@ class ClsScoreHandle(object):
 
 
 class FcClsFunction(torch.autograd.Function):
-    """Materialised logits = x W^T + b on the wgmma GEMM (bags_linear_fwd); backward reuses bags_bwd."""
+    """Materialised logits = x W^T + b on the wgmma GEMM (bags_linear_act_fwd); backward reuses bags_bwd."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, compute_dtype):
@@ -210,11 +210,8 @@ class FcClsFunction(torch.autograd.Function):
         dz = torch.zeros((N, ldd), dtype=xc.dtype, device=xc.device)
         dz[:, :Cc] = grad_out
         colsum = grad_out.float().sum(0, keepdim=True)
-        head_dt = ops.DeviceTables(1, 1, Cc, torch.zeros(1, 1, dtype=torch.int32, device=xc.device),
-                                   torch.zeros(1, dtype=torch.int32, device=xc.device),
-                                   ops.nat.int32_array([0, Cc]), np.array([[0, Cc]], dtype=np.int64))
-        dW, db, dX = ops.fused_bwd(dz, xc, wc, None, head_dt, colsum, need_dw=ctx.needs_input_grad[1],
-                                   need_db=ctx.needs_input_grad[2] and bd is not None,
+        dW, db, dX = ops.fused_bwd(dz, xc, wc, None, ops._single_slice_tables(Cc, xc.device), colsum,
+                                   need_dw=ctx.needs_input_grad[1], need_db=ctx.needs_input_grad[2] and bd is not None,
                                    need_dx=ctx.needs_input_grad[0])
         return (None if dX is None else dX.to(xd), None if dW is None else dW.to(wd),
                 None if db is None else db.to(bd), None)

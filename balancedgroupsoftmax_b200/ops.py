@@ -55,16 +55,16 @@ def _row_major(t: torch.Tensor) -> torch.Tensor:
 _workspaces: Dict[Tuple[int, int], torch.Tensor] = {}
 
 
-def _weights_arg(wmask: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-    """[G,N] sample weights as the kernels read them: contiguous 0/1 bytes (bool is the same storage), or fp32
-    (reweight head variant); other dtypes are cast to fp32."""
+def _weights_arg(wmask: Optional[torch.Tensor]) -> Tuple[Optional[torch.Tensor], int]:
+    """[G,N] sample weights as the kernels read them, with their weights_dtype code: contiguous 0/1 bytes (bool is
+    the same storage), or fp32 (reweight head variant); other dtypes are cast to fp32."""
     if wmask is None:
-        return None
+        return None, nat.WEIGHTS_U8
     if wmask.dtype == torch.bool:
         wmask = wmask.view(torch.uint8)
     elif wmask.dtype not in (torch.uint8, torch.float32):
         wmask = wmask.to(torch.float32)
-    return wmask.contiguous()
+    return wmask.contiguous(), (nat.WEIGHTS_F32 if wmask.dtype == torch.float32 else nat.WEIGHTS_U8)
 
 
 def _workspace(device: torch.device) -> torch.Tensor:
@@ -132,9 +132,10 @@ def linear_fwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor],
     if bias is not None:
         bias = bias.contiguous()
         assert bias.dtype == torch.float32
-    nat.check(nat.lib().bags_linear_fwd(x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias),
-                                        out.data_ptr(), out.stride(0), N, K, Cc, _dtype_code(x.dtype),
-                                        _stream_ptr(x.device)), 'bags_linear_fwd')
+    # the single-pass GEMM, never split-K (linear_act may choose it): the materialised logits keep one summation order
+    nat.check(nat.lib().bags_linear_act_fwd(x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias),
+                                            out.data_ptr(), out.stride(0), N, K, Cc, _dtype_code(x.dtype),
+                                            nat.DTYPE_F32, 0, _stream_ptr(x.device)), 'bags_linear_act_fwd')
     return out
 
 
@@ -151,9 +152,9 @@ def sample_others(labels: torch.Tensor, dt: DeviceTables, ratio: float, seed: in
     avg = torch.empty((dt.G,), dtype=torch.float32, device=labels.device)
     if seed_step is not None:
         assert seed_step.dtype == torch.int64 and seed_step.numel() == 1
-    nat.check(nat.lib().bags_sample_others_step(labels.data_ptr(), dt.label2bin.data_ptr(), N, dt.G, dt.num_classes,
-                                                float(ratio), int(seed) & 0xFFFFFFFFFFFFFFFF, nat.ptr(seed_step),
-                                                wmask.data_ptr(), avg.data_ptr(), _stream_ptr(labels.device)),
+    nat.check(nat.lib().bags_sample_others(labels.data_ptr(), dt.label2bin.data_ptr(), N, dt.G, dt.num_classes,
+                                           float(ratio), int(seed) & 0xFFFFFFFFFFFFFFFF, nat.ptr(seed_step),
+                                           wmask.data_ptr(), avg.data_ptr(), _stream_ptr(labels.device)),
               'bags_sample_others')
     return wmask, avg
 
@@ -205,12 +206,11 @@ def group_ce(logits: torch.Tensor, labels: torch.Tensor, dt: DeviceTables,
         dz = torch.empty((N, ldd), dtype=dz_dtype, device=dev)
         colsum = torch.empty((1, Cc), dtype=torch.float32, device=dev)
     ws = _workspace(dev)
-    wmask = _weights_arg(wmask)
-    entry = nat.lib().bags_group_ce_w if (wmask is not None and wmask.dtype == torch.float32) else nat.lib().bags_group_ce
-    nat.check(entry(
+    wmask, wcode = _weights_arg(wmask)
+    nat.check(nat.lib().bags_group_ce(
         logits.data_ptr(), logits.stride(0), labels.data_ptr(), dt.label2bin.data_ptr(), dt.slices_host,
-        nat.ptr(wmask), nat.ptr(avg), N, Cc, dt.G, dt.num_classes, loss.data_ptr(), nat.ptr(lse), nat.ptr(dz), ldd,
-        _dtype_code(dz_dtype), nat.ptr(colsum), ws.data_ptr(), ws.numel(), _stream_ptr(dev)), 'bags_group_ce')
+        nat.ptr(wmask), wcode, nat.ptr(avg), N, Cc, dt.G, dt.num_classes, loss.data_ptr(), nat.ptr(lse), nat.ptr(dz),
+        ldd, _dtype_code(dz_dtype), nat.ptr(colsum), ws.data_ptr(), ws.numel(), _stream_ptr(dev)), 'bags_group_ce')
     return loss, lse, dz, colsum
 
 
@@ -253,27 +253,17 @@ def fused_fwd(x, w, bias, labels, dt: DeviceTables, wmask, avg, logits: Optional
         if want_colsum:   # per-row-tile partials; by default the backward recomputes them from dz instead
             colsum = torch.empty((max((N + 127) // 128, 1), Cc), dtype=torch.float32, device=dev)
     ws = _workspace(dev)
-    wmask = _weights_arg(wmask)
-    wfloat = wmask is not None and wmask.dtype == torch.float32
-    if clear is not None and not wfloat:
-        # ``clear``: a contiguous buffer (the caller's dW) that the kernel zeroes while its MMAs run
-        assert clear.is_contiguous() and (clear.numel() * clear.element_size()) % 16 == 0
-        nat.check(nat.lib().bags_fwd_ex(
-            x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(),
-            dt.label2bin.data_ptr(), dt.slices_host, nat.ptr(wmask), nat.ptr(avg), N, K, Cc, dt.G, dt.num_classes,
-            _dtype_code(x.dtype), nat.ptr(logits), logits.stride(0) if logits is not None else 0, loss.data_ptr(),
-            nat.ptr(lse), nat.ptr(dz), ldd, nat.ptr(colsum), colsum.shape[0] if colsum is not None else 0, ws.data_ptr(),
-            ws.numel(), clear.data_ptr(), clear.numel() * clear.element_size(), _stream_ptr(dev)), 'bags_fwd_ex')
-        return loss, logits, lse, dz, colsum
+    wmask, wcode = _weights_arg(wmask)
     if clear is not None:
-        clear.zero_()
-    entry = nat.lib().bags_fwd_w if wfloat else nat.lib().bags_fwd
-    nat.check(entry(
+        # ``clear``: a contiguous buffer (the caller's dW) that the forward zeroes, on the fused route while its MMAs run
+        assert clear.is_contiguous() and (clear.numel() * clear.element_size()) % 16 == 0
+    nat.check(nat.lib().bags_fwd(
         x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(),
-        dt.label2bin.data_ptr(), dt.slices_host, nat.ptr(wmask), nat.ptr(avg), N, K, Cc, dt.G, dt.num_classes,
+        dt.label2bin.data_ptr(), dt.slices_host, nat.ptr(wmask), wcode, nat.ptr(avg), N, K, Cc, dt.G, dt.num_classes,
         _dtype_code(x.dtype), nat.ptr(logits), logits.stride(0) if logits is not None else 0, loss.data_ptr(),
         nat.ptr(lse), nat.ptr(dz), ldd, nat.ptr(colsum), colsum.shape[0] if colsum is not None else 0, ws.data_ptr(),
-        ws.numel(), _stream_ptr(dev)), 'bags_fwd')
+        ws.numel(), nat.ptr(clear), clear.numel() * clear.element_size() if clear is not None else 0,
+        _stream_ptr(dev)), 'bags_fwd')
     return loss, logits, lse, dz, colsum
 
 
@@ -323,7 +313,7 @@ def fused_bwd(dz, x, w, gout, dt: DeviceTables, colsum=None, need_dw=True, need_
     if gout is not None:
         gout = gout.contiguous()
         assert gout.dtype == torch.float32 and gout.numel() == dt.G
-    nat.check(nat.lib().bags_bwd_ex(
+    nat.check(nat.lib().bags_bwd(
         dz.data_ptr(), dz.stride(0), x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(gout),
         dt.slices_host, nat.ptr(colsum), (colsum.shape[0] if colsum.dim() == 2 else 1) if colsum is not None else 0,
         nat.ptr(dW) if need_dw else None, dW.stride(0) if need_dw else 0,

@@ -7,7 +7,7 @@
  *
  *   reference interface                                   replaced by
  *   ---------------------------------------------------   -------------------------
- *   ConvFCBBoxHead.forward: self.fc_cls(x_cls)            bags_linear_fwd
+ *   ConvFCBBoxHead.forward: self.fc_cls(x_cls)            bags_linear_act_fwd
  *     mmdet/models/bbox_heads/convfc_bbox_head.py:166
  *   GSBBoxHeadWith0._sample_others                        bags_sample_others
  *     mmdet/models/bbox_heads/gs_bbox_head_with0.py:63-89
@@ -54,10 +54,12 @@
 extern "C" {
 #endif
 
-#define BAGS_ABI_VERSION 1
+#define BAGS_ABI_VERSION 2
 #define BAGS_MAX_BINS 8
 #define BAGS_DTYPE_F32 0
 #define BAGS_DTYPE_BF16 1
+#define BAGS_WEIGHTS_U8 0    /* per-RoI sample weights: 0/1 bytes */
+#define BAGS_WEIGHTS_F32 1   /* per-RoI sample weights: fp32 (reweight head variant) */
 
 #define BAGS_OK 0
 #define BAGS_ERR_INVALID (-1)   /* bad argument / unsupported shape */
@@ -70,22 +72,15 @@ const char* bags_last_error(void);
 /* bytes the caller must provide (zero-initialised ONCE) as `workspace` to bags_group_ce / bags_fwd */
 size_t bags_workspace_bytes(void);
 
-/* out[N,C] = x[N,K] @ w[C,K]^T + bias[C]      (fp32 output)
- * x, w: dtype elements with leading dims ldx, ldw (elements; rows 16-byte aligned). bias may be NULL. */
-int bags_linear_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
-                    float* out, long long ldo, int N, int K, int C, int dtype, void* stream);
-
 /* wmask[G,N] (uint8 0/1) and avg[G] = max(sum w, 1): bin 0 all ones; bins >= 1 keep every in-bin row
  * and a uniform random subset of k = int(F * ratio) "others" rows (F = #in-bin rows), exactly as
- * _sample_others does, but on the device with a counter-based RNG keyed by `seed`. */
-int bags_sample_others(const int64_t* labels, const int32_t* label2bin, int N, int G, int classes,
-                       double ratio, uint64_t seed, uint8_t* wmask, float* avg, void* stream);
-/* Same, with the effective seed = seed + (*seed_step) * 0x9E3779B97F4A7C15 read on the DEVICE (seed_step may be
- * NULL).  For CUDA-graph replays, where by-value arguments are frozen at capture time: the caller advances the
+ * _sample_others does, but on the device with a counter-based RNG keyed by the effective seed
+ * seed + (*seed_step) * 0x9E3779B97F4A7C15, read on the DEVICE (seed_step may be NULL: the seed as given).
+ * seed_step serves CUDA-graph replays, where by-value arguments are frozen at capture time: the caller advances the
  * counter between replays (not with the kernel that immediately precedes this one in the stream). */
-int bags_sample_others_step(const int64_t* labels, const int32_t* label2bin, int N, int G, int classes,
-                            double ratio, uint64_t seed, const uint64_t* seed_step, uint8_t* wmask,
-                            float* avg, void* stream);
+int bags_sample_others(const int64_t* labels, const int32_t* label2bin, int N, int G, int classes,
+                       double ratio, uint64_t seed, const uint64_t* seed_step, uint8_t* wmask,
+                       float* avg, void* stream);
 
 /* avg[g] = max(sum_n wmask[g,n], 1) for caller-provided masks */
 int bags_mask_avg(const uint8_t* wmask, int N, int G, float* avg, void* stream);
@@ -94,50 +89,45 @@ int bags_mask_avg(const uint8_t* wmask, int N, int G, float* avg, void* stream);
  *   loss[g] = sum_n w[g,n] * (logsumexp(z[n, slice_g]) - z[n, start_g + label2bin[g, labels[n]]]) / avg[g]
  * Optional outputs (NULL to skip): lse[N,G]; dz[N,ldd] (dtype elements) = w/avg * (softmax - onehot),
  * i.e. d(sum_g loss_g)/dz before the per-bin upstream gradients are applied; colsum[C] = sum_n dz.
- * wmask NULL => all ones; avg NULL => N.  C % 4 == 0, ldz % 4 == 0, C <= 4096. */
+ * weights: [G,N] sample weights w of type weights_dtype -- BAGS_WEIGHTS_U8 (0/1 bytes, the sampler's masks) or
+ * BAGS_WEIGHTS_F32 (the reweight head variant's bags_reweight output); NULL => all ones.  avg NULL => N.
+ * C % 4 == 0, ldz % 4 == 0, C <= 4096. */
 int bags_group_ce(const float* logits, long long ldz, const int64_t* labels,
-                  const int32_t* label2bin, const int32_t* slices_host, const uint8_t* wmask,
-                  const float* avg, int N, int C, int G, int classes, float* loss, float* lse,
-                  void* dz, long long ldd, int dz_dtype, float* colsum, void* workspace,
+                  const int32_t* label2bin, const int32_t* slices_host, const void* weights,
+                  int weights_dtype, const float* avg, int N, int C, int G, int classes, float* loss,
+                  float* lse, void* dz, long long ldd, int dz_dtype, float* colsum, void* workspace,
                   size_t workspace_bytes, void* stream);
 
 /* 1 if bags_fwd can run its fused kernel (logits == NULL) for this bin table: C <= 1280, G <= 6, C % 4 == 0,
  * bins tile [0, C) contiguously. */
 int bags_fused_eligible(const int32_t* slices_host, int G, int C);
 
-/* fc_cls + grouped softmax-CE (+ dz, colsum) in one call.
+/* fc_cls + grouped softmax-CE (+ dz, colsum) in one call; weights / weights_dtype as in bags_group_ce.
  *   logits == NULL : fused kernel -- the logits stay in registers and never reach HBM
  *                    (requires bags_fused_eligible); ldz is ignored.
- *   logits != NULL : bags_linear_fwd into `logits` followed by bags_group_ce (same arguments).
+ *   logits != NULL : bags_linear_act_fwd (fp32 output, no activation) into `logits` followed by bags_group_ce
+ *                    (same arguments).
  * colsum (optional) is [colsum_tiles, C] with colsum_tiles = ceil(N/128): per-128-row-tile partial column sums
  * of dz (written with plain stores, no pre-zeroing needed); their sum over tiles is sum_n dz[n, :].
+ * clear (optional, NULL / 0 = none): `clear_bytes` bytes at `clear` (16-byte aligned, a multiple of 16; typically the
+ * caller's dW) are set to zero -- by the fused kernel's idle warps while the MMAs run, or by a memset on the
+ * materialised route.  Together with `colsum` this lets bags_bwd run without any preparation work (flag
+ * BAGS_BWD_DW_PREZEROED, no column-sum job).
  * The fused kernel is launched with programmatic dependent launch: when the preceding kernel in the stream is
  * bags_sample_others / bags_mask_avg, its GEMM mainloop overlaps them and only the epilogue waits. */
 int bags_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
              const int64_t* labels, const int32_t* label2bin, const int32_t* slices_host,
-             const uint8_t* wmask, const float* avg, int N, int K, int C, int G, int classes,
+             const void* weights, int weights_dtype, const float* avg, int N, int K, int C, int G, int classes,
              int dtype, float* logits, long long ldz, float* loss, float* lse, void* dz,
              long long ldd, float* colsum, int colsum_tiles, void* workspace, size_t workspace_bytes,
-             void* stream);
+             void* clear, size_t clear_bytes, void* stream);
 
 /* ---- reweight head variant (GSBBoxHeadWith0Reweight, mmdet/models/bbox_heads/gs_bbox_head_with0_reweight.py:57-109):
- * per-(bin, RoI) fp32 weights instead of 0/1 masks.  EXPERIMENTAL: not yet run on a GPU. ----
+ * per-(bin, RoI) fp32 weights instead of 0/1 masks, consumed by bags_fwd / bags_group_ce as BAGS_WEIGHTS_F32. ----
  * bags_reweight: wfloat[g,n] = wmask[g,n] * cls_weight[g, label2bin[g, labels[n]]] for g >= 1 (bin 0: wmask as is),
- *                avg[g] = max(sum_n wfloat[g,n], 1).  cls_weight is [G, wstride] fp32 (row 0 unused, index 0 = "others").
- * bags_fwd_w / bags_group_ce_w: bags_fwd / bags_group_ce with `wfloat` [G,N] fp32 in place of the byte mask. */
+ *                avg[g] = max(sum_n wfloat[g,n], 1).  cls_weight is [G, wstride] fp32 (row 0 unused, index 0 = "others"). */
 int bags_reweight(const int64_t* labels, const int32_t* label2bin, const uint8_t* wmask, const float* cls_weight,
                   int wstride, int N, int G, int classes, float* wfloat, float* avg, void* stream);
-int bags_fwd_w(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
-               const int64_t* labels, const int32_t* label2bin, const int32_t* slices_host,
-               const float* wfloat, const float* avg, int N, int K, int C, int G, int classes,
-               int dtype, float* logits, long long ldz, float* loss, float* lse, void* dz,
-               long long ldd, float* colsum, int colsum_tiles, void* workspace, size_t workspace_bytes,
-               void* stream);
-int bags_group_ce_w(const float* logits, long long ldz, const int64_t* labels,
-                    const int32_t* label2bin, const int32_t* slices_host, const float* wfloat,
-                    const float* avg, int N, int C, int G, int classes, float* loss, float* lse,
-                    void* dz, long long ldd, int dz_dtype, float* colsum, void* workspace,
-                    size_t workspace_bytes, void* stream);
 
 /* bytes of `wscratch` bags_bwd needs (row-scaled copy of w + bias-gradient partials) */
 size_t bags_bwd_scratch_bytes(int C, long long ldw, int dtype);
@@ -148,29 +138,14 @@ size_t bags_bwd_scratch_bytes(int C, long long ldw, int dtype);
  *   dX[N,K]  = (gout ⊙ dz) w         dtype elements            (NULL to skip)
  * colsum: optional [colsum_tiles, C] partial column sums of dz from the forward; NULL => recomputed from dz.
  * wscratch: 256-byte aligned, bags_bwd_scratch_bytes() bytes; required when (dX and gout) or (db without colsum).
+ * flags: BAGS_BWD_DW_PREZEROED = dW is already zero on entry (stream-ordered), e.g. by bags_fwd's clear hook.
  * Launch structure: one small preparation kernel (zero dW, scaled W, column-sum partials) whose execution is
  * overlapped by the dW GEMM's mainloop (programmatic dependent launch), then the dX GEMM. */
+#define BAGS_BWD_DW_PREZEROED 1
 int bags_bwd(const void* dz, long long ldd, const void* x, long long ldx, const void* w,
              long long ldw, const float* gout, const int32_t* slices_host, const float* colsum,
              int colsum_tiles, float* dW, long long lddw, float* db, void* dX, long long lddx,
-             void* wscratch, size_t wscratch_bytes, int N, int K, int C, int G, int dtype, void* stream);
-
-/* bags_fwd with a "clear" hook: the fused kernel's idle epilogue warps set `clear_bytes` bytes at `clear` (16-byte
- * aligned, a multiple of 16; typically the caller's dW) to zero while the MMAs run.  Together with `colsum` this lets
- * bags_bwd_ex run without any preparation work (no zeroing job, no column-sum job). */
-int bags_fwd_ex(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
-                const int64_t* labels, const int32_t* label2bin, const int32_t* slices_host,
-                const uint8_t* wmask, const float* avg, int N, int K, int C, int G, int classes, int dtype,
-                float* logits, long long ldz, float* loss, float* lse, void* dz, long long ldd, float* colsum,
-                int colsum_tiles, void* workspace, size_t workspace_bytes, void* clear, size_t clear_bytes,
-                void* stream);
-
-/* bags_bwd with flags: BAGS_BWD_DW_PREZEROED = dW is already zero on entry (stream-ordered), e.g. by bags_fwd_ex. */
-#define BAGS_BWD_DW_PREZEROED 1
-int bags_bwd_ex(const void* dz, long long ldd, const void* x, long long ldx, const void* w,
-                long long ldw, const float* gout, const int32_t* slices_host, const float* colsum,
-                int colsum_tiles, float* dW, long long lddw, float* db, void* dX, long long lddx,
-                void* wscratch, size_t wscratch_bytes, int N, int K, int C, int G, int dtype, int flags, void* stream);
+             void* wscratch, size_t wscratch_bytes, int N, int K, int C, int G, int dtype, int flags, void* stream);
 
 /* scores[N,classes]: scores[:,0] = softmax(z[:,slice_0])[:,0];
  * scores[:,c] = softmax(z[:,slice_0])[:,1] * softmax(z[:,slice_g])[:,j] where cls2col[c] = start_g + j.
@@ -218,12 +193,12 @@ int bags_class_nms_dense(const float* boxes, int box_cols, const int32_t* order,
 
 /* test hook: launch `blocks` x `threads` threads that wait `micros` microseconds and exit */
 int bags_debug_spin(int blocks, int threads, int micros, void* stream);
-/* Test hook: the number of `cluster`-CTA clusters (threads, dynamic shared memory per CTA) that can be resident at once. */
-int bags_debug_max_clusters(int cluster, int threads, int smem_bytes);
 
 /* The head's trunk, the step before the path (SURVEY.md 8f-3; convfc_bbox_head.py:138-143 shared FCs + ReLU, :167 fc_reg):
- * out[N,C] = act(x[N,K] W[C,K]^T + bias), act = ReLU when relu != 0, on the wgmma GEMM of bags_linear_fwd.
- * dtype = operand dtype of x and W; out_dtype: BAGS_DTYPE_F32, or BAGS_DTYPE_BF16 (bf16 operands only: feeds the next layer). */
+ * out[N,C] = act(x[N,K] W[C,K]^T + bias), act = ReLU when relu != 0, on the wgmma GEMM.  With relu = 0 and fp32 output
+ * it is also fc_cls (the materialised logits of bags_fwd).
+ * dtype = operand dtype of x and W; out_dtype: BAGS_DTYPE_F32 (out and bias 16-byte aligned), or BAGS_DTYPE_BF16
+ * (bf16 operands only: feeds the next layer). */
 int bags_linear_act_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
                         void* out, long long ldo, int N, int K, int C, int dtype, int out_dtype, int relu,
                         void* stream);

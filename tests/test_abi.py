@@ -27,38 +27,50 @@ def test_header_symbols_exported():
     assert sorted(nat.SIGNATURES.keys()) == names, 'ctypes SIGNATURES out of sync with the header'
 
 
-def test_abi_version_and_workspace():
+def test_abi_version_2_and_workspace():
     lib = nat.lib()
-    assert lib.bags_abi_version() == nat.ABI_VERSION == 1
+    assert lib.bags_abi_version() == nat.ABI_VERSION == 2
     assert lib.bags_workspace_bytes() >= 4096
 
 
-def test_invalid_arguments_return_codes_not_exceptions():
+def test_invalid_arguments_return_error_codes():
+    """Bad shapes, dtypes, workspaces and bin tables through the single-entry-point signatures: error codes and
+    messages, never exceptions."""
     lib = nat.lib()
     # NULL operands
-    rc = lib.bags_linear_fwd(None, 0, None, 0, None, None, 0, 4, 8, 8, nat.DTYPE_BF16, None)
+    rc = lib.bags_linear_act_fwd(None, 0, None, 0, None, None, 0, 4, 8, 8, nat.DTYPE_BF16, nat.DTYPE_F32, 0, None)
     assert rc == -1 and b'NULL' in lib.bags_last_error()
     # bad dtype
     buf = (C.c_char * 64)()
     p = C.addressof(buf)
-    rc = lib.bags_linear_fwd(p, 8, p, 8, None, p, 8, 4, 8, 8, 7, None)
+    rc = lib.bags_linear_act_fwd(p, 8, p, 8, None, p, 8, 4, 8, 8, 7, nat.DTYPE_F32, 0, None)
     assert rc == -1 and b'dtype' in lib.bags_last_error()
     # group_ce: workspace too small / C not multiple of 4 / bad slices
     sl = nat.int32_array([0, 2, 2, 6])
-    rc = lib.bags_group_ce(p, 8, p, p, sl, None, None, 1, 8, 2, 4, p, None, None, 0, 0, None, p, 16, None)
+    rc = lib.bags_group_ce(p, 8, p, p, sl, None, nat.WEIGHTS_U8, None, 1, 8, 2, 4, p, None, None, 0, 0, None, p, 16, None)
     assert rc == -1 and b'workspace' in lib.bags_last_error()
     ws = lib.bags_workspace_bytes()
-    rc = lib.bags_group_ce(p, 8, p, p, sl, None, None, 1, 6, 2, 4, p, None, None, 0, 0, None, p, ws, None)
+    rc = lib.bags_group_ce(p, 8, p, p, sl, None, nat.WEIGHTS_U8, None, 1, 6, 2, 4, p, None, None, 0, 0, None, p, ws, None)
     assert rc == -1 and b'multiple of 4' in lib.bags_last_error()
     bad = nat.int32_array([0, 2, 1, 6])   # overlapping slices
-    rc = lib.bags_group_ce(p, 8, p, p, bad, None, None, 1, 8, 2, 4, p, None, None, 0, 0, None, p, ws, None)
+    rc = lib.bags_group_ce(p, 8, p, p, bad, None, nat.WEIGHTS_U8, None, 1, 8, 2, 4, p, None, None, 0, 0, None, p, ws, None)
     assert rc == -1 and b'pred_slice' in lib.bags_last_error()
     # too many bins
-    rc = lib.bags_sample_others(p, p, 4, 9, 4, 8.0, 1, p, p, None)
+    rc = lib.bags_sample_others(p, p, 4, 9, 4, 8.0, 1, None, p, p, None)
     assert rc == -1
     with pytest.raises(nat.BagsNativeError):
         nat.check(rc, 'bags_sample_others')
 
+
+def test_unknown_weights_dtype_is_rejected():
+    """weights_dtype other than BAGS_WEIGHTS_U8 / BAGS_WEIGHTS_F32 is a bad argument, reported before any launch."""
+    lib = nat.lib()
+    buf = (C.c_char * 64)()
+    p = C.addressof(buf)
+    sl = nat.int32_array([0, 2, 2, 6])
+    ws = lib.bags_workspace_bytes()
+    rc = lib.bags_group_ce(p, 8, p, p, sl, p, 2, None, 1, 8, 2, 4, p, None, None, 0, 0, None, p, ws, None)
+    assert rc == -1 and b'weights dtype 2' in lib.bags_last_error()
 
 def test_ops_refuse_cpu_tensors():
     """No CPU fallback: handing the product a CPU tensor is an error, not a slow path."""

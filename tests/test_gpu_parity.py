@@ -528,8 +528,9 @@ def test_split_backward_matches_oracle(env, N, mode, gname):
 @pytest.mark.parametrize('mode', [torch.float32, torch.bfloat16], ids=['fp32', 'bf16'])
 @pytest.mark.parametrize('N', [200, 512, 4096])
 def test_preparation_in_forward_matches_oracle(env, N, mode, fwd_colsum):
-    """dW zeroed by the forward kernel's clear hook (bags_fwd_ex) -- and optionally the bias-gradient partials from the
-    forward too -- then bags_bwd_ex(DW_PREZEROED): same gradients as the oracle; the hook really zeroes a dirty buffer."""
+    """dW zeroed by the forward kernel's clear hook (bags_fwd's clear argument) -- and optionally the bias-gradient
+    partials from the forward too -- then bags_bwd(DW_PREZEROED): same gradients as the oracle; the hook really zeroes a
+    dirty buffer."""
     ops, t, dt, l2b, ps = env
     x, W, b, labels, remapped = _problem(N, seed=77 + N)
     gout = GOUTS['nonuniform']

@@ -491,8 +491,8 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   auto kernel = wf ? bags_fwd_fused_kernel<TF32, true> : bags_fwd_fused_kernel<TF32, false>;
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   const int grid = Cfg::CLUSTER * ((p.N + Cfg::BLOCK_M - 1) / Cfg::BLOCK_M);
-  // PDL INVARIANT (also the sampler's): this kernel reads x, W, bias and labels BEFORE its griddepcontrol.wait (only the
-  // sampler's masks / avg and every global write come after it).  That is correct as long as those tensors are not
+  // PDL INVARIANT (also the sampler's): this kernel reads x, W, bias, labels and label2bin BEFORE its
+  // griddepcontrol.wait (only the sampler's masks / avg and every global write come after it).  That is correct as long as those tensors are not
   // produced by the immediately preceding kernel of the stream with an early launch_dependents trigger -- true for torch
   // kernels (they never trigger early) and for this library's own chain (the predecessor is the sampler / the previous
   // step's backward or exchange, none of which writes them).  A future producer that triggers early must be followed by

@@ -3,19 +3,24 @@
 //   z = x W^T + b  is accumulated in registers and never written to HBM.
 //
 // A cluster of 4 CTAs owns one 128-row tile of RoIs; CTA r holds logit columns [320r, 320r+320) of those rows.
-// Warpgroup 0 is the producer (one TMA thread; its other three warps load the per-row labels / weights and run the
-// optional clear hook while the MMAs run); warpgroups 1 and 2 each own 64 rows and keep their 64 x 320 fp32
-// accumulators in registers (two wgmma m64n160 per K step).  In the wgmma fragment a row is held by the four lanes
-// of a quad (80 columns each), so row reductions are a walk over the thread's own columns plus two quad shuffles.
-// Bins are contiguous column ranges, so every walk keeps a running (bin, value) pair and touches shared memory only
-// where the bin changes:
+// The CTA is two warpgroups and nothing else: each owns 64 rows and keeps its 64 x 320 fp32 accumulators in registers
+// (two wgmma m64n160 per K step).  Thread 0 also issues the TMA loads, and every thread loads a share of the per-row
+// labels / weights.  The CTA has no producer warp on purpose: a ninth warp puts three warps on one SM sub-partition,
+// whose 16K registers then cap every thread of the kernel at 168, too few for the 160 accumulators -- ptxas spills
+// and serialises the wgmma.  With eight warps each thread may use 255 registers, and the mainloop keeps one k-block
+// of MMAs in flight while it waits for the next stage.
+// In the wgmma fragment a row is held by the four lanes of a quad (80 columns each), so row reductions are a walk
+// over the thread's own columns plus two quad shuffles.  Bins are contiguous column ranges, so every walk keeps a
+// running (bin, value) pair and touches shared memory only where the bin changes:
 //
 //   accumulators := bias before the first MMA (the epilogue never adds it)
-//   pass A  : per row and bin, the max over this CTA's columns; pass B: sum exp(z - max)
+//   pass A  : per row and bin, the max m over this CTA's columns
+//   pass B  : z := e = exp(z - m) in place, sum e; z[target] is kept for the loss
 //   exchange: every CTA sends its (max, sum) per row and bin to the four CTAs of the cluster (st.async into
-//             distributed shared memory, completion counted on an mbarrier); each combines the four into the lse
-//   pass C  : dz~ = w/avg * (exp(z - lse) - onehot) -> operand dtype -> HBM ; column sums of dz~ (bias gradient) ;
-//             loss_bin += w/avg * (lse - z[target])
+//             distributed shared memory, completion counted on an mbarrier); each combines the four into the lse,
+//             loss_bin += w/avg * (lse - z[target]) where the target column is this CTA's
+//   pass C  : dz~ = e * exp(m - lse) * w/avg - onehot * w/avg -> operand dtype -> HBM ; column sums of dz~ (bias
+//             gradient).  One exponential per logit in all.
 //
 // reference semantics: gs_bbox_head_with0.py:91-112 (labels/weights), :134-171 (slices + CE),
 // cross_entropy_loss.py:9-19, losses/utils.py:26-53 (sum / avg_factor).
@@ -46,8 +51,8 @@ struct FusedFwdParams {
   void* dz;                 // [N, ldd] operand dtype, or nullptr (loss only)
   long long ldd;
   int want_dz;
-  // optional: a buffer the producer warpgroup's idle warps set to zero while the MMAs run (the caller's dW: the
-  // backward's split-K red.add then needs no zeroing job)
+  // optional: a buffer the kernel sets to zero after its epilogue (the caller's dW: the backward's split-K red.add
+  // then needs no zeroing job)
   float4* clear;
   long long clear_vecs;
 };
@@ -65,10 +70,10 @@ struct FusedCfg {
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int CLUSTER = 4;
-  static constexpr int NUM_THREADS = 384;
+  static constexpr int NUM_THREADS = 256;
   static constexpr int MAXG = 6;
   static constexpr int XCH_BYTES = CLUSTER * MAXG * BLOCK_M * 8;   // cluster-level partials, float2 (max, sum)
-  static constexpr int ROW_BYTES = 4 * MAXG * BLOCK_M * 4;          // tcol, coef, max, lse per (bin, row)
+  static constexpr int ROW_BYTES = 5 * MAXG * BLOCK_M * 4;          // tcol, coef, max, scale, z[target] per (bin, row)
   static constexpr int PART_BYTES = MAXG * 2 * 256 * 4;             // per-thread running partials
   static constexpr int MISC_BYTES = 3 * BLOCK_N * 4 /*bias, bin, colsum*/ + 64 /*loss*/ + 256 /*barriers*/;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + XCH_BYTES + ROW_BYTES + PART_BYTES + MISC_BYTES + 1024;
@@ -85,12 +90,6 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
   return r;
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {   // arrive without waiting
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 // 8-byte store into the shared memory of CTA `rank` of the cluster that also credits 8 bytes to that CTA's
 // mbarrier: the receiver just waits on its own barrier, no cluster-wide barrier / fence is involved
@@ -111,7 +110,7 @@ __device__ __forceinline__ unsigned int atom_add_release_gpu(unsigned int* addr,
 // WF = true: p.wmask points at fp32 per-(bin, RoI) weights instead of 0/1 bytes (the reweight head variant,
 // gs_bbox_head_with0_reweight.py:57-85)
 template <bool TF32, bool WF = false>
-__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(384, 1)
+__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(FusedCfg<TF32>::NUM_THREADS, 1)
 bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                       const FusedFwdParams p) {
   using Cfg = FusedCfg<TF32>;
@@ -126,8 +125,9 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   int* s_tcol = reinterpret_cast<int*>(reinterpret_cast<uint8_t*>(xch) + Cfg::XCH_BYTES);   // [MAXG][128]
   float* s_coef = reinterpret_cast<float*>(s_tcol + MAXG * BLOCK_M);                 // [MAXG][128] w / avg
   float* s_mrow = s_coef + MAXG * BLOCK_M;                                           // [MAXG][128] CTA row max
-  float* s_lse = s_mrow + MAXG * BLOCK_M;                                            // [MAXG][128]
-  float* s_part = s_lse + MAXG * BLOCK_M;                                            // [MAXG][2][256]
+  float* s_scale = s_mrow + MAXG * BLOCK_M;                                          // [MAXG][128] exp(max - lse) w / avg
+  float* s_zt = s_scale + MAXG * BLOCK_M;                                            // [MAXG][128] z[target column]
+  float* s_part = s_zt + MAXG * BLOCK_M;                                             // [MAXG][2][256]
   float* s_bias = s_part + MAXG * 2 * 256;                                           // [320]
   int* s_colbin = reinterpret_cast<int*>(s_bias + BLOCK_N);                          // [320] bin or -1
   float* s_colsum = reinterpret_cast<float*>(s_colbin + BLOCK_N);                    // [320]
@@ -138,7 +138,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   uint64_t* xch_bar = bars + 2 * STAGES;   // counts the bytes of the four CTAs' softmax partials landing in xch
   __shared__ int s_gs[kMaxG], s_ge[kMaxG];
 
-  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+  const int tid = threadIdx.x, wg = tid >> 7;   // warpgroup: rows [64 wg, 64 wg + 64) of the tile
   const uint32_t rank = cluster_ctarank();
   const int row_tile = blockIdx.x / Cfg::CLUSTER;
   const int m0 = row_tile * BLOCK_M;
@@ -150,7 +150,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     tma_prefetch_desc(&tmap_x);
     tma_prefetch_desc(&tmap_w);
 #pragma unroll
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], Cfg::NUM_THREADS); }
     mbar_init(xch_bar, 1);
     fence_mbar_init();
     // every row of every CTA of the cluster sends one float2 per bin
@@ -178,62 +178,39 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   __syncthreads();
   cluster_arrive();   // phase 1 of the cluster barrier; waited for just before the first remote shared-memory store
 
-  if (wg == 0) {
-    setmaxnreg_dec<40>();
-    if (tid == 0) {
-      // ===================== TMA producer =====================
-      for (int kb = 0; kb < p.kblocks; ++kb) {
-        const int stage = kb % STAGES;
-        const uint32_t phase = static_cast<uint32_t>(kb / STAGES) & 1u;
-        mbar_wait(&empty_bar[stage], phase ^ 1u);
-        mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-        const int k0 = kb * BLOCK_K;
-        uint8_t* sa = smem_a + stage * Cfg::A_BYTES;
-        uint8_t* sb = smem_b + stage * Cfg::B_BYTES;
-        tma_load_2d(sa, &tmap_x, &full_bar[stage], k0, m0);
-        tma_load_2d(sb, &tmap_w, &full_bar[stage], k0, n0);
-        tma_load_2d(sb + HALF_N * 128, &tmap_w, &full_bar[stage], k0, n0 + HALF_N);
-      }
-    } else if (tid >= 32) {
-      // ===================== row information (+ clear hook) under the mainloop =====================
-      pdl_wait();   // masks / avg come from the preceding sampler kernel (programmatic dependent launch)
-      const int ht = tid - 32;   // 0..95
-      if (p.clear != nullptr) {   // (a write: only after the wait -- the buffer may still be in use by an earlier kernel)
-        const long long stride = static_cast<long long>(gridDim.x) * 96;
-        const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-        for (long long i = static_cast<long long>(blockIdx.x) * 96 + ht; i < p.clear_vecs; i += stride) p.clear[i] = zero4;
-      }
-      for (int row_l = ht; row_l < BLOCK_M; row_l += 96) {
-        const int row = m0 + row_l;
-        long long lab = 0;
-        if (row < p.N) lab = __ldg(p.labels + row);
-        const bool lab_ok = (row < p.N) && lab >= 0 && lab < p.classes;
-        for (int g = 0; g < G; ++g) {
-          int t = lab_ok ? __ldg(p.l2b + g * p.classes + static_cast<int>(lab)) : 0;
-          t = (t >= 0 && t < s_ge[g] - s_gs[g]) ? t : 0;
-          float w = 0.f;
-          if (row < p.N)
-            w = (p.wmask != nullptr)
-                    ? (WF ? __ldg(reinterpret_cast<const float*>(p.wmask) + static_cast<long long>(g) * p.N + row)
-                          : static_cast<float>(__ldg(p.wmask + static_cast<long long>(g) * p.N + row)))
-                    : 1.0f;
-          const float inv_avg = 1.0f / (p.avg != nullptr ? __ldg(p.avg + g) : fmaxf(static_cast<float>(p.N), 1.0f));
-          s_tcol[g * BLOCK_M + row_l] = s_gs[g] + t;
-          s_coef[g * BLOCK_M + row_l] = w * inv_avg;
-        }
-      }
-      named_bar_arrive(1, 96 + 256);
+  // TMA producer (thread 0): k-block kb goes to stage kb % STAGES
+  auto issue = [&](int kb) {
+    const int stage = kb % STAGES;
+    mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+    const int k0 = kb * BLOCK_K;
+    uint8_t* sa = smem_a + stage * Cfg::A_BYTES;
+    uint8_t* sb = smem_b + stage * Cfg::B_BYTES;
+    tma_load_2d(sa, &tmap_x, &full_bar[stage], k0, m0);
+    tma_load_2d(sb, &tmap_w, &full_bar[stage], k0, n0);
+    tma_load_2d(sb + HALF_N * 128, &tmap_w, &full_bar[stage], k0, n0 + HALF_N);
+  };
+  if (tid == 0)
+    for (int kb = 0; kb < STAGES && kb < p.kblocks; ++kb) issue(kb);   // every stage starts out free
+
+  // ---- row information, part 1: the target column of every (row, bin) while the first stages load.  Labels and the
+  // label -> bin-label table are not produced by the preceding kernel, so they are read before griddepcontrol.wait.
+  // Thread t handles row t % 128 and bins t / 128, t / 128 + 2, t / 128 + 4. ----
+  static_assert(Cfg::NUM_THREADS == 2 * BLOCK_M && MAXG == 6, "row information: two threads per row, three bins each");
+  const int info_row = tid & (BLOCK_M - 1), info_g0 = tid / BLOCK_M;
+  const bool info_ok = m0 + info_row < p.N;
+  {
+    const long long lab = info_ok ? __ldg(p.labels + m0 + info_row) : -1;
+    const bool lab_ok = info_ok && lab >= 0 && lab < p.classes;
+    for (int g = info_g0; g < G; g += 2) {
+      int t = lab_ok ? __ldg(p.l2b + g * p.classes + static_cast<int>(lab)) : 0;
+      t = (t >= 0 && t < s_ge[g] - s_gs[g]) ? t : 0;
+      s_tcol[g * BLOCK_M + info_row] = s_gs[g] + t;
     }
-    __syncwarp();
-    cluster_wait();
-    return;
   }
 
-  // ===================== consumers: mainloop =====================
-  setmaxnreg_inc<232>();
-  const int cw = wg - 1, ctid = threadIdx.x - 128;
-  const int warp = tid >> 5, lane = tid & 31, q = lane & 3;
-  const int row_l0 = cw * 64 + warp * 16 + (lane >> 2);   // rows row_l0 and row_l0 + 8 of the tile
+  // ===================== mainloop =====================
+  const int warp = (tid >> 5) & 3, lane = tid & 31, q = lane & 3;
+  const int row_l0 = wg * 64 + warp * 16 + (lane >> 2);   // rows row_l0 and row_l0 + 8 of the tile
   float acc0[80], acc1[80];
 #pragma unroll
   for (int j = 0; j < HALF_N / 8; ++j) {
@@ -245,7 +222,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     }
   }
   {
-    const uint32_t a_off = cw * 8192;   // this warpgroup's 64 rows of the A tile
+    const uint32_t a_off = wg * 8192;   // this warpgroup's 64 rows of the A tile
     for (int kb = 0; kb < p.kblocks; ++kb) {
       const int stage = kb % STAGES;
       mbar_wait(&full_bar[stage], static_cast<uint32_t>(kb / STAGES) & 1u);
@@ -263,100 +240,149 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
         else      { wgmma_bf16_n160<0, 0>(acc0, adesc, bdesc0, 1u); wgmma_bf16_n160<0, 0>(acc1, adesc, bdesc1, 1u); }
       }
       wgmma_commit();
-      wgmma_wait<0>();
+      // keep this k-block's MMAs in flight; the previous k-block's are complete, so its stage can be refilled
+      wgmma_wait<1>();
       fence_regs(acc0);
       fence_regs(acc1);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (kb > 0) {
+        const int prev = kb - 1;
+        // every thread arrives and waits, only the TMA issue is thread 0's: with the barrier wait inside a branch
+        // that one thread takes, ptxas serialises the wgmma (C7518)
+        mbar_arrive(&empty_bar[prev % STAGES]);
+        if (prev + STAGES < p.kblocks) {   // once the whole CTA is done with the stage, refill it
+          mbar_wait(&empty_bar[prev % STAGES], static_cast<uint32_t>(prev / STAGES) & 1u);
+          if (tid == 0) issue(prev + STAGES);
+        }
+      }
     }
+    wgmma_wait<0>();   // (the last stage is never released: every k-block has been issued)
+    fence_regs(acc0);
+    fence_regs(acc1);
   }
   pdl_wait();   // every global write below comes after the predecessor grid
 
-  // walk the thread's 160 elements of row slot rr in column order: f(z, local column)
-#define BAGS_WALK(rr, F)                                                                           \
-  do {                                                                                             \
-    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) {                                       \
-      _Pragma("unroll") for (int e = 0; e < 2; ++e) F(acc0[4 * j + 2 * (rr) + e], 8 * j + 2 * q + e); \
-    }                                                                                              \
-    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) {                                       \
-      _Pragma("unroll") for (int e = 0; e < 2; ++e) F(acc1[4 * j + 2 * (rr) + e], HALF_N + 8 * j + 2 * q + e); \
-    }                                                                                              \
-  } while (0)
-
-  float mrow[2][MAXG], srow[2][MAXG];
+  // ---- row information, part 2: w / avg.  Masks and avg come from the preceding sampler kernel (programmatic
+  // dependent launch), so they are read after the wait; they are stored after pass A, which hides the latency ----
+  float info_coef[MAXG / 2];
 #pragma unroll
-  for (int rr = 0; rr < 2; ++rr) {
-    const int row_l = row_l0 + 8 * rr;
-    // ---- pass A: per-bin max over this thread's columns, then over the quad ----
-#pragma unroll
-    for (int g = 0; g < MAXG; ++g) s_part[(g * 2 + rr) * 256 + ctid] = -INFINITY;
-    {
-      int gc = -1;
-      float mc = -INFINITY;
-      auto stepA = [&](float z, int c) {
-        const int b = s_colbin[c];
-        if (b != gc) {
-          if (gc >= 0) s_part[(gc * 2 + rr) * 256 + ctid] = mc;
-          gc = b; mc = -INFINITY;
-        }
-        mc = fmaxf(mc, z);
-      };
-      BAGS_WALK(rr, stepA);
-      if (gc >= 0) s_part[(gc * 2 + rr) * 256 + ctid] = mc;
+  for (int i = 0; i < MAXG / 2; ++i) {
+    const int g = info_g0 + 2 * i, row = m0 + info_row;
+    float w = 0.f, inv_avg = 0.f;
+    if (g < G) {
+      if (info_ok)
+        w = (p.wmask != nullptr)
+                ? (WF ? __ldg(reinterpret_cast<const float*>(p.wmask) + static_cast<long long>(g) * p.N + row)
+                      : static_cast<float>(__ldg(p.wmask + static_cast<long long>(g) * p.N + row)))
+                : 1.0f;
+      inv_avg = 1.0f / (p.avg != nullptr ? __ldg(p.avg + g) : fmaxf(static_cast<float>(p.N), 1.0f));
     }
+    info_coef[i] = w * inv_avg;
+  }
+
+  // walk the thread's 2 x 160 elements in column order: f(z of row row_l0, z of row row_l0 + 8, local column)
+#define BAGS_WALK(F)                                                                                         \
+  do {                                                                                                       \
+    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) {                                                 \
+      _Pragma("unroll") for (int e = 0; e < 2; ++e) F(acc0[4 * j + e], acc0[4 * j + 2 + e], 8 * j + 2 * q + e); \
+    }                                                                                                        \
+    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) {                                                 \
+      _Pragma("unroll") for (int e = 0; e < 2; ++e)                                                          \
+        F(acc1[4 * j + e], acc1[4 * j + 2 + e], HALF_N + 8 * j + 2 * q + e);                                 \
+    }                                                                                                        \
+  } while (0)
+  // per-thread partials of (bin, row slot) -> s_part; the running pair is flushed where the bin changes
+#define BAGS_PART(g, rr) s_part[((g) * 2 + (rr)) * 256 + tid]
+
+  // ---- pass A: per-bin max over this thread's columns, then over the quad ----
 #pragma unroll
-    for (int g = 0; g < MAXG; ++g) {
-      float m = s_part[(g * 2 + rr) * 256 + ctid];
+  for (int g = 0; g < MAXG; ++g) BAGS_PART(g, 0) = BAGS_PART(g, 1) = -INFINITY;
+  {
+    int gc = -1;
+    float mc[2] = {-INFINITY, -INFINITY};
+    auto stepA = [&](float z0, float z1, int c) {
+      const int b = s_colbin[c];
+      if (b != gc) {
+        if (gc >= 0) { BAGS_PART(gc, 0) = mc[0]; BAGS_PART(gc, 1) = mc[1]; }
+        gc = b; mc[0] = mc[1] = -INFINITY;
+      }
+      mc[0] = fmaxf(mc[0], z0);
+      mc[1] = fmaxf(mc[1], z1);
+    };
+    BAGS_WALK(stepA);
+    if (gc >= 0) { BAGS_PART(gc, 0) = mc[0]; BAGS_PART(gc, 1) = mc[1]; }
+  }
+  for (int g = 0; g < G; ++g) {
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      float m = BAGS_PART(g, rr);
       m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
       m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-      mrow[rr][g] = m;
-      if (q == 0 && g < G) s_mrow[g * BLOCK_M + row_l] = m;
+      if (q == 0) s_mrow[g * BLOCK_M + row_l0 + 8 * rr] = m;
     }
-    __syncwarp();
-    // ---- pass B: per-bin sum of exp(z - max) ----
+  }
 #pragma unroll
-    for (int g = 0; g < MAXG; ++g) s_part[(g * 2 + rr) * 256 + ctid] = 0.f;
-    {
-      int gc = -1;
-      float mb = 0.f, sc = 0.f;
-      auto stepB = [&](float z, int c) {
-        const int b = s_colbin[c];
-        if (b != gc) {
-          if (gc >= 0) s_part[(gc * 2 + rr) * 256 + ctid] = sc;
-          gc = b; sc = 0.f;
-          mb = (b >= 0) ? s_mrow[b * BLOCK_M + row_l] * kLog2e : 0.f;
+  for (int i = 0; i < MAXG / 2; ++i)
+    if (info_g0 + 2 * i < G) s_coef[(info_g0 + 2 * i) * BLOCK_M + info_row] = info_coef[i];
+  __syncthreads();   // s_tcol / s_coef of every row; s_mrow of the quad
+
+  // ---- pass B: z := e = exp(z - max) in place, per-bin sum of e; z[target] for the loss ----
+#pragma unroll
+  for (int g = 0; g < MAXG; ++g) BAGS_PART(g, 0) = BAGS_PART(g, 1) = 0.f;
+  {
+    int gc = -1;
+    float mb[2] = {0.f, 0.f}, sc[2] = {0.f, 0.f};
+    int tc[2] = {-1, -1};
+    auto stepB = [&](float& z0, float& z1, int c) {
+      const int b = s_colbin[c];
+      if (b != gc) {
+        if (gc >= 0) { BAGS_PART(gc, 0) = sc[0]; BAGS_PART(gc, 1) = sc[1]; }
+        gc = b; sc[0] = sc[1] = 0.f;
+        if (b >= 0) {
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr) {
+            mb[rr] = s_mrow[b * BLOCK_M + row_l0 + 8 * rr] * kLog2e;
+            tc[rr] = s_tcol[b * BLOCK_M + row_l0 + 8 * rr] - n0;   // local column of the target
+          }
         }
-        if (b >= 0) sc += exp2f(fmaf(z, kLog2e, -mb));
-      };
-      BAGS_WALK(rr, stepB);
-      if (gc >= 0) s_part[(gc * 2 + rr) * 256 + ctid] = sc;
-    }
-#pragma unroll
-    for (int g = 0; g < MAXG; ++g) {
-      float s = s_part[(g * 2 + rr) * 256 + ctid];
-      s += __shfl_xor_sync(0xffffffffu, s, 1);
-      s += __shfl_xor_sync(0xffffffffu, s, 2);
-      srow[rr][g] = s;
-    }
+      }
+      if (b >= 0) {
+        if (c == tc[0]) s_zt[b * BLOCK_M + row_l0] = z0;
+        if (c == tc[1]) s_zt[b * BLOCK_M + row_l0 + 8] = z1;
+        z0 = exp2f(fmaf(z0, kLog2e, -mb[0]));
+        z1 = exp2f(fmaf(z1, kLog2e, -mb[1]));
+        sc[0] += z0;
+        sc[1] += z1;
+      }
+    };
+    BAGS_WALK(stepB);
+    if (gc >= 0) { BAGS_PART(gc, 0) = sc[0]; BAGS_PART(gc, 1) = sc[1]; }
   }
 
   // ---- exchange: publish (max, sum) of every (row, bin) to the four CTAs of the cluster ----
   cluster_wait();   // (phase 1, arrived during setup) every CTA of the cluster is running: remote smem is live
-  if (q == 0) {
+  {
     const uint32_t baddr = smem_u32(xch_bar);
+    for (int g = 0; g < G; ++g) {
 #pragma unroll
-    for (int rr = 0; rr < 2; ++rr)
+      for (int rr = 0; rr < 2; ++rr) {
+        float s = BAGS_PART(g, rr);
+        s += __shfl_xor_sync(0xffffffffu, s, 1);
+        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        if (q == 0) {
+          const int row_l = row_l0 + 8 * rr;
+          const uint32_t addr = smem_u32(&xch[(static_cast<int>(rank) * MAXG + g) * BLOCK_M + row_l]);
+          const float m = s_mrow[g * BLOCK_M + row_l];
 #pragma unroll
-      for (int g = 0; g < MAXG; ++g) {
-        if (g >= G) break;
-        const uint32_t addr = smem_u32(&xch[(static_cast<int>(rank) * MAXG + g) * BLOCK_M + row_l0 + 8 * rr]);
-#pragma unroll
-        for (uint32_t r = 0; r < 4; ++r) st_async_cluster_f2(addr, baddr, r, mrow[rr][g], srow[rr][g]);
+          for (uint32_t r = 0; r < 4; ++r) st_async_cluster_f2(addr, baddr, r, m, s);
+        }
       }
+    }
   }
+#undef BAGS_PART
   // all partials of all four CTAs have landed once the transaction count of xch_bar is reached; nobody leaves
   // before that, so no CTA exits while a peer still writes into its shared memory
   mbar_wait(xch_bar, 0);
+  __syncwarp();   // s_zt of the quad
   if (q == 0) {
 #pragma unroll
     for (int rr = 0; rr < 2; ++rr) {
@@ -370,19 +396,22 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
 #pragma unroll
         for (int s = 0; s < Cfg::CLUSTER; ++s) S += (v[s].x == -INFINITY) ? 0.f : v[s].y * exp2f((v[s].x - M) * kLog2e);
         const float lse_v = M + logf(S);
-        s_lse[g * BLOCK_M + row_l] = lse_v;
+        const float cf = s_coef[g * BLOCK_M + row_l];
+        s_scale[g * BLOCK_M + row_l] = exp2f((s_mrow[g * BLOCK_M + row_l] - lse_v) * kLog2e) * cf;
+        const int tcol = s_tcol[g * BLOCK_M + row_l];
+        if (cf != 0.f && tcol >= n0 && tcol < n0 + BLOCK_N) atomicAdd(&s_loss[g], cf * (lse_v - s_zt[g * BLOCK_M + row_l]));
         if (p.lse != nullptr && row < p.N && s_gs[g] >= n0 && s_gs[g] < n0 + BLOCK_N)
           p.lse[static_cast<long long>(row) * G + g] = lse_v;
       }
     }
   }
-  named_bar_sync(1, 96 + 256);   // s_tcol / s_coef from the producer warpgroup; s_lse of the quads
+  __syncwarp();   // s_scale of the quad
   // ---- pass C: dz, loss, column sums ----
   {
     const bool f32 = TF32;
     const bool want_cs = p.colsum != nullptr && p.want_dz;
     int gc = -1;
-    float lb[2] = {0.f, 0.f}, cf[2] = {0.f, 0.f};
+    float sc[2] = {0.f, 0.f}, cf[2] = {0.f, 0.f};
     int tc[2] = {-1, -1};
     uint8_t* dzrow[2];
     bool row_ok[2];
@@ -392,9 +421,9 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
       row_ok[rr] = p.want_dz && row < p.N;
       dzrow[rr] = reinterpret_cast<uint8_t*>(p.dz) + static_cast<long long>(row) * p.ldd * (f32 ? 4 : 2);
     }
-    auto stepC = [&](float z0a, float z0b, float z1a, float z1b, int c) {   // rows 0/1 x columns c, c + 1
+    auto stepC = [&](float e0a, float e0b, float e1a, float e1b, int c) {   // rows 0/1 x columns c, c + 1
       float d[2][2];
-      const float zz[2][2] = {{z0a, z0b}, {z1a, z1b}};
+      const float ee[2][2] = {{e0a, e0b}, {e1a, e1b}};
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int b = s_colbin[c + e];
@@ -403,23 +432,18 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
           if (b >= 0) {
 #pragma unroll
             for (int rr = 0; rr < 2; ++rr) {
-              lb[rr] = s_lse[b * BLOCK_M + row_l0 + 8 * rr];
+              sc[rr] = s_scale[b * BLOCK_M + row_l0 + 8 * rr];
               cf[rr] = s_coef[b * BLOCK_M + row_l0 + 8 * rr];
-              tc[rr] = s_tcol[b * BLOCK_M + row_l0 + 8 * rr];
+              tc[rr] = s_tcol[b * BLOCK_M + row_l0 + 8 * rr] - n0;
             }
           }
         }
-        const int col = n0 + c + e;
 #pragma unroll
         for (int rr = 0; rr < 2; ++rr) {
           float v = 0.f;
           if (b >= 0) {
-            const float z = zz[rr][e];
-            v = exp2f((z - lb[rr]) * kLog2e) * cf[rr];
-            if (col == tc[rr]) {
-              v -= cf[rr];
-              if (cf[rr] != 0.f) atomicAdd(&s_loss[b], cf[rr] * (lb[rr] - z));
-            }
+            v = ee[rr][e] * sc[rr];
+            if (c + e == tc[rr]) v -= cf[rr];
           }
           d[rr][e] = v;
         }
@@ -460,13 +484,19 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
       stepC(acc1[4 * j], acc1[4 * j + 1], acc1[4 * j + 2], acc1[4 * j + 3], HALF_N + 8 * j + 2 * q);
   }
 #undef BAGS_WALK
-  named_bar_sync(2, 256);   // s_loss / s_colsum complete
+  __syncthreads();   // s_loss / s_colsum complete
 
   if (p.colsum != nullptr && p.want_dz) {   // optional per-row-tile bias-gradient partials
-    for (int c = ctid; c < BLOCK_N; c += 256)
+    for (int c = tid; c < BLOCK_N; c += Cfg::NUM_THREADS)
       if (n0 + c < p.C) p.colsum[static_cast<long long>(row_tile) * p.C + n0 + c] = s_colsum[c];
   }
-  if (ctid < 32) {
+  if (p.clear != nullptr) {   // (a write: only after the wait -- the buffer may still be in use by an earlier kernel)
+    const long long stride = static_cast<long long>(gridDim.x) * Cfg::NUM_THREADS;
+    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long i = static_cast<long long>(blockIdx.x) * Cfg::NUM_THREADS + tid; i < p.clear_vecs; i += stride)
+      p.clear[i] = zero4;
+  }
+  if (tid < 32) {
     // ---- loss bookkeeping: per-CTA partials, the last CTA of the grid sums them in a fixed order ----
     unsigned int last = 0;
     if (lane == 0) {

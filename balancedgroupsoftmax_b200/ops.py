@@ -560,7 +560,7 @@ class GroupSoftmaxFunction(torch.autograd.Function):
         else:
             b32 = bias.float().contiguous()
         need_grad = any(ctx.needs_input_grad[:3])
-        # dW is allocated here and zeroed by the forward kernel's idle epilogue warps (its split-K red.add in the
+        # dW is allocated here and zeroed by the forward kernel (its split-K red.add in the
         # backward then needs no zeroing job); BAGS_FWD_COLSUM=1 also takes the bias-gradient partials from the forward
         dW = None
         ctx.grad_bucket = grad_bucket if (grad_bucket is not None and need_grad and ctx.needs_input_grad[1]) else None

@@ -110,7 +110,7 @@ int bags_fused_eligible(const int32_t* slices_host, int G, int C);
  * colsum (optional) is [colsum_tiles, C] with colsum_tiles = ceil(N/128): per-128-row-tile partial column sums
  * of dz (written with plain stores, no pre-zeroing needed); their sum over tiles is sum_n dz[n, :].
  * clear (optional, NULL / 0 = none): `clear_bytes` bytes at `clear` (16-byte aligned, a multiple of 16; typically the
- * caller's dW) are set to zero -- by the fused kernel's idle warps while the MMAs run, or by a memset on the
+ * caller's dW) are set to zero -- by the fused kernel after its epilogue, or by a memset on the
  * materialised route.  Together with `colsum` this lets bags_bwd run without any preparation work (flag
  * BAGS_BWD_DW_PREZEROED, no column-sum job).
  * The fused kernel is launched with programmatic dependent launch: when the preceding kernel in the stream is

@@ -170,20 +170,28 @@ extern "C" int bags_reload_env(void) {
 // Kernel launch.  pdl: with the programmatic-stream-serialization attribute (PDL; BAGS_PDL=0 turns it off), so the
 // kernel may begin while its predecessor in the stream is still running; every kernel of this library guards its
 // first access to predecessor-produced data (and its first write) with griddepcontrol.wait, so stream semantics are
-// preserved.
+// preserved.  cooperative: the runtime guarantees that all CTAs of the grid are resident at once, and fails the launch
+// when they cannot be (for kernels whose CTAs wait for each other).
 template <typename... KArgs, typename... Args>
 static cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl,
-                          Args&&... args) {
+                          bool cooperative, Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  unsigned n = 0;
+  if (pdl && env_int("BAGS_PDL", 1)) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n++].val.programmaticStreamSerializationAllowed = 1;
+  }
+  if (cooperative) {
+    attr[n].id = cudaLaunchAttributeCooperative;
+    attr[n++].val.cooperative = 1;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = (pdl && env_int("BAGS_PDL", 1)) ? 1 : 0;
+  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
 
@@ -229,7 +237,7 @@ static int launch_gemm(const GemmArgs& ga, const DeviceInfo& di, cudaStream_t st
   const int grid = units < di.num_sms ? units : di.num_sms;
 
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, pdl, ta, tb, p));
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, pdl, false, ta, tb, p));
   return BAGS_OK;
 }
 
@@ -243,7 +251,10 @@ static int pick_splits(int tiles, int kblocks, int num_sms) {
 // ----------------------------------------------------------------------------
 // public entry points
 // ----------------------------------------------------------------------------
-extern "C" size_t bags_workspace_bytes(void) { return 256 + 4096 * kMaxG * sizeof(float); }
+// workspace: loss counter (256 B) and per-CTA loss partials of up to 4096 CTAs, then the fused forward's exchange
+// (arrival counters and slots of its CTA groups)
+static constexpr size_t kLossWorkspaceBytes = 256 + 4096 * kMaxG * sizeof(float);
+extern "C" size_t bags_workspace_bytes(void) { return kLossWorkspaceBytes + kFusedXchBytes; }
 
 // y = act(x W^T + b): the head's shared FCs (ReLU), fc_reg and fc_cls (identity) on the same wgmma pipeline
 // (convfc_bbox_head.py:138-143,166-167: nn.Linear + ReLU through cuBLAS / ATen in the reference)
@@ -366,7 +377,7 @@ extern "C" int bags_sample_others(const int64_t* labels, const int32_t* label2bi
   const unsigned long long sd = static_cast<unsigned long long>(seed);
   const unsigned long long* st = reinterpret_cast<const unsigned long long*>(seed_step);
   auto kernel = N <= 4096 ? sample_others_kernel<4> : N <= 16384 ? sample_others_kernel<16> : sample_others_kernel<0>;
-  BAGS_CUDA(launch(kernel, dim3(G), dim3(1024), 0, stream, true, lab, label2bin, classes, G, N, ratio, sd, wmask, avg, st));
+  BAGS_CUDA(launch(kernel, dim3(G), dim3(1024), 0, stream, true, false, lab, label2bin, classes, G, N, ratio, sd, wmask, avg, st));
   return BAGS_OK;
 }
 
@@ -473,7 +484,7 @@ extern "C" int bags_fused_eligible(const int32_t* slices_host, int G, int C) {
 
 template <bool TF32>
 static int launch_fused_fwd(const void* x, long long ldx, const void* w, long long ldw, const FusedFwdParams& p0,
-                            void* dz, long long ldd, cudaStream_t stream, bool wf) {
+                            void* dz, long long ldd, int num_sms, cudaStream_t stream, bool wf) {
   using Cfg = FusedCfg<TF32>;
   const int dtype = TF32 ? BAGS_DTYPE_F32 : BAGS_DTYPE_BF16;
   CUtensorMap tx, tw;
@@ -490,14 +501,29 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   p.want_dz = dz != nullptr ? 1 : 0;
   auto kernel = wf ? bags_fwd_fused_kernel<TF32, true> : bags_fwd_fused_kernel<TF32, false>;
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  const int grid = Cfg::CLUSTER * ((p.N + Cfg::BLOCK_M - 1) / Cfg::BLOCK_M);
+  // persistent grid of CTA groups, all resident at once: the four CTAs of a group wait for each other's softmax
+  // partials.  At 4096 RoIs on 132 SMs this is 32 groups, i.e. 128 CTAs in one wave.
+  int per_sm = 0;
+  BAGS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, Cfg::NUM_THREADS, Cfg::SMEM_BYTES));
+  const int row_tiles = (p.N + Cfg::BLOCK_M - 1) / Cfg::BLOCK_M;
+  int groups = num_sms * per_sm / Cfg::RANKS;
+  if (groups > row_tiles) groups = row_tiles;
+  if (groups > kFusedMaxGroups) groups = kFusedMaxGroups;
+  if (groups < 1)
+    return fail(BAGS_ERR_CUDA, "bags_fwd: the fused kernel cannot keep %d CTAs resident (%d SMs, %d CTA(s) per SM)",
+                Cfg::RANKS, num_sms, per_sm);
+  const int grid = Cfg::RANKS * groups;
   // PDL INVARIANT (also the sampler's): this kernel reads x, W, bias, labels and label2bin BEFORE its
   // griddepcontrol.wait (only the sampler's masks / avg and every global write come after it).  That is correct as long as those tensors are not
   // produced by the immediately preceding kernel of the stream with an early launch_dependents trigger -- true for torch
   // kernels (they never trigger early) and for this library's own chain (the predecessor is the sampler / the previous
   // step's backward or exchange, none of which writes them).  A future producer that triggers early must be followed by
   // a non-PDL launch (BAGS_PDL=0) or move these reads behind the wait.
-  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, true, tx, tw, p));
+  // The cooperative launch fails (BAGS_ERR_CUDA) rather than hangs when the grid cannot be co-resident, e.g. on a part
+  // with fewer SMs than the device query reported or under an MPS limit.  Every CTA triggers its dependents only while
+  // it runs (after its first exchange), so a dependent grid cannot take an SM that a not yet resident CTA of this grid
+  // needs.
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, true, true, tx, tw, p));
   return BAGS_OK;
 }
 
@@ -551,8 +577,6 @@ extern "C" int bags_fwd(const void* x, long long ldx, const void* w, long long l
     return BAGS_OK;
   }
   if (bias != nullptr) BAGS_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "bags_fwd: bias must be 16-byte aligned");
-  const int grid = 4 * ((N + 127) / 128);
-  BAGS_REQUIRE(grid <= 4096, "bags_fwd: N=%d too large for the fused path's loss workspace", N);
   FusedFwdParams p{};
   p.N = N; p.C = C; p.K = K; p.gt = gt; p.bias = bias;
   p.labels = reinterpret_cast<const long long*>(labels);
@@ -560,11 +584,13 @@ extern "C" int bags_fwd(const void* x, long long ldx, const void* w, long long l
   p.loss = loss; p.lse = lse; p.colsum = colsum;
   p.counter = reinterpret_cast<unsigned int*>(workspace);
   p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  p.xch_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes);
+  p.xch = reinterpret_cast<float2*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes + kFusedXchCounterBytes);
   p.clear = reinterpret_cast<float4*>(clear);
   p.clear_vecs = static_cast<long long>(clear_bytes / 16);
   const bool wf = weights_dtype == BAGS_WEIGHTS_F32;
-  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, stream, wf)
-                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, stream, wf);
+  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, wf)
+                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, wf);
 }
 
 extern "C" int bags_reweight(const int64_t* labels, const int32_t* label2bin, const uint8_t* wmask,
@@ -612,7 +638,7 @@ static int launch_bwd_merged(const void* dz, long long ldd, const void* x, long 
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CW::SMEM_BYTES));
   const int units = bp.dw_units + bp.dx_units;
   const int grid = units < di.num_sms ? units : di.num_sms;
-  BAGS_CUDA(launch(kernel, dim3(grid), dim3(CW::NUM_THREADS), CW::SMEM_BYTES, stream, true, t_dzT, t_xT, t_dz, t_w, t_wp, bp));
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(CW::NUM_THREADS), CW::SMEM_BYTES, stream, true, false, t_dzT, t_xT, t_dz, t_w, t_wp, bp));
   return BAGS_OK;
 }
 
@@ -686,7 +712,7 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
     pp.skip_scale_if_uniform = merged ? 1 : 0;   // the merged kernel reads W itself when all gout[g] are equal
     const int grid = pp.z_ctas + pp.s_ctas + pp.c_ctas;
     if (grid > 0) {
-      BAGS_CUDA(launch(bf ? bwd_prep_kernel<false> : bwd_prep_kernel<true>, dim3(grid), dim3(256), 0, stream, true, pp));
+      BAGS_CUDA(launch(bf ? bwd_prep_kernel<false> : bwd_prep_kernel<true>, dim3(grid), dim3(256), 0, stream, true, false, pp));
       prep_launched = true;
     }
   }
@@ -844,7 +870,7 @@ extern "C" int bags_grad_allreduce(void* const* peer_bufs_host, void* mc_buf, lo
   const dim3 grid(static_cast<unsigned>(blocks)), block(static_cast<unsigned>(threads));
   auto kernel = mm ? (epoch ? bags_grad_allreduce_kernel<true, true> : bags_grad_allreduce_kernel<true, false>)
                   : (epoch ? bags_grad_allreduce_kernel<false, true> : bags_grad_allreduce_kernel<false, false>);
-  BAGS_CUDA(launch(kernel, grid, block, 0, stream, true, p));
+  BAGS_CUDA(launch(kernel, grid, block, 0, stream, true, false, p));
   return BAGS_OK;
 }
 

@@ -69,7 +69,8 @@ extern "C" {
 int bags_abi_version(void);
 const char* bags_last_error(void);
 
-/* bytes the caller must provide (zero-initialised ONCE) as `workspace` to bags_group_ce / bags_fwd */
+/* bytes the caller must provide (zero-initialised ONCE) as `workspace` to bags_group_ce / bags_fwd: one workspace per
+ * stream, kept across calls (it holds the fused forward's exchange counters, which are never reset) */
 size_t bags_workspace_bytes(void);
 
 /* wmask[G,N] (uint8 0/1) and avg[G] = max(sum w, 1): bin 0 all ones; bins >= 1 keep every in-bin row
@@ -114,7 +115,9 @@ int bags_fused_eligible(const int32_t* slices_host, int G, int C);
  * materialised route.  Together with `colsum` this lets bags_bwd run without any preparation work (flag
  * BAGS_BWD_DW_PREZEROED, no column-sum job).
  * The fused kernel is launched with programmatic dependent launch: when the preceding kernel in the stream is
- * bags_sample_others / bags_mask_avg, its GEMM mainloop overlaps them and only the epilogue waits. */
+ * bags_sample_others / bags_mask_avg, its GEMM mainloop overlaps them and only the epilogue waits.  It is also a
+ * cooperative launch of at most one 4-CTA group per 4 SMs that loops over the row tiles (no limit on N); where that
+ * grid cannot be resident at once, bags_fwd returns BAGS_ERR_CUDA. */
 int bags_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
              const int64_t* labels, const int32_t* label2bin, const int32_t* slices_host,
              const void* weights, int weights_dtype, const float* avg, int N, int K, int C, int G, int classes,

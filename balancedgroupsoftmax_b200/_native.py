@@ -39,6 +39,8 @@ SIGNATURES = {
     'bags_fused_eligible': (_i, [_vp, _i, _i]),
     'bags_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _vp, _i, _vp, _i, _i, _i, _i, _i, _i, _vp, _ll,
                       _vp, _vp, _vp, _ll, _vp, _i, _vp, _sz, _vp, _sz, _vp]),
+    'bags_ce_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _ll, _vp, _i, _vp, _sz,
+                         _vp, _sz, _vp]),
     'bags_reweight': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     'bags_bwd_scratch_bytes': (_sz, [_i, _ll, _i]),
     'bags_bwd': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _ll, _vp, _sz, _i, _i,

@@ -593,6 +593,62 @@ extern "C" int bags_fwd(const void* x, long long ldx, const void* w, long long l
                                   : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, wf);
 }
 
+// fc_cls + plain softmax CE over all C logits (ReweightBBoxHead, BBoxHead.loss): the fused kernel with one bin (0, C),
+// the label as the target column (l2b == nullptr) and fp32 per-RoI weights.  Unlike bags_fwd, C need not be a
+// multiple of 4 (1231 LVIS classes): the kernel reads the bias and writes the column sums with scalar accesses and
+// stores dz in pairs of even columns, which only needs ldd % 8 == 0.
+extern "C" int bags_ce_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
+                           const int64_t* labels, const float* weights, const float* avg, int N, int K, int C,
+                           int dtype, float* loss, float* acc, void* dz, long long ldd, float* colsum,
+                           int colsum_tiles, void* workspace, size_t workspace_bytes, void* clear, size_t clear_bytes,
+                           void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  constexpr int kMaxC = FusedCfg<false>::RANKS * FusedCfg<false>::BLOCK_N;
+  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "bags_ce_fwd: bad dtype %d", dtype);
+  BAGS_REQUIRE(N >= 0 && K >= 1 && C >= 1 && C <= kMaxC, "bags_ce_fwd: bad shape N=%d K=%d C=%d (1 <= C <= %d)", N, K,
+               C, kMaxC);
+  BAGS_REQUIRE(loss && workspace && (N == 0 || (x && w && labels)), "bags_ce_fwd: NULL argument");
+  BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "bags_ce_fwd: workspace too small (%zu < %zu)",
+               workspace_bytes, bags_workspace_bytes());
+  BAGS_REQUIRE(acc == nullptr || N <= (1 << 24),
+               "bags_ce_fwd: N=%d: the accuracy count is exact up to 2^24 rows only", N);
+  if (dz != nullptr) BAGS_REQUIRE(ldd >= C && (ldd % 8) == 0, "bags_ce_fwd: ldd=%lld must be a multiple of 8 and >= C", ldd);
+  if (colsum != nullptr)
+    BAGS_REQUIRE(colsum_tiles == (N + 127) / 128 || (N == 0 && colsum_tiles >= 1),
+                 "bags_ce_fwd: colsum must hold ceil(N/128) = %d row tiles of C floats (got %d)", (N + 127) / 128,
+                 colsum_tiles);
+  if (clear != nullptr)
+    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(clear) & 15) == 0 && (clear_bytes % 16) == 0,
+                 "bags_ce_fwd: the buffer to clear must be 16-byte aligned and a multiple of 16 bytes");
+  const int32_t slices[2] = {0, C};
+  GroupTable gt;
+  if (int rc = make_group_table(gt, slices, 1, C)) return rc;
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  if (N == 0) {
+    BAGS_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), stream));
+    if (acc != nullptr) BAGS_CUDA(cudaMemsetAsync(acc, 0, sizeof(float), stream));
+    if (colsum != nullptr) BAGS_CUDA(cudaMemsetAsync(colsum, 0, sizeof(float) * C * colsum_tiles, stream));
+    if (clear != nullptr) BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, stream));
+    return BAGS_OK;
+  }
+  FusedFwdParams p{};
+  p.N = N; p.C = C; p.K = K; p.gt = gt; p.bias = bias;
+  p.labels = reinterpret_cast<const long long*>(labels);
+  p.l2b = nullptr; p.classes = C;
+  p.wmask = reinterpret_cast<const uint8_t*>(weights); p.avg = avg;
+  p.loss = loss; p.acc = acc; p.acc_scale = static_cast<float>(100.0 / N);   // accuracy.py: correct * (100.0 / N)
+  p.lse = nullptr; p.colsum = colsum;
+  p.counter = reinterpret_cast<unsigned int*>(workspace);
+  p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  p.xch_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes);
+  p.xch = reinterpret_cast<float2*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes + kFusedXchCounterBytes);
+  p.clear = reinterpret_cast<float4*>(clear);
+  p.clear_vecs = static_cast<long long>(clear_bytes / 16);
+  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true)
+                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true);
+}
+
 extern "C" int bags_reweight(const int64_t* labels, const int32_t* label2bin, const uint8_t* wmask,
                              const float* cls_weight, int wstride, int N, int G, int classes, float* wfloat,
                              float* avg, void* stream_) {

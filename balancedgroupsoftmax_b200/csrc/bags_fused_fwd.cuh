@@ -33,7 +33,12 @@
 // cross_entropy_loss.py:9-19, losses/utils.py:26-53 (sum / avg_factor).
 //
 // Preconditions (checked on the host, otherwise the unfused path runs): C <= 1280, G <= 6, bins
-// tile [0, C) contiguously.
+// tile [0, C) contiguously.  The kernel itself takes any C: every column >= C is masked (bias preload, bins, dz pair
+// store, column sums), and the W tensor map zero-fills its rows >= C.
+//
+// The same kernel is the plain softmax-CE head (bags_ce_fwd, reweight_bbox_head.py / bbox_head.py:97-129): one bin
+// (0, C), l2b == nullptr (the label is the target column), fp32 per-RoI weights, and optionally the top-1 accuracy,
+// counted where the loss is formed (z[target] == row max) and reduced with the loss partials.
 #pragma once
 #include "bags_kernels.cuh"
 #include "bags_ptx.cuh"
@@ -46,11 +51,14 @@ struct FusedFwdParams {
   GroupTable gt;
   const float* bias;        // [C] or nullptr
   const long long* labels;  // [N]
-  const int* l2b;           // [G, classes]
+  const int* l2b;           // [G, classes], or nullptr: the label is the target column (one bin (0, C), plain CE)
   int classes;
   const uint8_t* wmask;     // [G, N] 0/1 bytes (or fp32 weights when the kernel is instantiated with WF) or nullptr (all ones)
   const float* avg;         // [G] or nullptr (N)
   float* loss;              // [G]
+  // optional top-1 accuracy of bin 0 (nullptr: none): acc[0] = acc_scale * #{rows : z[target] == row max}
+  float* acc;
+  float acc_scale;          // 100 / N
   float* lse;               // [N, G] or nullptr
   float* colsum;            // [row tiles, C] per-row-tile column sums of dz (plain stores) or nullptr
   float* part;              // [gridDim.x, kMaxG]
@@ -89,6 +97,7 @@ struct FusedCfg {
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ROW_BYTES + PART_BYTES + MISC_BYTES + 1024;
   static_assert(SMEM_BYTES <= 232448, "fused forward exceeds shared memory");
   static constexpr int SLOT_ELEMS = RANKS * MAXG * BLOCK_M;          // float2 per exchange slot
+  static_assert(MAXG < kMaxG, "the last per-CTA partial slot carries the accuracy count");
 };
 
 // Exchange workspace of the fused forward (the caller's per-stream workspace): at most kFusedMaxGroups CTA groups,
@@ -213,7 +222,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     const long long lab = info_ok ? __ldg(p.labels + m0 + info_row) : -1;
     const bool lab_ok = info_ok && lab >= 0 && lab < p.classes;
     for (int g = info_g0; g < G; g += 2) {
-      int t = lab_ok ? __ldg(p.l2b + g * p.classes + static_cast<int>(lab)) : 0;
+      int t = !lab_ok ? 0 : (p.l2b != nullptr ? __ldg(p.l2b + g * p.classes + static_cast<int>(lab)) : static_cast<int>(lab));
       t = (t >= 0 && t < s_ge[g] - s_gs[g]) ? t : 0;
       s_tcol[g * BLOCK_M + info_row] = s_gs[g] + t;
     }
@@ -424,7 +433,13 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
         const float cf = s_coef[g * BLOCK_M + row_l];
         s_scale[g * BLOCK_M + row_l] = exp2f((s_mrow[g * BLOCK_M + row_l] - lse_v) * kLog2e) * cf;
         const int tcol = s_tcol[g * BLOCK_M + row_l];
-        if (cf != 0.f && tcol >= n0 && tcol < n0 + BLOCK_N) atomicAdd(&s_loss[g], cf * (lse_v - s_zt[g * BLOCK_M + row_l]));
+        if (tcol >= n0 && tcol < n0 + BLOCK_N) {
+          const float zt = s_zt[g * BLOCK_M + row_l];
+          if (cf != 0.f) atomicAdd(&s_loss[g], cf * (lse_v - zt));
+          // top-1 accuracy (a comparison, not an argmax: a tie with the row max counts as correct); the count rides
+          // the spare last slot of the per-CTA loss partials
+          if (p.acc != nullptr && g == 0 && row < p.N && zt == M) atomicAdd(&s_loss[kMaxG - 1], 1.f);
+        }
         if (p.lse != nullptr && row < p.N && s_gs[g] >= n0 && s_gs[g] < n0 + BLOCK_N)
           p.lse[static_cast<long long>(row) * G + g] = lse_v;
       }
@@ -550,6 +565,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
       for (int g = 0; g < kMaxG; ++g) {
         const float t = warp_sum(accl[g]);
         if (lane == 0 && g < G) p.loss[g] = t;   // already divided by avg (coef = w/avg)
+        if (lane == 0 && g == kMaxG - 1 && p.acc != nullptr) p.acc[0] = t * p.acc_scale;   // exact count (< 2^24)
       }
       if (lane == 0) *p.counter = 0u;
     }

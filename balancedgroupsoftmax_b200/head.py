@@ -32,11 +32,12 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 import torch
 import torch.nn as nn
+import torch.nn.functional as F
 from torch.nn.modules.utils import _pair
 
 from . import ops
 from .fp16 import auto_fp16, force_fp32
-from .losses import CrossEntropyLoss, SmoothL1Loss  # noqa: F401  (registers them)
+from .losses import CrossEntropyLoss, SmoothL1Loss, accuracy  # noqa: F401  (registers them)
 from .registry import HEADS, build_loss, register
 from .tables import GroupTables, load_reference_files
 
@@ -183,6 +184,10 @@ class ClsScoreHandle(object):
         return func(*unwrap(tuple(args)), **unwrap(kwargs or {}))
 
 
+def _as_tensor(cls_score):
+    return cls_score.tensor() if isinstance(cls_score, ClsScoreHandle) else cls_score
+
+
 class FcClsFunction(torch.autograd.Function):
     """Materialised logits = x W^T + b on the wgmma GEMM (bags_linear_act_fwd); backward reuses bags_bwd."""
 
@@ -270,6 +275,52 @@ class BBoxHead(nn.Module):
         return fn([r.pos_bboxes for r in sampling_results], [r.neg_bboxes for r in sampling_results],
                   [r.pos_gt_bboxes for r in sampling_results], [r.pos_gt_labels for r in sampling_results],
                   rcnn_train_cfg, reg_classes, target_means=self.target_means, target_stds=self.target_stds)
+
+    @force_fp32(apply_to=('cls_score', 'bbox_pred'))
+    def loss(self, cls_score, bbox_pred, labels, label_weights, bbox_targets, bbox_weights, reduction_override=None):
+        """bbox_head.py:97-129: softmax CE over all classes (sample weights ``label_weights``), its top-1 ``acc`` and
+        the box loss.  The normaliser max(#(label_weights > 0), 1) stays on the device (no host sync)."""
+        losses = dict()
+        if cls_score is not None:
+            losses['loss_cls'] = self._cls_loss(cls_score, labels, label_weights, label_weights, reduction_override)
+            losses['acc'] = accuracy(_as_tensor(cls_score), labels)
+        if bbox_pred is not None:
+            losses['loss_bbox'] = self._bbox_loss(bbox_pred, labels, bbox_targets, bbox_weights, reduction_override)
+        return losses
+
+    def _cls_loss(self, cls_score, labels, weight, label_weights, reduction_override):
+        """loss_cls over materialised logits with avg_factor = max(#(label_weights > 0), 1) (None for 'sum')."""
+        avg = (label_weights > 0).sum(dtype=torch.float32).clamp_min(1.0)
+        return self.loss_cls(_as_tensor(cls_score), labels, weight,
+                             avg_factor=None if reduction_override == 'sum' else avg,
+                             reduction_override=reduction_override)
+
+    def _nms(self, bboxes, scores, cfg):
+        """multiclass_nms (mmdet/core/post_processing/bbox_nms.py): the native class-aware hard NMS, mmdet's own
+        function for the other NMS types."""
+        nms_cfg = _cfg_get(cfg, 'nms')
+        nms_type = _cfg_get(nms_cfg, 'type', 'nms')
+        if nms_type == 'nms' and os.environ.get('BAGS_NMS_NATIVE', '1') != '0':
+            # hard NMS (every configs/bags/* file): the device-side class-aware NMS -- one sort, one kernel, one sync
+            # instead of the reference's Python loop over 1230 classes (bbox_nms.py:34-54)
+            return ops.multiclass_nms(bboxes, scores, float(_cfg_get(cfg, 'score_thr')),
+                                      float(_cfg_get(nms_cfg, 'iou_thr')), int(_cfg_get(cfg, 'max_per_img')))
+        multiclass_nms = _mmdet_core('multiclass_nms')
+        if multiclass_nms is None:
+            raise NotImplementedError('nms type %r is not implemented natively (hard NMS is); install mmdetection v1.x '
+                                      'for soft-NMS' % (nms_type,))
+        return multiclass_nms(bboxes, scores, cfg.score_thr, cfg.nms, cfg.max_per_img)
+
+    @force_fp32(apply_to=('cls_score', 'bbox_pred'))
+    def get_det_bboxes(self, rois, cls_score, bbox_pred, img_shape, scale_factor, rescale=False, cfg=None):
+        """bbox_head.py:131-168: softmax over all classes, box decoding, class-aware NMS."""
+        if isinstance(cls_score, list):
+            cls_score = sum(_as_tensor(c) for c in cls_score) / float(len(cls_score))
+        scores = F.softmax(_as_tensor(cls_score), dim=1) if cls_score is not None else None
+        bboxes = self._decode(rois, bbox_pred, img_shape, scale_factor, rescale)
+        if cfg is None:
+            return bboxes, scores
+        return self._nms(bboxes, scores, cfg)
 
     def _bbox_loss(self, bbox_pred, labels, bbox_targets, bbox_weights, reduction_override):
         pos_inds = labels > 0
@@ -418,7 +469,82 @@ def _cfg_get(cfg, key, default=None):
     return getattr(cfg, key, default)
 
 
-class GSBBoxHeadWith0(SharedFCBBoxHead):
+_DTYPES = {'bf16': torch.bfloat16, 'bfloat16': torch.bfloat16, 'fp32': torch.float32, 'float32': torch.float32,
+           'tf32': torch.float32}
+
+
+class NativeFcClsHead(SharedFCBBoxHead):
+    """What the heads with a native classifier share: the shared FCs and fc_reg on this library's wgmma GEMMs, fc_cls
+    through ``FcClsFunction``, train / eval operand dtypes, and a training ``forward`` that returns a
+    ``ClsScoreHandle`` so that ``loss`` can run fc_cls and the loss in one fused kernel.
+
+    Execution keys, read from the head's own config dict (``gs_config`` / ``reweight_cfg``):
+        compute_dtype      'bf16' (default) or 'fp32' (TF32 products) for the fc_cls contraction in training
+        eval_compute_dtype 'fp32' (default) / 'bf16' for the test-time logits
+        native_trunk       True (default): shared FCs / fc_reg on this library's wgmma GEMMs
+        fuse_loss          True (default): training forward returns a ClsScoreHandle
+    """
+
+    def _init_execution(self, cfg):
+        cd = _cfg_get(cfg, 'compute_dtype', os.environ.get('BAGS_COMPUTE_DTYPE', 'bf16'))
+        self.compute_dtype = _DTYPES[str(cd).lower()]
+        # test-time logits: fp32 operands (TF32 products) by default -- a reference fp32 checkpoint scored through bf16
+        # operands moves logits by ~1e-2, which reaches the score_thr / NMS ranking of rare classes
+        ed = _cfg_get(cfg, 'eval_compute_dtype', os.environ.get('BAGS_EVAL_COMPUTE_DTYPE', 'fp32'))
+        self.eval_compute_dtype = _DTYPES[str(ed).lower()]
+        # shared FCs + fc_reg on this library's wgmma GEMMs (bias + ReLU in the epilogue) instead of nn.Linear / cuBLAS
+        self.native_trunk = bool(_cfg_get(cfg, 'native_trunk', os.environ.get('BAGS_NATIVE_TRUNK', '1') != '0'))
+        self.fuse_loss = bool(_cfg_get(cfg, 'fuse_loss', True))
+
+    @staticmethod
+    def _cuda_index(device) -> int:
+        device = torch.device(device)
+        if device.type != 'cuda':
+            raise ops.nat.BagsNativeError(
+                'the BAGS head hot path runs on an H100 GPU only (tensor on %s); there is no CPU fallback' % device)
+        return device.index if device.index is not None else torch.cuda.current_device()
+
+    def _active_dtype(self):
+        return self.compute_dtype if self.training else self.eval_compute_dtype
+
+    def _fc_cls_logits(self, x_cls):
+        return FcClsFunction.apply(x_cls, self.fc_cls.weight, self.fc_cls.bias, self._active_dtype())
+
+    def _use_native_trunk(self, x) -> bool:
+        return (self.native_trunk and x.is_cuda and not self.with_avg_pool and self.num_shared_fcs > 0
+                and self.num_cls_fcs == 0 and self.num_reg_fcs == 0)
+
+    def _trunk(self, x):
+        """convfc_bbox_head.py:132-160 for the FC-only configuration the BAGS configs use: flatten -> (Linear + ReLU) x
+        num_shared_fcs, each one LinearActFunction (wgmma GEMM, bias + ReLU in its epilogue; the activations travel
+        in the operand dtype)."""
+        if not self._use_native_trunk(x):
+            return super()._trunk(x)
+        cd = self._active_dtype()
+        act_dtype = torch.bfloat16 if cd == torch.bfloat16 else torch.float32
+        x = x.reshape(x.size(0), -1)
+        for fc in self.shared_fcs:
+            x = ops.LinearActFunction.apply(x, fc.weight, fc.bias, True, cd, act_dtype)
+        return x, x
+
+    def _fc_reg(self, x_reg):
+        if self.native_trunk and x_reg.is_cuda:
+            return ops.LinearActFunction.apply(x_reg, self.fc_reg.weight, self.fc_reg.bias, False, self._active_dtype(),
+                                               torch.float32)
+        return self.fc_reg(x_reg)
+
+    @auto_fp16()
+    def forward(self, x):
+        x_cls, x_reg = self._trunk(x)
+        bbox_pred = self._fc_reg(x_reg) if self.with_reg else None
+        if not self.with_cls:
+            return None, bbox_pred
+        if self.training and self.fuse_loss and torch.is_grad_enabled():
+            return ClsScoreHandle(self, x_cls), bbox_pred
+        return self._fc_cls_logits(x_cls), bbox_pred
+
+
+class GSBBoxHeadWith0(NativeFcClsHead):
     """Balanced Group Softmax head (gs_bbox_head_with0.py:14-380), fused H100 execution.
 
     Extra, optional ``gs_config`` keys (all default to reference behaviour where one exists):
@@ -468,22 +594,12 @@ class GSBBoxHeadWith0(SharedFCBBoxHead):
         self.fg_splits = [torch.from_numpy(s) for s in tables.fg_splits]
         self.others_sample_ratio = float(_cfg_get(gs_config, 'others_sample_ratio'))
 
-        cd = _cfg_get(gs_config, 'compute_dtype', os.environ.get('BAGS_COMPUTE_DTYPE', 'bf16'))
-        self.compute_dtype = {'bf16': torch.bfloat16, 'bfloat16': torch.bfloat16, 'fp32': torch.float32,
-                              'float32': torch.float32, 'tf32': torch.float32}[str(cd).lower()]
-        # test-time logits: fp32 operands (TF32 products) by default -- a reference fp32 checkpoint scored through bf16
-        # operands moves logits by ~1e-2, which reaches the score_thr / NMS ranking of rare classes
-        ed = _cfg_get(gs_config, 'eval_compute_dtype', os.environ.get('BAGS_EVAL_COMPUTE_DTYPE', 'fp32'))
-        self.eval_compute_dtype = {'bf16': torch.bfloat16, 'bfloat16': torch.bfloat16, 'fp32': torch.float32,
-                                   'float32': torch.float32, 'tf32': torch.float32}[str(ed).lower()]
-        # shared FCs + fc_reg on this library's wgmma GEMMs (bias + ReLU in the epilogue) instead of nn.Linear / cuBLAS
-        self.native_trunk = bool(_cfg_get(gs_config, 'native_trunk', os.environ.get('BAGS_NATIVE_TRUNK', '1') != '0'))
+        self._init_execution(gs_config)
         # opt-in: CUDA-graph replay per recurring RoI count behind loss() (api.GraphCachedHeadLoss)
         self.graph_cache = bool(_cfg_get(gs_config, 'graph_cache', os.environ.get('BAGS_GRAPH_CACHE', '0') == '1'))
         self._graph_loss = None
         self.sampler = str(_cfg_get(gs_config, 'sampler', 'device'))
         assert self.sampler in ('device', 'numpy')
-        self.fuse_loss = bool(_cfg_get(gs_config, 'fuse_loss', True))
         self._device_tables: Dict[int, ops.DeviceTables] = {}
         self._sample_calls = 0
         self.last_sample = None  # (wmask [G,N] uint8, avg [G]) of the latest loss() call, for inspection
@@ -512,56 +628,12 @@ class GSBBoxHeadWith0(SharedFCBBoxHead):
 
     # ---- device-side tables -------------------------------------------------------------
     def device_tables(self, device) -> ops.DeviceTables:
-        device = torch.device(device)
-        if device.type != 'cuda':
-            raise ops.nat.BagsNativeError(
-                'the BAGS head hot path runs on an H100 GPU only (tensor on %s); there is no CPU fallback' % device)
-        idx = device.index if device.index is not None else torch.cuda.current_device()
+        idx = self._cuda_index(device)
         dt = self._device_tables.get(idx)
         if dt is None:
-            dt = ops.DeviceTables.from_tables(self.tables, device)
+            dt = ops.DeviceTables.from_tables(self.tables, torch.device(device))
             self._device_tables[idx] = dt
         return dt
-
-    # ---- forward ------------------------------------------------------------------------
-    def _active_dtype(self):
-        return self.compute_dtype if self.training else self.eval_compute_dtype
-
-    def _fc_cls_logits(self, x_cls):
-        return FcClsFunction.apply(x_cls, self.fc_cls.weight, self.fc_cls.bias, self._active_dtype())
-
-    def _use_native_trunk(self, x) -> bool:
-        return (self.native_trunk and x.is_cuda and not self.with_avg_pool and self.num_shared_fcs > 0
-                and self.num_cls_fcs == 0 and self.num_reg_fcs == 0)
-
-    def _trunk(self, x):
-        """convfc_bbox_head.py:132-160 for the FC-only configuration the BAGS configs use: flatten -> (Linear + ReLU) x
-        num_shared_fcs, each one LinearActFunction (wgmma GEMM, bias + ReLU in its epilogue; the activations travel
-        in the operand dtype)."""
-        if not self._use_native_trunk(x):
-            return super()._trunk(x)
-        cd = self._active_dtype()
-        act_dtype = torch.bfloat16 if cd == torch.bfloat16 else torch.float32
-        x = x.reshape(x.size(0), -1)
-        for fc in self.shared_fcs:
-            x = ops.LinearActFunction.apply(x, fc.weight, fc.bias, True, cd, act_dtype)
-        return x, x
-
-    def _fc_reg(self, x_reg):
-        if self.native_trunk and x_reg.is_cuda:
-            return ops.LinearActFunction.apply(x_reg, self.fc_reg.weight, self.fc_reg.bias, False, self._active_dtype(),
-                                               torch.float32)
-        return self.fc_reg(x_reg)
-
-    @auto_fp16()
-    def forward(self, x):
-        x_cls, x_reg = self._trunk(x)
-        bbox_pred = self._fc_reg(x_reg) if self.with_reg else None
-        if not self.with_cls:
-            return None, bbox_pred
-        if self.training and self.fuse_loss and torch.is_grad_enabled():
-            return ClsScoreHandle(self, x_cls), bbox_pred
-        return self._fc_cls_logits(x_cls), bbox_pred
 
     # ---- label remap / sampling ---------------------------------------------------------
     def _next_seed(self) -> int:
@@ -676,18 +748,7 @@ class GSBBoxHeadWith0(SharedFCBBoxHead):
         bboxes = self._decode(rois, bbox_pred, img_shape, scale_factor, rescale)
         if cfg is None:
             return bboxes, scores
-        nms_cfg = _cfg_get(cfg, 'nms')
-        nms_type = _cfg_get(nms_cfg, 'type', 'nms')
-        if nms_type == 'nms' and os.environ.get('BAGS_NMS_NATIVE', '1') != '0':
-            # hard NMS (every configs/bags/* file): the device-side class-aware NMS -- one sort, one kernel, one sync
-            # instead of the reference's Python loop over 1230 classes (bbox_nms.py:34-54)
-            return ops.multiclass_nms(bboxes, scores, float(_cfg_get(cfg, 'score_thr')),
-                                      float(_cfg_get(nms_cfg, 'iou_thr')), int(_cfg_get(cfg, 'max_per_img')))
-        multiclass_nms = _mmdet_core('multiclass_nms')
-        if multiclass_nms is None:
-            raise NotImplementedError('nms type %r is not implemented natively (hard NMS is); install mmdetection v1.x '
-                                      'for soft-NMS' % (nms_type,))
-        return multiclass_nms(bboxes, scores, cfg.score_thr, cfg.nms, cfg.max_per_img)
+        return self._nms(bboxes, scores, cfg)
 
 
 class GSBBoxHead(GSBBoxHeadWith0):
@@ -734,5 +795,76 @@ class GSBBoxHeadWith0Reweight(GSBBoxHeadWith0):
         return ops.reweight(labels, self.device_tables(dev), wmask, self._cls_weight_dev[idx])
 
 
-for _cls in (BBoxHead, ConvFCBBoxHead, SharedFCBBoxHead, GSBBoxHeadWith0, GSBBoxHead, GSBBoxHeadWith0Reweight):
+class ReweightBBoxHead(NativeFcClsHead):
+    """Class-reweighted softmax head (mmdet/models/bbox_heads/reweight_bbox_head.py), the re-weighting baselines of
+    configs/transferred/faster_rcnn_r50_fpn_1x_lvis_reweight{all,head,head_bf,head_bfocal,head_bours}.py:
+    softmax CE over all ``num_classes`` logits, each RoI weighted by ``cls_weight[label]``, normalised by
+    max(#(label_weights > 0), 1); ``loss`` also returns the top-1 accuracy ``acc``.  The test path is BBoxHead's
+    (softmax, decode, NMS).
+
+    ``reweight_cfg.cls_weight`` names a ``torch.load``-able 1-D tensor of ``num_classes`` weights (the files
+    ``python -m balancedgroupsoftmax_b200.tables --cls-weight ...`` writes); ``reweight_cfg.cls_weights`` may pass the
+    vector directly.  It is kept as fp32 (the reference casts the gathered weights to fp32, cross_entropy_loss.py:15)
+    and copied to a GPU when a loss first runs there.  ``reweight_cfg`` also takes the execution keys of
+    ``NativeFcClsHead``.
+
+    In training with a softmax ``CrossEntropyLoss`` (reduction 'mean') as ``loss_cls``, fc_cls, the weighted CE and the
+    accuracy run in one fused kernel (``ops.SoftmaxCEFunction``: the [N, C] logits never reach memory) and the
+    backward in one bags_bwd call; dX is computed only when the RoI features need a gradient.  Any other ``loss_cls``
+    (e.g. the FocalLoss of reweighthead_bfocal) or ``reduction_override`` runs the reference's op sequence on
+    materialised logits."""
+
+    def __init__(self, num_fcs=2, fc_out_channels=1024, reweight_cfg=None, *args, **kwargs):
+        super().__init__(num_fcs=num_fcs, fc_out_channels=fc_out_channels, *args, **kwargs)
+        assert reweight_cfg is not None, 'ReweightBBoxHead needs reweight_cfg'
+        w = _cfg_get(reweight_cfg, 'cls_weights')
+        if w is None:
+            w = torch.load(_cfg_get(reweight_cfg, 'cls_weight'), map_location='cpu')
+        w = torch.as_tensor(np.asarray(w.detach().cpu() if torch.is_tensor(w) else w)).to(torch.float32).reshape(-1)
+        if w.numel() != self.num_classes:
+            raise ValueError('ReweightBBoxHead: %d class weights for %d classes' % (w.numel(), self.num_classes))
+        self.cls_weight = w          # a plain attribute as in the reference (not in the state dict)
+        self._cls_weight_dev: Dict[int, torch.Tensor] = {}
+        self._init_execution(reweight_cfg)
+
+    def _reweight(self, labels):
+        """cls_weight[labels] (reweight_bbox_head.py:29-33), gathered on the labels' device."""
+        idx = self._cuda_index(labels.device) if labels.is_cuda else None
+        if idx is None:
+            return self.cls_weight[labels]
+        w = self._cls_weight_dev.get(idx)
+        if w is None:
+            w = self._cls_weight_dev[idx] = self.cls_weight.to(labels.device)
+        return w[labels]
+
+    def _fused_loss_ok(self) -> bool:
+        lc = self.loss_cls
+        return (type(lc).__name__ == 'CrossEntropyLoss' and not getattr(lc, 'use_sigmoid', False)
+                and not getattr(lc, 'use_mask', False) and getattr(lc, 'reduction', None) == 'mean')
+
+    @force_fp32(apply_to=('cls_score', 'bbox_pred'))
+    def loss(self, cls_score, bbox_pred, labels, label_weights, bbox_targets, bbox_weights, reduction_override=None):
+        losses = dict()
+        if cls_score is not None:
+            assert reduction_override in (None, 'none', 'mean', 'sum')
+            weight = self._reweight(labels)
+            if (reduction_override in (None, 'mean') and self._fused_loss_ok() and isinstance(cls_score, ClsScoreHandle)
+                    and cls_score._logits is None):
+                avg = (label_weights > 0).sum(dtype=torch.float32).clamp_min(1.0).reshape(1)
+                acc = torch.empty((1,), dtype=torch.float32, device=labels.device)
+                loss = ops.SoftmaxCEFunction.apply(cls_score.x_cls, self.fc_cls.weight, self.fc_cls.bias, labels,
+                                                   weight, avg, self.compute_dtype, acc)[0]
+                lw = self.loss_cls.loss_weight
+                losses['loss_cls'] = loss if lw == 1.0 else loss * lw
+                losses['acc'] = acc
+            else:
+                losses['loss_cls'] = self._cls_loss(cls_score, labels, weight, label_weights, reduction_override)
+                losses['acc'] = accuracy(_as_tensor(cls_score), labels)
+        if bbox_pred is not None:
+            losses['loss_bbox'] = self._bbox_loss(bbox_pred, labels, bbox_targets, bbox_weights, reduction_override)
+        return losses
+
+
+for _cls in (BBoxHead, ConvFCBBoxHead, SharedFCBBoxHead, GSBBoxHeadWith0, GSBBoxHead, GSBBoxHeadWith0Reweight,
+             ReweightBBoxHead):
     register(HEADS, _cls)

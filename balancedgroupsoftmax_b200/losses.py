@@ -69,6 +69,20 @@ class CrossEntropyLoss(nn.Module):
         return self.loss_weight * _reduce(loss, weight, reduction, avg_factor)
 
 
+def accuracy(pred, target, topk=1):
+    """Top-k accuracy in percent, mmdet/models/losses/accuracy.py:4-21 (``losses['acc']`` of BBoxHead.loss)."""
+    assert isinstance(topk, (int, tuple))
+    return_single = isinstance(topk, int)
+    if return_single:
+        topk = (topk, )
+    maxk = max(topk)
+    _, pred_label = pred.topk(maxk, dim=1)
+    pred_label = pred_label.t()
+    correct = pred_label.eq(target.view(1, -1).expand_as(pred_label))
+    res = [correct[:k].reshape(-1).float().sum(0, keepdim=True).mul_(100.0 / pred.size(0)) for k in topk]
+    return res[0] if return_single else res
+
+
 class SmoothL1Loss(nn.Module):
 
     def __init__(self, beta=1.0, reduction='mean', loss_weight=1.0):

@@ -128,6 +128,7 @@ def linear_fwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor],
     N, K = x.shape
     Cc = w.shape[0]
     if out is None:
+        # (any C: the GEMM epilogue stores column pairs only where ldo is even, single floats otherwise -- 1231 classes)
         out = torch.empty((N, Cc), dtype=torch.float32, device=x.device)
     if bias is not None:
         bias = bias.contiguous()
@@ -265,6 +266,53 @@ def fused_fwd(x, w, bias, labels, dt: DeviceTables, wmask, avg, logits: Optional
         ws.numel(), nat.ptr(clear), clear.numel() * clear.element_size() if clear is not None else 0,
         _stream_ptr(dev)), 'bags_fwd')
     return loss, logits, lse, dz, colsum
+
+
+def ce_fwd(x, w, bias, labels, weights=None, avg=None, want_acc: bool = False, want_dz: bool = True,
+           want_colsum: bool = False, clear: Optional[torch.Tensor] = None, acc_out: Optional[torch.Tensor] = None):
+    """bags_ce_fwd: fc_cls + softmax CE over all C logits in the fused kernel (ReweightBBoxHead / BBoxHead.loss).
+    Returns (loss [1], acc [1] | None, dz [N, pad_cols(C)] | None, colsum [ceil(N/128), C] | None).
+
+    ``weights``: fp32 [N] per-RoI weights (None: 1); ``avg``: fp32 [1] normaliser on the device (None: N).
+    ``want_acc``: also the top-1 accuracy in percent (ties with the row maximum count as correct), written into
+    ``acc_out`` when given.  ``clear``: as in ``fused_fwd``."""
+    _require_cuda(x, w, bias, labels, weights, avg, clear, acc_out)
+    x, w = _row_major(x), _row_major(w)
+    if x.dtype != w.dtype:
+        raise nat.BagsNativeError('x (%s) and w (%s) must share a dtype' % (x.dtype, w.dtype))
+    labels = labels.contiguous()
+    N, K = x.shape
+    Cc = w.shape[0]
+    dev = x.device
+    if bias is not None:
+        assert bias.dtype == torch.float32
+        bias = bias.contiguous()
+    if weights is not None:
+        weights = weights.to(torch.float32).contiguous()
+        assert weights.numel() == N
+    if avg is not None:
+        assert avg.dtype == torch.float32 and avg.numel() >= 1
+    loss = torch.empty((1,), dtype=torch.float32, device=dev)
+    acc = None
+    if want_acc:
+        acc = acc_out if acc_out is not None else torch.empty((1,), dtype=torch.float32, device=dev)
+        assert acc.dtype == torch.float32 and acc.numel() == 1
+    dz = colsum = None
+    ldd = 0
+    if want_dz:
+        ldd = pad_cols(Cc)
+        dz = torch.empty((N, ldd), dtype=x.dtype, device=dev)
+        if want_colsum:
+            colsum = torch.empty((max((N + 127) // 128, 1), Cc), dtype=torch.float32, device=dev)
+    if clear is not None:
+        assert clear.is_contiguous() and (clear.numel() * clear.element_size()) % 16 == 0
+    ws = _workspace(dev)
+    nat.check(nat.lib().bags_ce_fwd(
+        x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(), nat.ptr(weights),
+        nat.ptr(avg), N, K, Cc, _dtype_code(x.dtype), loss.data_ptr(), nat.ptr(acc), nat.ptr(dz), ldd, nat.ptr(colsum),
+        colsum.shape[0] if colsum is not None else 0, ws.data_ptr(), ws.numel(), nat.ptr(clear),
+        clear.numel() * clear.element_size() if clear is not None else 0, _stream_ptr(dev)), 'bags_ce_fwd')
+    return loss, acc, dz, colsum
 
 
 _scratch_cache: Dict[Tuple, torch.Tensor] = {}
@@ -471,6 +519,7 @@ def _bf16_operand(t: torch.Tensor) -> torch.Tensor:
 
 
 def _single_slice_tables(cols: int, device) -> DeviceTables:
+    """One bin (0, cols): the table of bags_bwd for a plain layer or the softmax-CE head."""
     return DeviceTables(1, 1, cols, torch.zeros(1, 1, dtype=torch.int32, device=device),
                         torch.zeros(1, dtype=torch.int32, device=device), nat.int32_array([0, cols]),
                         np.array([[0, cols]], dtype=np.int64))
@@ -524,6 +573,49 @@ PREP_IN_FORWARD = os.environ.get('BAGS_PREP_IN_FORWARD', '1') != '0'
 FWD_COLSUM = os.environ.get('BAGS_FWD_COLSUM', '0') == '1'
 
 
+def _fc_cls_operands(x, weight, bias, compute_dtype):
+    """(xc, wc, b32): the fc_cls operands the fused forward reads.  bf16: fp32 masters are cast (the weight only when
+    it changed); float32: fp32 operands, TF32 products.  The bias is always fp32."""
+    if compute_dtype == torch.bfloat16:
+        xc = _row_major(x) if x.dtype == torch.bfloat16 else cast_bf16(_row_major(x.float()))
+        wc = _bf16_operand(weight)      # fp32 master: re-cast only when the parameter changed (version counter)
+    elif compute_dtype == torch.float32:
+        if x.dtype != torch.float32 or weight.dtype != torch.float32:
+            raise nat.BagsNativeError('float32 compute needs float32 x and weight')
+        xc, wc = _row_major(x), _row_major(weight)
+    else:
+        raise nat.BagsNativeError('compute_dtype must be torch.bfloat16 or torch.float32')
+    if bias is None or (bias.dtype == torch.float32 and bias.is_contiguous()):
+        b32 = bias
+    else:
+        b32 = bias.float().contiguous()
+    return xc, wc, b32
+
+
+def _save_param_dtypes(ctx, x, weight, bias) -> None:
+    ctx.x_dtype = x.dtype
+    ctx.w_dtype = weight.dtype
+    ctx.has_bias = bias is not None
+    ctx.bias_dtype = None if bias is None else bias.dtype
+
+
+def _gout(grad_loss: torch.Tensor) -> torch.Tensor:
+    return grad_loss if (grad_loss.dtype == torch.float32 and grad_loss.is_contiguous()) \
+        else grad_loss.to(torch.float32).contiguous()
+
+
+def _grads_in_param_dtypes(ctx, dX, dW, db):
+    """dX, dW, db in the dtypes of x, the weight and the bias (the kernels produce dX in the operand dtype, dW / db
+    in fp32)."""
+    if dX is not None and dX.dtype != ctx.x_dtype:
+        dX = dX.to(ctx.x_dtype)
+    if dW is not None and dW.dtype != ctx.w_dtype:
+        dW = dW.to(ctx.w_dtype)
+    if db is not None and db.dtype != ctx.bias_dtype:
+        db = db.to(ctx.bias_dtype)
+    return dX, dW, db
+
+
 class GroupSoftmaxFunction(torch.autograd.Function):
     """losses[G] = BAGS(fc_cls(x)) with a fused backward.
 
@@ -546,19 +638,7 @@ class GroupSoftmaxFunction(torch.autograd.Function):
         the returned weight / bias gradients ARE the bucket views, holding the mean over ranks."""
         _require_cuda(x, weight, bias, labels)
         # (autograd does not record inside Function.forward: the inputs are used as they are, no detach() round trips)
-        if compute_dtype == torch.bfloat16:
-            xc = _row_major(x) if x.dtype == torch.bfloat16 else cast_bf16(_row_major(x.float()))
-            wc = _bf16_operand(weight)      # fp32 master: re-cast only when the parameter changed (version counter)
-        elif compute_dtype == torch.float32:
-            if x.dtype != torch.float32 or weight.dtype != torch.float32:
-                raise nat.BagsNativeError('float32 compute needs float32 x and weight')
-            xc, wc = _row_major(x), _row_major(weight)
-        else:
-            raise nat.BagsNativeError('compute_dtype must be torch.bfloat16 or torch.float32')
-        if bias is None or (bias.dtype == torch.float32 and bias.is_contiguous()):
-            b32 = bias
-        else:
-            b32 = bias.float().contiguous()
+        xc, wc, b32 = _fc_cls_operands(x, weight, bias, compute_dtype)
         need_grad = any(ctx.needs_input_grad[:3])
         # dW is allocated here and zeroed by the forward kernel (its split-K red.add in the
         # backward then needs no zeroing job); BAGS_FWD_COLSUM=1 also takes the bias-gradient partials from the forward
@@ -578,10 +658,7 @@ class GroupSoftmaxFunction(torch.autograd.Function):
         ctx.dW = dW
         ctx.colsum = colsum if dW is not None else None
         ctx.dt = dt
-        ctx.x_dtype = x.dtype
-        ctx.w_dtype = weight.dtype
-        ctx.has_bias = bias is not None
-        ctx.bias_dtype = None if bias is None else bias.dtype
+        _save_param_dtypes(ctx, x, weight, bias)
         if need_grad:
             ctx.save_for_backward(xc, wc, dz)
         return loss
@@ -591,8 +668,7 @@ class GroupSoftmaxFunction(torch.autograd.Function):
     def backward(ctx, grad_loss):
         xc, wc, dz = ctx.saved_tensors
         need_dx, need_dw, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        gout = grad_loss if (grad_loss.dtype == torch.float32 and grad_loss.is_contiguous()) \
-            else grad_loss.to(torch.float32).contiguous()
+        gout = _gout(grad_loss)
         dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
         bucket = ctx.grad_bucket
         if bucket is not None and need_dw:
@@ -613,13 +689,47 @@ class GroupSoftmaxFunction(torch.autograd.Function):
             dW, db, dX = fused_bwd(dz, xc, wc, gout, ctx.dt, ctx.colsum, need_dw=need_dw,
                                    need_db=(need_db and ctx.has_bias), need_dx=need_dx,
                                    dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None)
-        if dX is not None and dX.dtype != ctx.x_dtype:
-            dX = dX.to(ctx.x_dtype)
-        if dW is not None and dW.dtype != ctx.w_dtype:
-            dW = dW.to(ctx.w_dtype)
-        if db is not None and db.dtype != ctx.bias_dtype:
-            db = db.to(ctx.bias_dtype)
+        dX, dW, db = _grads_in_param_dtypes(ctx, dX, dW, db)
         return dX, dW, db, None, None, None, None, None, None, None
+
+
+class SoftmaxCEFunction(torch.autograd.Function):
+    """loss[1] = softmax CE of fc_cls(x) over all C logits, per-RoI weighted (ReweightBBoxHead.loss) -- the
+    single-bin counterpart of ``GroupSoftmaxFunction``, with the same operand casting:
+
+    forward : bags_ce_fwd (fused fc_cls GEMM + softmax-CE; logits stay on chip; saves dz~; optional top-1 accuracy
+              into ``acc_out``, a [1] fp32 tensor, which is not differentiable)
+    backward: bags_bwd over the single slice (0, C); dX only when x needs a gradient (head-only training freezes
+              the trunk), dW zeroed by the forward kernel."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, labels, weights, avg, compute_dtype, acc_out=None):
+        _require_cuda(x, weight, bias, labels)
+        xc, wc, b32 = _fc_cls_operands(x, weight, bias, compute_dtype)
+        need_grad = any(ctx.needs_input_grad[:3])
+        dW = None
+        if need_grad and ctx.needs_input_grad[1] and PREP_IN_FORWARD:
+            dW = torch.empty((wc.shape[0], wc.shape[1]), dtype=torch.float32, device=xc.device)
+        loss, _, dz, _ = ce_fwd(xc, wc, b32, labels, weights, avg, want_acc=acc_out is not None, want_dz=need_grad,
+                                clear=dW, acc_out=acc_out)
+        ctx.dW = dW
+        ctx.num_cols = wc.shape[0]
+        _save_param_dtypes(ctx, x, weight, bias)
+        if need_grad:
+            ctx.save_for_backward(xc, wc, dz)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss):
+        xc, wc, dz = ctx.saved_tensors
+        need_dx, need_dw, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
+        dW, db, dX = fused_bwd(dz, xc, wc, _gout(grad_loss), _single_slice_tables(ctx.num_cols, xc.device), None,
+                               need_dw=need_dw, need_db=(need_db and ctx.has_bias), need_dx=need_dx,
+                               dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None)
+        dX, dW, db = _grads_in_param_dtypes(ctx, dX, dW, db)
+        return dX, dW, db, None, None, None, None, None
 
 
 class GroupCEFunction(torch.autograd.Function):

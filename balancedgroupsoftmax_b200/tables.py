@@ -167,10 +167,64 @@ def instance_counts_from_annotations(ann_file: str) -> Dict[int, int]:
     return counts
 
 
+CLS_WEIGHT_FILES = {'inv': 'cls_weight.pt', 'bf': 'cls_weight_bf.pt', 'bours': 'cls_weight_bours.pt'}
+
+
+def class_weights(instance_counts: Mapping[int, int], num_classes: int = 1231, kind: str = 'inv') -> np.ndarray:
+    """Per-class loss weights of ReweightBBoxHead, float64 [num_classes] (index 0 = background), restating
+    tools/lvis_analyse.py with its quirks:
+
+      'inv'   get_cate_weight (:338-365): 1 / count with the background count set to 1, divided by the foreground
+              mean, background weight 1, clipped to [0.1, 5]                                  -> cls_weight.pt
+      'bf'    get_cate_weight_bf (:370-405): class-balanced (1 - beta) / (1 - beta^count), beta = 0.999, with the
+              background count 3 x the foreground total, divided by the mean over all classes, not clipped
+                                                                                              -> cls_weight_bf.pt
+      'bours' get_cate_weight_bours (:409-445): class-balanced weights of the foreground only, divided by their mean,
+              background weight 1, clipped to [0.1, 5]                                        -> cls_weight_bours.pt
+
+    A category with no instance gets an infinite raw weight, as in the reference (clipped to 5 where it clips)."""
+    counts = np.zeros((num_classes,), dtype=np.float64)
+    for cid, c in instance_counts.items():
+        counts[cid] = c
+    beta = 0.999
+    with np.errstate(divide='ignore', invalid='ignore'):
+        if kind == 'inv':
+            counts[0] = 1
+            weight = np.ones_like(counts) / counts
+            weight = weight / weight[1:].mean()
+            weight[0] = 1
+        elif kind == 'bf':
+            counts[0] = np.sum(counts[1:]) * 3
+            tmp = np.ones_like(counts)
+            weight = (tmp - beta) / (tmp - np.power(beta, counts))
+            return weight / np.mean(weight)
+        elif kind == 'bours':
+            fg = counts[1:]
+            tmp = np.ones_like(fg)
+            w = (tmp - beta) / (tmp - np.power(beta, fg))
+            weight = np.ones((num_classes,), dtype=np.float64)
+            weight[1:] = w / np.mean(w)
+        else:
+            raise ValueError('unknown class-weight kind %r (inv, bf, bours)' % (kind,))
+    weight = np.where(weight > 5, 5, weight)
+    return np.where(weight < 0.1, 0.1, weight)
+
+
+def save_class_weights(weight: np.ndarray, directory: str, kind: str) -> str:
+    """torch.save the float64 weight tensor under the file name the reference's configs load."""
+    import torch
+    os.makedirs(directory, exist_ok=True)
+    path = os.path.join(directory, CLS_WEIGHT_FILES[kind])
+    torch.save(torch.from_numpy(np.asarray(weight, dtype=np.float64)), path)
+    return path
+
+
 def main(argv=None) -> int:
     """python -m balancedgroupsoftmax_b200.tables --ann lvis_v0.5_train.json --out data/lvis
     Writes label2binlabel.pt, pred_slice_with0.pt and valsplit.pkl in the reference's formats
-    (tools/lvis_analyse.py: get_cate_gs + get_split; --thresholds generalises the 5-bin split)."""
+    (tools/lvis_analyse.py: get_cate_gs + get_split; --thresholds generalises the 5-bin split).
+    With --cls-weight it writes the class-weight files of the re-weighting baselines instead
+    (get_cate_weight / _bf / _bours: cls_weight.pt, cls_weight_bf.pt, cls_weight_bours.pt)."""
     import argparse
     ap = argparse.ArgumentParser(description=main.__doc__)
     ap.add_argument('--ann', help='LVIS-style training annotation json (categories with instance_count)')
@@ -178,6 +232,8 @@ def main(argv=None) -> int:
                     help='no annotation file: seeded long-tailed synthetic counts')
     ap.add_argument('--num-classes', type=int, default=None, help='labels incl. background (default: max id + 1)')
     ap.add_argument('--thresholds', type=int, nargs='+', default=list(DEFAULT_THRESHOLDS))
+    ap.add_argument('--cls-weight', nargs='+', choices=sorted(CLS_WEIGHT_FILES), default=None,
+                    help='write the per-class weight file(s) of ReweightBBoxHead instead of the group tables')
     ap.add_argument('--out', required=True)
     args = ap.parse_args(argv)
     if args.ann:
@@ -187,6 +243,12 @@ def main(argv=None) -> int:
     else:
         ap.error('give --ann or --synthetic')
     num_classes = args.num_classes or (max(counts) + 1)
+    if args.cls_weight:
+        for kind in args.cls_weight:
+            w = class_weights(counts, num_classes, kind)
+            path = save_class_weights(w, args.out, kind)
+            print('%s: min %.4g max %.4g -> %s' % (kind, float(w.min()), float(w.max()), path))
+        return 0
     tables = build_group_tables(counts, num_classes, args.thresholds)
     paths = save_reference_files(tables, args.out)
     print('bins: %s' % ', '.join('%d+1' % len(s) if i else '2' for i, s in enumerate([None] + tables.fg_splits)))

@@ -18,6 +18,8 @@
  *     mmdet/models/losses/cross_entropy_loss.py:9-19,86-103 ;
  *     mmdet/models/losses/utils.py:26-53
  *   fc_cls + loss in one call                             bags_fwd
+ *   ReweightBBoxHead.loss: fc_cls + weighted softmax CE   bags_ce_fwd
+ *     + accuracy (reweight_bbox_head.py:36-55)
  *   autograd backward of the above (dW, db, dX)           bags_bwd
  *     triggered at mmdet/core/utils/dist_utils.py:53
  *   GSBBoxHeadWith0._merge_score                          bags_merge_scores
@@ -124,6 +126,21 @@ int bags_fwd(const void* x, long long ldx, const void* w, long long ldw, const f
              int dtype, float* logits, long long ldz, float* loss, float* lse, void* dz,
              long long ldd, float* colsum, int colsum_tiles, void* workspace, size_t workspace_bytes,
              void* clear, size_t clear_bytes, void* stream);
+
+/* fc_cls + softmax cross-entropy over all C logits (ReweightBBoxHead, mmdet/models/bbox_heads/reweight_bbox_head.py;
+ * BBoxHead.loss, bbox_head.py:97-129), logits kept on chip -- the fused kernel of bags_fwd with the single bin (0, C):
+ *   loss[0] = sum_n w[n] * (logsumexp(z[n,:]) - z[n, labels[n]]) / avg[0]      (weights NULL => w = 1, avg NULL => N)
+ *   acc[0]  = 100 * #{n : z[n, labels[n]] == max_c z[n, c]} / N                (optional, NULL to skip; mmdet accuracy,
+ *             topk = 1.  A tie with the row maximum counts as correct.  N <= 2^24 when requested: the count is exact)
+ * weights: fp32 [N] per-RoI weights (cls_weight[labels] for ReweightBBoxHead).
+ * dz, colsum, clear, workspace: as bags_fwd (ldd % 8 == 0, colsum [ceil(N/128), C]); dW, db and dX then come from
+ * bags_bwd with the single slice (0, C) and gout = dL/dloss[0].
+ * 1 <= C <= 1280, any C (not only multiples of 4); labels in [0, C) (a label outside it is scored against column 0).
+ * N == 0: loss = 0, acc = 0. */
+int bags_ce_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias, const int64_t* labels,
+                const float* weights, const float* avg, int N, int K, int C, int dtype, float* loss, float* acc,
+                void* dz, long long ldd, float* colsum, int colsum_tiles, void* workspace, size_t workspace_bytes,
+                void* clear, size_t clear_bytes, void* stream);
 
 /* ---- reweight head variant (GSBBoxHeadWith0Reweight, mmdet/models/bbox_heads/gs_bbox_head_with0_reweight.py:57-109):
  * per-(bin, RoI) fp32 weights instead of 0/1 masks, consumed by bags_fwd / bags_group_ce as BAGS_WEIGHTS_F32. ----

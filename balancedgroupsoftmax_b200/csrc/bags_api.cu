@@ -494,11 +494,23 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   if (rc) return rc;
   if (dz != nullptr && (reinterpret_cast<uintptr_t>(dz) & 15) != 0)
     return fail(BAGS_ERR_INVALID, "bags_fwd: dz must be 16-byte aligned");
+  // dz [N, C] with row stride ldd: the kernel stages each tile's dz in shared memory and stores it with TMA in boxes
+  // of 128 bytes x 128 rows.  A TMA store writes whole 16-byte pieces at the tensor's right edge, so the map spans the
+  // columns up to the last 16-byte boundary at or before C; the kernel writes the rest, and the padding columns
+  // [C, ldd) stay untouched.
+  const int dz_tma_cols = p0.C & ~(16 / Cfg::ELT - 1);
+  CUtensorMap tdz{};
+  if (dz != nullptr && dz_tma_cols > 0) {
+    rc = make_tmap(&tdz, dz, dtype, dz_tma_cols, p0.N, ldd, Cfg::BOX_COLS, Cfg::BLOCK_M);
+    if (rc) return rc;
+  }
   FusedFwdParams p = p0;
   p.dz = dz;
   p.ldd = ldd;
+  p.dz_tma_cols = dz != nullptr ? dz_tma_cols : 0;
   p.kblocks = (p.K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
   p.want_dz = dz != nullptr ? 1 : 0;
+  p.timing = g_timing;   // rows [0, grid) (grid <= 4 * kFusedMaxGroups); the gradient exchange stamps from row 4096
   auto kernel = wf ? bags_fwd_fused_kernel<TF32, true> : bags_fwd_fused_kernel<TF32, false>;
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   // persistent grid of CTA groups, all resident at once: the four CTAs of a group wait for each other's softmax
@@ -523,7 +535,7 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   // with fewer SMs than the device query reported or under an MPS limit.  Every CTA triggers its dependents only while
   // it runs (after its first exchange), so a dependent grid cannot take an SM that a not yet resident CTA of this grid
   // needs.
-  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, true, true, tx, tw, p));
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, true, true, tx, tw, tdz, p));
   return BAGS_OK;
 }
 

@@ -18,23 +18,26 @@
 // of MMAs in flight while it waits for the next stage.
 // In the wgmma fragment a row is held by the four lanes of a quad (80 columns each), so row reductions are a walk
 // over the thread's own columns plus two quad shuffles.  Bins are contiguous column ranges, so every walk keeps a
-// running (bin, value) pair and touches shared memory only where the bin changes:
+// running (bin, value) pair and touches shared memory only where the bin changes.  A thread holds two columns of
+// each 8-column chunk, and a CTA's 320 columns hold at most G + 1 bin changes, so the bin is resolved per chunk: a
+// chunk inside the running bin is walked without any lookup, only the few others element by element.
 //
 //   accumulators := bias before the first MMA (the epilogue never adds it)
 //   pass A  : per row and bin, the max m over this CTA's columns
 //   pass B  : z := e = exp(z - m) in place, sum e; z[target] is kept for the loss
 //   exchange: every CTA stores its (max, sum) per row and bin to the group's slot in global memory and counts its
-//             arrival on the group's counter; once all four have arrived, each reads the four partials back (L2) and
-//             combines them into the lse, loss_bin += w/avg * (lse - z[target]) where the target column is this CTA's
-//   pass C  : dz~ = e * exp(m - lse) * w/avg - onehot * w/avg -> operand dtype -> HBM ; column sums of dz~ (bias
-//             gradient).  One exponential per logit in all.
+//             arrival on the group's counter (and zeroes its share of the optional `clear` buffer while it waits);
+//             once all four have arrived, each reads the four partials back (L2) and combines them into the lse,
+//             loss_bin += w/avg * (lse - z[target]) where the target column is this CTA's
+//   pass C  : dz~ = e * exp(m - lse) * w/avg - onehot * w/avg -> operand dtype -> the idle pipeline stages -> TMA
+//             stores to HBM ; column sums of dz~ (bias gradient) from the staged tile.  One exponential per logit.
 //
 // reference semantics: gs_bbox_head_with0.py:91-112 (labels/weights), :134-171 (slices + CE),
 // cross_entropy_loss.py:9-19, losses/utils.py:26-53 (sum / avg_factor).
 //
 // Preconditions (checked on the host, otherwise the unfused path runs): C <= 1280, G <= 6, bins
-// tile [0, C) contiguously.  The kernel itself takes any C: every column >= C is masked (bias preload, bins, dz pair
-// store, column sums), and the W tensor map zero-fills its rows >= C.
+// tile [0, C) contiguously.  The kernel itself takes any C: every column >= C is masked (bias preload, bins, column
+// sums), the W tensor map zero-fills its rows >= C, and dz is stored for columns < C and rows < N only.
 //
 // The same kernel is the plain softmax-CE head (bags_ce_fwd, reweight_bbox_head.py / bbox_head.py:97-129): one bin
 // (0, C), l2b == nullptr (the label is the target column), fp32 per-RoI weights, and optionally the top-1 accuracy,
@@ -70,10 +73,18 @@ struct FusedFwdParams {
   void* dz;                 // [N, ldd] operand dtype, or nullptr (loss only)
   long long ldd;
   int want_dz;
-  // optional: a buffer the kernel sets to zero after its epilogue (the caller's dW: the backward's split-K red.add
-  // then needs no zeroing job)
+  // dz columns [0, dz_tma_cols) leave through TMA stores (the extent of tmap_dz, 0: none), [dz_tma_cols, C) through
+  // plain stores.  At the right edge of a tensor a TMA store writes whole 16-byte pieces, so the map ends at the last
+  // 16-byte boundary at or before C, and the padding columns [C, ldd) stay untouched.
+  int dz_tma_cols;
+  // optional: a buffer the kernel sets to zero while its CTAs wait for their peers' softmax partials (the caller's dW:
+  // the backward's split-K red.add then needs no zeroing job)
   float4* clear;
   long long clear_vecs;
+  // optional debug timeline (bags_debug_set_timing), [gridDim.x][8] %globaltimer stamps of thread 0, or nullptr:
+  // 0 start, 1 end of the mainloop, 2 after pass A, 3 after pass B, 4 exchange wait done, 5 end of pass C, 6 end of
+  // the CTA.  Slots 1-5 are those of the CTA's last row tile.
+  long long* timing;
 };
 
 template <bool TF32>
@@ -93,9 +104,16 @@ struct FusedCfg {
   static constexpr int MAXG = 6;
   static constexpr int ROW_BYTES = 5 * MAXG * BLOCK_M * 4;          // tcol, coef, max, scale, z[target] per (bin, row)
   static constexpr int PART_BYTES = MAXG * 2 * 256 * 4;             // per-thread running partials
-  static constexpr int MISC_BYTES = 3 * BLOCK_N * 4 /*bias, bin, colsum*/ + 64 /*loss*/ + 256 /*barriers*/;
+  static constexpr int MISC_BYTES = 2 * BLOCK_N * 4 /*bias, bin*/ + 64 /*loss*/ + 256 /*barriers*/;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + ROW_BYTES + PART_BYTES + MISC_BYTES + 1024;
   static_assert(SMEM_BYTES <= 232448, "fused forward exceeds shared memory");
+  // dz of the tile is staged in the (then idle) pipeline stages as 128-byte-wide column boxes of 128 rows, 128B
+  // swizzled, and written by TMA stores
+  static constexpr int BOX_COLS = 128 / ELT;
+  static constexpr int BOX_BYTES = BLOCK_M * 128;
+  static constexpr int BOXES = BLOCK_N / BOX_COLS;
+  static_assert(BOXES * BOX_BYTES <= STAGES * STAGE_BYTES, "the dz tile does not fit the pipeline stages");
+  static constexpr int CHUNKS = BLOCK_N / 8;   // 8-column chunks of the tile: a thread holds 2 columns of each
   static constexpr int SLOT_ELEMS = RANKS * MAXG * BLOCK_M;          // float2 per exchange slot
   static_assert(MAXG < kMaxG, "the last per-CTA partial slot carries the accuracy count");
 };
@@ -121,10 +139,11 @@ __device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* addr)
 
 // WF = true: p.wmask points at fp32 per-(bin, RoI) weights instead of 0/1 bytes (the reweight head variant,
 // gs_bbox_head_with0_reweight.py:57-85)
+// tmap_dz: dz [N, C] in the operand dtype (row stride ldd), boxes of BOX_COLS x 128, 128B swizzle; unused without dz
 template <bool TF32, bool WF = false>
 __global__ void __launch_bounds__(FusedCfg<TF32>::NUM_THREADS, 1)
 bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                      const FusedFwdParams p) {
+                      const __grid_constant__ CUtensorMap tmap_dz, const FusedFwdParams p) {
   using Cfg = FusedCfg<TF32>;
   constexpr int BLOCK_M = Cfg::BLOCK_M, BLOCK_N = Cfg::BLOCK_N, BLOCK_K = Cfg::BLOCK_K, STAGES = Cfg::STAGES;
   constexpr int MAXG = Cfg::MAXG, HALF_N = Cfg::HALF_N, RANKS = Cfg::RANKS;
@@ -141,12 +160,14 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   float* s_part = s_zt + MAXG * BLOCK_M;                                             // [MAXG][2][256]
   float* s_bias = s_part + MAXG * 2 * 256;                                           // [320]
   int* s_colbin = reinterpret_cast<int*>(s_bias + BLOCK_N);                          // [320] bin or -1
-  float* s_colsum = reinterpret_cast<float*>(s_colbin + BLOCK_N);                    // [320]
-  float* s_loss = s_colsum + BLOCK_N;                                                // [16]
+  float* s_loss = reinterpret_cast<float*>(s_colbin + BLOCK_N);                      // [16]
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_loss + 16);
   uint64_t* full_bar = bars;
   uint64_t* empty_bar = bars + STAGES;
   __shared__ int s_gs[kMaxG], s_ge[kMaxG];
+  // per quad lane q: bit J set = chunk J takes the per-element path of the walks (see below)
+  __shared__ unsigned long long s_slow[4];
+  static_assert(Cfg::CHUNKS <= 64, "one bit per chunk");
 
   const int tid = threadIdx.x, wg = tid >> 7;   // warpgroup: rows [64 wg, 64 wg + 64) of the tile
   const int rank = static_cast<int>(blockIdx.x) % RANKS, group = static_cast<int>(blockIdx.x) / RANKS;
@@ -157,13 +178,16 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   unsigned int* xch_counter = p.xch_counter + group * kFusedCounterStride;
 
   if (threadIdx.x == 0) {
+    stamp(p.timing, 0);
     tma_prefetch_desc(&tmap_x);
     tma_prefetch_desc(&tmap_w);
+    if (p.want_dz && p.dz_tma_cols > 0) tma_prefetch_desc(&tmap_dz);
 #pragma unroll
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], Cfg::NUM_THREADS); }
     fence_mbar_init();
   }
   if (threadIdx.x < 16) s_loss[threadIdx.x] = 0.f;
+  if (threadIdx.x < 4) s_slow[threadIdx.x] = 0ull;
   if (threadIdx.x < kMaxG) {
     int gs = 0, ge = 0;
 #pragma unroll
@@ -179,8 +203,17 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     for (int i = 0; i < MAXG; ++i)
       if (i < G && col < p.C && col >= p.gt.start[i] && col < p.gt.start[i] + p.gt.len[i]) b = i;
     s_colbin[c] = b;
-    s_colsum[c] = 0.f;
     s_bias[c] = (p.bias != nullptr && col < p.C) ? __ldg(p.bias + col) : 0.f;
+  }
+  // The walks below go over the thread's two columns 8J + 2q, 8J + 2q + 1 of every 8-column chunk J in column order,
+  // keeping a running bin.  Chunk J is "slow" for quad lane q unless both columns lie in a bin (< C) and in the same
+  // bin as the lane's last column of chunk J - 1 -- then the running bin is already theirs, and the walk needs no
+  // bin lookup there.  Bins are contiguous, so a CTA has at most G + 1 bin changes plus the chunks at or past C.
+  __syncthreads();   // s_colbin; s_slow is zero
+  if (threadIdx.x < 4 * Cfg::CHUNKS) {
+    const int qq = threadIdx.x & 3, J = threadIdx.x >> 2, c = 8 * J + 2 * qq;
+    const int b0 = s_colbin[c], b1 = s_colbin[c + 1], bp = J > 0 ? s_colbin[c - 7] : -1;
+    if (b0 < 0 || b1 != b0 || bp != b0) atomicOr(&s_slow[qq], 1ull << J);
   }
   __syncthreads();
 
@@ -205,6 +238,8 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     tma_load_2d(sb, &tmap_w, &full_bar[stage], k0, n0);
     tma_load_2d(sb + HALF_N * 128, &tmap_w, &full_bar[stage], k0, n0 + HALF_N);
   };
+  // the previous tile's dz left the stages through TMA stores, which must have read them before they are refilled
+  if (tid == 0 && tile_i > 0) tma_store_wait_read<0>();
   for (int kb = 0; kb < STAGES && kb < p.kblocks; ++kb) {
     const int it = it0 + kb;
     // the stage is free once the previous tile's k-block it - STAGES has released it (all threads wait: see below)
@@ -278,6 +313,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     fence_regs(acc1);
     mbar_arrive(&empty_bar[(it0 + p.kblocks - 1) % STAGES]);   // the last k-block's stage, for the next tile
   }
+  if (tid == 0) stamp(p.timing, 1);
   pdl_wait();   // every global write below comes after the predecessor grid
 
   // ---- row information, part 2: w / avg.  Masks and avg come from the preceding sampler kernel (programmatic
@@ -298,17 +334,18 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     info_coef[i] = w * inv_avg;
   }
 
-  // walk the thread's 2 x 160 elements in column order: f(z of row row_l0, z of row row_l0 + 8, local column)
-#define BAGS_WALK(F)                                                                                         \
+  // Walk the thread's 2 x 160 elements in column order, one 8-column chunk at a time:
+  // F(accumulators, j, J, c): rows row_l0 / row_l0 + 8 x local columns c, c + 1 of chunk J are acc[4j], acc[4j + 1] /
+  // acc[4j + 2], acc[4j + 3].  A chunk whose bit in `slow` is clear lies in the running bin (see s_slow): the walk
+  // takes it without a bin lookup; the others go element by element through s_colbin.  (Computing the bin from the
+  // kernel parameters instead costs more registers than the kernel has: ptxas spills.)
+  const unsigned long long slow = s_slow[q];
+#define BAGS_CHUNKS(F)                                                                                       \
   do {                                                                                                       \
-    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) {                                                 \
-      _Pragma("unroll") for (int e = 0; e < 2; ++e) F(acc0[4 * j + e], acc0[4 * j + 2 + e], 8 * j + 2 * q + e); \
-    }                                                                                                        \
-    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) {                                                 \
-      _Pragma("unroll") for (int e = 0; e < 2; ++e)                                                          \
-        F(acc1[4 * j + e], acc1[4 * j + 2 + e], HALF_N + 8 * j + 2 * q + e);                                 \
-    }                                                                                                        \
+    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) F(acc0, j, j, 8 * j + 2 * q);                     \
+    _Pragma("unroll") for (int j = 0; j < HALF_N / 8; ++j) F(acc1, j, HALF_N / 8 + j, HALF_N + 8 * j + 2 * q); \
   } while (0)
+#define BAGS_IS_SLOW(J) (((slow >> (J)) & 1ull) != 0ull)
   // per-thread partials of (bin, row slot) -> s_part; the running pair is flushed where the bin changes
 #define BAGS_PART(g, rr) s_part[((g) * 2 + (rr)) * 256 + tid]
 
@@ -327,7 +364,16 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
       mc[0] = fmaxf(mc[0], z0);
       mc[1] = fmaxf(mc[1], z1);
     };
-    BAGS_WALK(stepA);
+    auto chunkA = [&](float (&a)[80], int j, int J, int c) {
+      if (BAGS_IS_SLOW(J)) {
+        stepA(a[4 * j], a[4 * j + 2], c);
+        stepA(a[4 * j + 1], a[4 * j + 3], c + 1);
+      } else {
+        mc[0] = fmaxf(fmaxf(mc[0], a[4 * j]), a[4 * j + 1]);
+        mc[1] = fmaxf(fmaxf(mc[1], a[4 * j + 2]), a[4 * j + 3]);
+      }
+    };
+    BAGS_CHUNKS(chunkA);
     if (gc >= 0) { BAGS_PART(gc, 0) = mc[0]; BAGS_PART(gc, 1) = mc[1]; }
   }
   for (int g = 0; g < G; ++g) {
@@ -343,18 +389,37 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   for (int i = 0; i < MAXG / 2; ++i)
     if (info_g0 + 2 * i < G) s_coef[(info_g0 + 2 * i) * BLOCK_M + info_row] = info_coef[i];
   __syncthreads();   // s_tcol / s_coef of every row; s_mrow of the quad
+  if (tid == 0) stamp(p.timing, 2);
 
   // ---- pass B: z := e = exp(z - max) in place, per-bin sum of e; z[target] for the loss ----
 #pragma unroll
   for (int g = 0; g < MAXG; ++g) BAGS_PART(g, 0) = BAGS_PART(g, 1) = 0.f;
   {
     int gc = -1;
-    float mb[2] = {0.f, 0.f}, sc[2] = {0.f, 0.f};
+    float mb[2] = {0.f, 0.f}, sc[2] = {0.f, 0.f}, zt[2] = {0.f, 0.f};
     int tc[2] = {-1, -1};
+    // z[target] is picked into a register on the way and stored where the bin ends, by the lane that holds the
+    // target column (the target lies inside its bin)
+    auto flushB = [&]() {
+      if (gc >= 0) {
+        BAGS_PART(gc, 0) = sc[0]; BAGS_PART(gc, 1) = sc[1];
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr)
+          if (tc[rr] >= 0 && tc[rr] < BLOCK_N && ((tc[rr] >> 1) & 3) == q) s_zt[gc * BLOCK_M + row_l0 + 8 * rr] = zt[rr];
+      }
+    };
+    auto expB = [&](float& z0, float& z1, int c) {
+      zt[0] = (c == tc[0]) ? z0 : zt[0];
+      zt[1] = (c == tc[1]) ? z1 : zt[1];
+      z0 = exp2f(fmaf(z0, kLog2e, -mb[0]));
+      z1 = exp2f(fmaf(z1, kLog2e, -mb[1]));
+      sc[0] += z0;
+      sc[1] += z1;
+    };
     auto stepB = [&](float& z0, float& z1, int c) {
       const int b = s_colbin[c];
       if (b != gc) {
-        if (gc >= 0) { BAGS_PART(gc, 0) = sc[0]; BAGS_PART(gc, 1) = sc[1]; }
+        flushB();
         gc = b; sc[0] = sc[1] = 0.f;
         if (b >= 0) {
 #pragma unroll
@@ -364,17 +429,19 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
           }
         }
       }
-      if (b >= 0) {
-        if (c == tc[0]) s_zt[b * BLOCK_M + row_l0] = z0;
-        if (c == tc[1]) s_zt[b * BLOCK_M + row_l0 + 8] = z1;
-        z0 = exp2f(fmaf(z0, kLog2e, -mb[0]));
-        z1 = exp2f(fmaf(z1, kLog2e, -mb[1]));
-        sc[0] += z0;
-        sc[1] += z1;
+      if (b >= 0) expB(z0, z1, c);
+    };
+    auto chunkB = [&](float (&a)[80], int j, int J, int c) {
+      if (BAGS_IS_SLOW(J)) {
+        stepB(a[4 * j], a[4 * j + 2], c);
+        stepB(a[4 * j + 1], a[4 * j + 3], c + 1);
+      } else {
+        expB(a[4 * j], a[4 * j + 2], c);
+        expB(a[4 * j + 1], a[4 * j + 3], c + 1);
       }
     };
-    BAGS_WALK(stepB);
-    if (gc >= 0) { BAGS_PART(gc, 0) = sc[0]; BAGS_PART(gc, 1) = sc[1]; }
+    BAGS_CHUNKS(chunkB);
+    flushB();
   }
 
   // ---- exchange: publish (max, sum) of every (row, bin) to the group's slot of this tile's parity ----
@@ -398,17 +465,30 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   }
 #undef BAGS_PART
   __syncthreads();   // this CTA's partials are stored (and s_zt is complete)
+  unsigned int xch_target = 0;
   if (tid == 0) {
+    stamp(p.timing, 3);
     // Arrival counters are never reset: every tile adds four arrivals, so a tile's four arrivals are the ones that
     // take the counter to the next multiple of 4 -- across tiles, launches and graph replays on one stream.
     __threadfence();
-    const unsigned int target = (atom_add_release_gpu(xch_counter, 1u) & ~3u) + 4u;
+    xch_target = (atom_add_release_gpu(xch_counter, 1u) & ~3u) + 4u;
+  }
+  // The optional buffer clear (a write: only after the wait -- the buffer may still be in use by an earlier kernel) is
+  // issued while the peers' partials are awaited.
+  if (tile_i == 0 && p.clear != nullptr) {
+    const long long stride = static_cast<long long>(gridDim.x) * Cfg::NUM_THREADS;
+    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (long long i = static_cast<long long>(blockIdx.x) * Cfg::NUM_THREADS + tid; i < p.clear_vecs; i += stride)
+      p.clear[i] = zero4;
+  }
+  if (tid == 0) {
     uint32_t spins = 0, ns = 32;
-    while (static_cast<int>(ld_acquire_gpu(xch_counter) - target) < 0) {
+    while (static_cast<int>(ld_acquire_gpu(xch_counter) - xch_target) < 0) {
       if (++spins > BAGS_WAIT_LIMIT) __trap();
       __nanosleep(ns);
       ns = ns < 256 ? 2 * ns : 256;
     }
+    stamp(p.timing, 4);
   }
   __syncthreads();   // all four CTAs' partials are visible (read through L2 below)
   // PDL INVARIANT: every CTA triggers once it runs -- here, after its first exchange -- and a dependent grid is launched
@@ -417,18 +497,27 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   // rather than at the start of the kernel made the 4096-RoI benchmark step about 3 % faster on an H100 80GB HBM3 at
   // 400 W.)  Dependents guard their first dependent access with griddepcontrol.wait.
   if (tile_i == 0) pdl_trigger();
-  if (q == 0) {
+  {
+    // The quad's 2 x G (row, bin) pairs k = 2 g + rr are spread over its four lanes (lane q: k = q, q + 4, q + 8), and
+    // every lane issues all its L2 loads before it uses any.
+    constexpr int PAIRS = 2 * MAXG / 4;
+    float2 v[PAIRS][RANKS];
 #pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      const int row_l = row_l0 + 8 * rr, row = m0 + row_l;
-      for (int g = 0; g < G; ++g) {
-        float2 v[RANKS];
+    for (int i = 0; i < PAIRS; ++i) {
+      const int k = q + 4 * i, g = k >> 1, row_l = row_l0 + 8 * (k & 1);
 #pragma unroll
-        for (int s = 0; s < RANKS; ++s) v[s] = __ldcg(&xch[(s * MAXG + g) * BLOCK_M + row_l]);
-        const float M = fmaxf(fmaxf(v[0].x, v[1].x), fmaxf(v[2].x, v[3].x));
+      for (int s = 0; s < RANKS; ++s)
+        v[i][s] = g < G ? __ldcg(&xch[(s * MAXG + g) * BLOCK_M + row_l]) : make_float2(0.f, 0.f);
+    }
+#pragma unroll
+    for (int i = 0; i < PAIRS; ++i) {
+      const int k = q + 4 * i, g = k >> 1, row_l = row_l0 + 8 * (k & 1), row = m0 + row_l;
+      if (g < G) {
+        const float M = fmaxf(fmaxf(v[i][0].x, v[i][1].x), fmaxf(v[i][2].x, v[i][3].x));
         float S = 0.f;
 #pragma unroll
-        for (int s = 0; s < RANKS; ++s) S += (v[s].x == -INFINITY) ? 0.f : v[s].y * exp2f((v[s].x - M) * kLog2e);
+        for (int s = 0; s < RANKS; ++s)
+          S += (v[i][s].x == -INFINITY) ? 0.f : v[i][s].y * exp2f((v[i][s].x - M) * kLog2e);
         const float lse_v = M + logf(S);
         const float cf = s_coef[g * BLOCK_M + row_l];
         s_scale[g * BLOCK_M + row_l] = exp2f((s_mrow[g * BLOCK_M + row_l] - lse_v) * kLog2e) * cf;
@@ -446,100 +535,108 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     }
   }
   __syncwarp();   // s_scale of the quad
-  // ---- pass C: dz, loss, column sums ----
-  {
-    const bool f32 = TF32;
-    const bool want_cs = p.colsum != nullptr && p.want_dz;
+  // ---- pass C: dz -> the staged tile (operand dtype, the pipeline stages) -> TMA stores; column sums ----
+  // Column c of the tile is column c % BOX_COLS of box c / BOX_COLS; a box row is 128 bytes whose 16-byte pieces are
+  // swizzled with the row (piece ^ row % 8), as TMA SWIZZLE_128B expects.  Both rows of the thread have row % 8 =
+  // lane / 4.  Columns >= C and rows >= N are staged like the others and never stored.
+  if (p.want_dz) {
+    constexpr int ELT = Cfg::ELT, BOX_BYTES = Cfg::BOX_BYTES;
+    const int r8 = lane >> 2;
+    uint8_t* const stg = smem + row_l0 * 128 + (TF32 ? 8 * (q & 1) : 4 * q);
+    // stg: the thread's row and byte within a 16-byte piece; stage_off(J): box and swizzled piece of chunk J
+    const uint32_t swz = TF32 ? static_cast<uint32_t>(((q >> 1) ^ r8) << 4) : static_cast<uint32_t>(r8 << 4);
+    auto stage_off = [&](int J) -> uint32_t {
+      return TF32 ? (J / 4) * BOX_BYTES + ((static_cast<uint32_t>(J % 4) << 5) ^ swz)
+                  : (J / 8) * BOX_BYTES + ((static_cast<uint32_t>(J % 8) << 4) ^ swz);
+    };
     int gc = -1;
     float sc[2] = {0.f, 0.f}, cf[2] = {0.f, 0.f};
     int tc[2] = {-1, -1};
-    uint8_t* dzrow[2];
-    bool row_ok[2];
+    auto dzC = [&](float e, int rr, int c) {
+      float v = e * sc[rr];
+      if (c == tc[rr]) v -= cf[rr];
+      return v;
+    };
+    auto stepC = [&](float e0, float e1, int c, float& d0, float& d1) {   // rows 0/1 x column c
+      const int b = s_colbin[c];
+      if (b != gc) {
+        gc = b;
+        if (b >= 0) {
 #pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      const int row = m0 + row_l0 + 8 * rr;
-      row_ok[rr] = p.want_dz && row < p.N;
-      dzrow[rr] = reinterpret_cast<uint8_t*>(p.dz) + static_cast<long long>(row) * p.ldd * (f32 ? 4 : 2);
-    }
-    auto stepC = [&](float e0a, float e0b, float e1a, float e1b, int c) {   // rows 0/1 x columns c, c + 1
+          for (int rr = 0; rr < 2; ++rr) {
+            sc[rr] = s_scale[b * BLOCK_M + row_l0 + 8 * rr];
+            cf[rr] = s_coef[b * BLOCK_M + row_l0 + 8 * rr];
+            tc[rr] = s_tcol[b * BLOCK_M + row_l0 + 8 * rr] - n0;
+          }
+        }
+      }
+      d0 = b >= 0 ? dzC(e0, 0, c) : 0.f;
+      d1 = b >= 0 ? dzC(e1, 1, c) : 0.f;
+    };
+    auto chunkC = [&](float (&a)[80], int j, int J, int c) {
       float d[2][2];
-      const float ee[2][2] = {{e0a, e0b}, {e1a, e1b}};
-#pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int b = s_colbin[c + e];
-        if (b != gc) {
-          gc = b;
-          if (b >= 0) {
-#pragma unroll
-            for (int rr = 0; rr < 2; ++rr) {
-              sc[rr] = s_scale[b * BLOCK_M + row_l0 + 8 * rr];
-              cf[rr] = s_coef[b * BLOCK_M + row_l0 + 8 * rr];
-              tc[rr] = s_tcol[b * BLOCK_M + row_l0 + 8 * rr] - n0;
-            }
-          }
-        }
-#pragma unroll
-        for (int rr = 0; rr < 2; ++rr) {
-          float v = 0.f;
-          if (b >= 0) {
-            v = ee[rr][e] * sc[rr];
-            if (c + e == tc[rr]) v -= cf[rr];
-          }
-          d[rr][e] = v;
-        }
-      }
-      const int col = n0 + c;
-#pragma unroll
-      for (int rr = 0; rr < 2; ++rr) {
-        if (!f32) {   // the stored (rounded) values feed the column sums
-          d[rr][0] = __bfloat162float(__float2bfloat16_rn(d[rr][0]));
-          d[rr][1] = __bfloat162float(__float2bfloat16_rn(d[rr][1]));
-        }
-        if (row_ok[rr] && col < p.C) {
-          if (col + 1 < p.C) {
-            if (f32) *reinterpret_cast<float2*>(dzrow[rr] + col * 4) = make_float2(d[rr][0], d[rr][1]);
-            else     *reinterpret_cast<uint32_t*>(dzrow[rr] + col * 2) = pack_bf16x2(d[rr][0], d[rr][1]);
-          } else {
-            if (f32) *reinterpret_cast<float*>(dzrow[rr] + col * 4) = d[rr][0];
-            else     *reinterpret_cast<__nv_bfloat16*>(dzrow[rr] + col * 2) = __float2bfloat16_rn(d[rr][0]);
-          }
-        }
-      }
-      if (want_cs) {
+      if (BAGS_IS_SLOW(J)) {
+        stepC(a[4 * j], a[4 * j + 2], c, d[0][0], d[1][0]);
+        stepC(a[4 * j + 1], a[4 * j + 3], c + 1, d[0][1], d[1][1]);
+      } else {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
-          float cs = d[0][e] + d[1][e];
-          cs += __shfl_xor_sync(0xffffffffu, cs, 4);
-          cs += __shfl_xor_sync(0xffffffffu, cs, 8);
-          cs += __shfl_xor_sync(0xffffffffu, cs, 16);
-          if (lane < 4) atomicAdd(&s_colsum[c + e], cs);
+          d[0][e] = dzC(a[4 * j + e], 0, c + e);
+          d[1][e] = dzC(a[4 * j + 2 + e], 1, c + e);
         }
       }
+      const uint32_t off = stage_off(J);
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        if (TF32) *reinterpret_cast<float2*>(stg + off + rr * 1024) = make_float2(d[rr][0], d[rr][1]);
+        else      *reinterpret_cast<uint32_t*>(stg + off + rr * 1024) = pack_bf16x2(d[rr][0], d[rr][1]);
+      }
     };
-#pragma unroll
-    for (int j = 0; j < HALF_N / 8; ++j)
-      stepC(acc0[4 * j], acc0[4 * j + 1], acc0[4 * j + 2], acc0[4 * j + 3], 8 * j + 2 * q);
-#pragma unroll
-    for (int j = 0; j < HALF_N / 8; ++j)
-      stepC(acc1[4 * j], acc1[4 * j + 1], acc1[4 * j + 2], acc1[4 * j + 3], HALF_N + 8 * j + 2 * q);
-  }
-#undef BAGS_WALK
-  __syncthreads();   // s_colsum complete; the tile's shared row information is no longer read
-
-  if (p.colsum != nullptr && p.want_dz) {   // optional per-row-tile bias-gradient partials
-    for (int c = tid; c < BLOCK_N; c += Cfg::NUM_THREADS) {
-      if (n0 + c < p.C) p.colsum[static_cast<long long>(row_tile) * p.C + n0 + c] = s_colsum[c];
-      s_colsum[c] = 0.f;   // (the next tile adds to it only after its own __syncthreads)
+    BAGS_CHUNKS(chunkC);
+    fence_proxy_async_smem();   // the staged tile is read by the TMA (async proxy)
+    __syncthreads();
+    if (tid == 0) {
+#pragma unroll 1
+      for (int bx = 0; bx < Cfg::BOXES; ++bx)
+        if (n0 + bx * Cfg::BOX_COLS < p.dz_tma_cols)
+          tma_store_2d(&tmap_dz, smem + bx * BOX_BYTES, n0 + bx * Cfg::BOX_COLS, m0);
+      tma_store_commit();
+    }
+    // the last few columns [dz_tma_cols, C) (at most 16 bytes of a row, all in one CTA) take plain stores
+    const int tail0 = max(p.dz_tma_cols, n0) - n0, tail = min(p.C, n0 + BLOCK_N) - n0 - tail0;
+    if (tail > 0) {
+      for (int i = tid; i < BLOCK_M * 8; i += Cfg::NUM_THREADS) {
+        const int r = i >> 3, c = tail0 + (i & 7);
+        if ((i & 7) < tail && m0 + r < p.N) {
+          const int byte = (c % Cfg::BOX_COLS) * ELT;
+          const uint8_t* a = smem + (c / Cfg::BOX_COLS) * BOX_BYTES + r * 128 + ((((byte >> 4) ^ r) & 7) << 4) + (byte & 15);
+          uint8_t* dst = static_cast<uint8_t*>(p.dz) + (static_cast<long long>(m0 + r) * p.ldd + n0 + c) * ELT;
+          if (TF32) *reinterpret_cast<float*>(dst) = *reinterpret_cast<const float*>(a);
+          else      *reinterpret_cast<uint16_t*>(dst) = *reinterpret_cast<const uint16_t*>(a);
+        }
+      }
+    }
+    if (p.colsum != nullptr) {   // optional per-row-tile bias-gradient partials: the stored (rounded) values, in row order
+      for (int c = tid; c < BLOCK_N; c += Cfg::NUM_THREADS) {
+        if (n0 + c >= p.C) continue;
+        const int byte = (c % Cfg::BOX_COLS) * ELT;
+        const uint8_t* col = smem + (c / Cfg::BOX_COLS) * BOX_BYTES + (byte & 15);
+        const int piece = byte >> 4;
+        float s = 0.f;
+#pragma unroll 8
+        for (int r = 0; r < BLOCK_M; ++r) {
+          const uint8_t* a = col + r * 128 + ((piece ^ (r & 7)) << 4);
+          s += TF32 ? *reinterpret_cast<const float*>(a) : __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(a));
+        }
+        p.colsum[static_cast<long long>(row_tile) * p.C + n0 + c] = s;
+      }
     }
   }
+#undef BAGS_CHUNKS
+#undef BAGS_IS_SLOW
+  __syncthreads();   // the staged tile and the tile's shared row information are no longer read
+  if (tid == 0) stamp(p.timing, 5);
   }   // row tiles
-
-  if (p.clear != nullptr) {   // (a write: only after the wait -- the buffer may still be in use by an earlier kernel)
-    const long long stride = static_cast<long long>(gridDim.x) * Cfg::NUM_THREADS;
-    const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (long long i = static_cast<long long>(blockIdx.x) * Cfg::NUM_THREADS + tid; i < p.clear_vecs; i += stride)
-      p.clear[i] = zero4;
-  }
   if (tid < 32) {
     // ---- loss bookkeeping: per-CTA partials, the last CTA of the grid sums them in a fixed order ----
     unsigned int last = 0;
@@ -569,6 +666,10 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
       }
       if (lane == 0) *p.counter = 0u;
     }
+  }
+  if (tid == 0) {
+    tma_store_wait_all();   // the dz stores have read the stages and are complete
+    stamp(p.timing, 6);
   }
 }
 

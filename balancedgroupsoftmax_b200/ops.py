@@ -256,7 +256,8 @@ def fused_fwd(x, w, bias, labels, dt: DeviceTables, wmask, avg, logits: Optional
     ws = _workspace(dev)
     wmask, wcode = _weights_arg(wmask)
     if clear is not None:
-        # ``clear``: a contiguous buffer (the caller's dW) that the forward zeroes, on the fused route while its MMAs run
+        # ``clear``: a contiguous buffer (the caller's dW) that the forward zeroes, on the fused route while its CTAs
+        # exchange their softmax partials
         assert clear.is_contiguous() and (clear.numel() * clear.element_size()) % 16 == 0
     nat.check(nat.lib().bags_fwd(
         x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(),

@@ -113,7 +113,7 @@ int bags_fused_eligible(const int32_t* slices_host, int G, int C);
  * colsum (optional) is [colsum_tiles, C] with colsum_tiles = ceil(N/128): per-128-row-tile partial column sums
  * of dz (written with plain stores, no pre-zeroing needed); their sum over tiles is sum_n dz[n, :].
  * clear (optional, NULL / 0 = none): `clear_bytes` bytes at `clear` (16-byte aligned, a multiple of 16; typically the
- * caller's dW) are set to zero -- by the fused kernel after its epilogue, or by a memset on the
+ * caller's dW) are set to zero -- by the fused kernel while its CTAs wait for each other's softmax partials, or by a memset on the
  * materialised route.  Together with `colsum` this lets bags_bwd run without any preparation work (flag
  * BAGS_BWD_DW_PREZEROED, no column-sum job).
  * The fused kernel is launched with programmatic dependent launch: when the preceding kernel in the stream is
@@ -246,9 +246,11 @@ int bags_gemm_probe(const void* a, long long lda, int a_mn, const void* b, long 
                     void* out, long long ldo, int M, int N, int K, int dtype, int block_n,
                     int splits, int epi, void* stream);
 
-/* Test hook: point the gradient-exchange kernel (bags_grad_allreduce) at a device buffer of int64 %globaltimer
- * stamps; it writes [blocks][8] slots starting at row 4096 of the buffer.  The GEMM and fused-forward kernels do
- * not stamp it.  NULL (the default) disables it.  Not thread-safe; for profiling only. */
+/* Test hook: point the fused forward (bags_fwd / bags_ce_fwd without logits) and the gradient-exchange kernel
+ * (bags_grad_allreduce) at a device buffer of int64 %globaltimer stamps, [blocks][8] slots per kernel.  The fused
+ * forward writes rows [0, blocks) (at most 256 CTAs; tools/fused_fwd_phases.py reads its phases), the gradient
+ * exchange rows from 4096 on.  The GEMM and backward kernels do not stamp it.  NULL (the default) disables it.
+ * Not thread-safe; for profiling only. */
 int bags_debug_set_timing(void* dev_ptr);
 
 /* The library reads its tuning / experiment switches (BAGS_* environment variables) once per name and caches them;

@@ -467,15 +467,20 @@ extern "C" int bags_group_ce(const float* logits, long long ldz, const int64_t* 
 // ----------------------------------------------------------------------------
 // fused forward (GEMM + grouped softmax-CE in one kernel)
 // ----------------------------------------------------------------------------
-static bool fused_eligible(const int32_t* slices_host, int G, int C) {
-  if (slices_host == nullptr || G < 1 || G > FusedCfg<false>::MAXG || C > 4 * FusedCfg<false>::BLOCK_N || (C % 4) != 0)
-    return false;
+// the bins tile [0, C) contiguously: every logit column lies in a bin
+static bool bins_tile(const int32_t* slices_host, int G, int C) {
   int end = 0;
-  for (int g = 0; g < G; ++g) {   // bins must tile [0, C) contiguously
+  for (int g = 0; g < G; ++g) {
     if (slices_host[2 * g] != end || slices_host[2 * g + 1] < 1) return false;
     end += slices_host[2 * g + 1];
   }
   return end == C;
+}
+
+static bool fused_eligible(const int32_t* slices_host, int G, int C) {
+  if (slices_host == nullptr || G < 1 || G > FusedCfg<false>::MAXG || C > 4 * FusedCfg<false>::BLOCK_N || (C % 4) != 0)
+    return false;
+  return bins_tile(slices_host, G, C);
 }
 
 extern "C" int bags_fused_eligible(const int32_t* slices_host, int G, int C) {
@@ -768,6 +773,9 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
   // contractions in one merged launch, or the one requested as a plain split-K dW (red.add) / dX GEMM ----
   // both contractions requested: one merged persistent launch after the preparation kernel (see bags_bwd_merged_kernel)
   const bool merged = dW != nullptr && dX != nullptr && N > 0 && env_int("BAGS_BWD_MERGED", 1);
+  // a dz column outside every bin is scaled by 0 when gout is given: the merged kernel's uniform-gout shortcut (dz W,
+  // output scaled by gout[0]) would scale it by gout[0], so it is taken only when the bins tile [0, C)
+  const bool no_gaps = bins_tile(slices_host, G, C);
   BwdPrepParams pp{};
   bool prep_launched = false;
   if (dW != nullptr || want_scale || want_colpart) {
@@ -777,7 +785,7 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
     pp.z_ctas = (dW != nullptr && !prezeroed) ? di.num_sms : 0;
     pp.s_ctas = want_scale ? di.num_sms : 0;
     pp.c_ctas = want_colpart ? ((C + 63) / 64) * kColsumTiles : 0;
-    pp.skip_scale_if_uniform = merged ? 1 : 0;   // the merged kernel reads W itself when all gout[g] are equal
+    pp.skip_scale_if_uniform = (merged && no_gaps) ? 1 : 0;   // the merged kernel reads W itself (see bp.uniform_ok)
     const int grid = pp.z_ctas + pp.s_ctas + pp.c_ctas;
     if (grid > 0) {
       BAGS_CUDA(launch(bf ? bwd_prep_kernel<false> : bwd_prep_kernel<true>, dim3(grid), dim3(256), 0, stream, true, false, pp));
@@ -830,6 +838,7 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
     bp.w = static_cast<const float*>(w);
     bp.gout = gout;
     bp.G = gt.G;
+    bp.uniform_ok = no_gaps ? 1 : 0;
     return bf ? launch_bwd_merged<false>(dz, ldd, x, ldx, w, wb, ldw, bp, di, stream)
               : launch_bwd_merged<true>(dz, ldd, x, ldx, w, wb, ldw, bp, di, stream);
   }
@@ -1015,6 +1024,8 @@ extern "C" int bags_cast_bf16(const float* src, long long lds, void* dst, long l
   BAGS_REQUIRE(src && dst, "bags_cast_bf16: NULL argument");
   BAGS_REQUIRE(rows >= 0 && cols >= 0 && (cols % 4) == 0 && (lds % 4) == 0 && (ldd % 4) == 0,
                "bags_cast_bf16: cols and leading dims must be multiples of 4");
+  BAGS_REQUIRE((reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 7) == 0,
+               "bags_cast_bf16: src must be 16-byte and dst 8-byte aligned");
   if (rows == 0 || cols == 0) return BAGS_OK;
   const long long total = (long long)rows * (cols / 4);
   long long grid = (total + 255) / 256;

@@ -348,9 +348,10 @@ bags_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 //   dX units : dX[N,K]   = dz W'                       (A = dz K-major,  B = W' MN-major, plain stores)
 //
 // The units form one work list (dW first: their split-K partials are the longer tail), dealt round-robin to the
-// CTAs, so the SMs that finish their dW share early take dX tiles instead of idling at a kernel boundary.  When all
-// gout[g] are equal (the reference's setting) the dX units read W itself and scale their output by gout[0]: the
-// preparation kernel then skips the scaled copy W' (it makes the same device-side decision).
+// CTAs, so the SMs that finish their dW share early take dX tiles instead of idling at a kernel boundary.  When the
+// bins tile [0, C) and all gout[g] are equal (the reference's setting) the dX units read W itself and scale their
+// output by gout[0]: the preparation kernel then skips the scaled copy W' (it makes the same device-side decision).
+// With gaps between the bins W' is always built, since its gap rows are 0 while W's are not.
 // ---------------------------------------------------------------------------------------------------------------------
 struct BwdMergedParams {
   GemmParams dw;     // tile counts, splits and epilogue fields of the dW problem
@@ -359,6 +360,7 @@ struct BwdMergedParams {
   const float* w;    // W (B of the dX units when gout is uniform)
   const float* gout; // [G] per-bin upstream gradients, or nullptr (dX reads b_ptr unscaled)
   int G;
+  int uniform_ok;    // the bins tile [0, C): a uniform gout may take the W shortcut
 };
 
 template <bool TF32>
@@ -383,7 +385,7 @@ bags_bwd_merged_kernel(const __grid_constant__ CUtensorMap t_dzT, const __grid_c
   // dz, the zeroed dW, W' and the bias-gradient partials all come from the preceding kernels
   pdl_wait();
   float g0 = 1.0f;
-  const bool uniform = p.gout != nullptr && gout_uniform(p.gout, p.G, g0);
+  const bool uniform = p.uniform_ok && p.gout != nullptr && gout_uniform(p.gout, p.G, g0);
   const float* xb = uniform ? p.w : p.dx.b_ptr;
   const CUtensorMap* txb = uniform ? &t_w : &t_wp;
   const float xscale = uniform ? g0 : 1.0f;

@@ -644,7 +644,8 @@ __device__ __forceinline__ void bwd_prep_job(const BwdPrepParams& p, int b, int 
   } else if (b < p.z_ctas + p.s_ctas + p.c_ctas) {
     // ---- (3) column sums of dz over one row group, one 64-column strip per job.  Thread t owns 8 columns
     // (t % 8) of rows (t / 8) + 32 i: 16-byte loads, 8 of them in flight per thread; padded columns of dz exist
-    // up to ldd (a multiple of 8), columns beyond that read as zero ----
+    // up to ldd, columns beyond that read as zero.  bf16 rows have ldd % 8 == 0; fp32 rows only ldd % 4 == 0, so
+    // an fp32 thread whose 8 columns straddle ldd reads the leading group of 4 alone ----
     const int ci = b - p.z_ctas - p.s_ctas;
     const int nstrips = (p.C + 63) / 64;
     const int strip = ci % nstrips, rg = ci / nstrips;
@@ -656,7 +657,8 @@ __device__ __forceinline__ void bwd_prep_job(const BwdPrepParams& p, int b, int 
     float acc[8];
 #pragma unroll
     for (int q = 0; q < 8; ++q) acc[q] = 0.f;
-    if (col + 8 <= p.ldd) {
+    const bool second4 = col + 8 <= p.ldd;   // (F32: the upper 16 bytes of the thread's 8 columns)
+    if (second4 || (F32 && col + 4 <= p.ldd)) {
       for (int rb = r0 + rl; rb < r1; rb += 32 * 8) {
         uint4 v[8], v2[8];
 #pragma unroll
@@ -668,7 +670,7 @@ __device__ __forceinline__ void bwd_prep_job(const BwdPrepParams& p, int b, int 
             if (F32) {
               const uint4* src = reinterpret_cast<const uint4*>(reinterpret_cast<const float*>(p.dz) + static_cast<long long>(r) * p.ldd + col);
               v[u] = __ldcg(src);
-              v2[u] = __ldcg(src + 1);
+              if (second4) v2[u] = __ldcg(src + 1);
             } else {
               v[u] = __ldcg(reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(p.dz) + static_cast<long long>(r) * p.ldd + col));
             }

@@ -156,6 +156,8 @@ size_t bags_bwd_scratch_bytes(int C, long long ldw, int dtype);
  *   dW[C,K]  = (gout ⊙ dz)^T x      fp32, overwritten         (NULL to skip)
  *   db[C]    = gout ⊙ sum_n dz[n,:]  fp32                      (NULL to skip)
  *   dX[N,K]  = (gout ⊙ dz) w         dtype elements            (NULL to skip)
+ * Bins need not tile [0, C): with gout given, a dz column outside every bin is scaled by 0 (it contributes to none of
+ * dW, db, dX); with gout NULL every column is scaled by 1.
  * colsum: optional [colsum_tiles, C] partial column sums of dz from the forward; NULL => recomputed from dz.
  * wscratch: 256-byte aligned, bags_bwd_scratch_bytes() bytes; required when (dX and gout) or (db without colsum).
  * flags: BAGS_BWD_DW_PREZEROED = dW is already zero on entry (stream-ordered), e.g. by bags_fwd's clear hook.
@@ -236,7 +238,8 @@ int bags_linear_act_fwd_splitk(const void* x, long long ldx, const void* w, long
 int bags_act_bwd(const void* dy, long long lddy, int dy_dtype, const void* y, long long ldy, int y_dtype,
                  void* g, long long ldg, int g_dtype, int rows, int cols, void* stream);
 
-/* dst[rows, cols] (bf16, leading dim ldd) = bf16(src[rows, cols] fp32, leading dim lds); cols % 4 == 0 */
+/* dst[rows, cols] (bf16, leading dim ldd) = bf16(src[rows, cols] fp32, leading dim lds), rounded to nearest even;
+ * cols, lds and ldd % 4 == 0, src 16-byte and dst 8-byte aligned */
 int bags_cast_bf16(const float* src, long long lds, void* dst, long long ldd, int rows, int cols,
                    void* stream);
 

@@ -32,41 +32,6 @@ def rel(a, b):
     return ((a - b).norm() / b.norm().clamp_min(1e-30)).item()
 
 
-def case_gemm(name):
-    np, torch, ops, _, _ = _setup()
-    dev = 'cuda'
-    _, kind, dt = name.split('.')
-    dtype = torch.bfloat16 if dt == 'bf16' else torch.float32
-    tol = 2e-5 if dt == 'bf16' else 2e-3
-    out = {}
-    shapes = [(300, 1236, 1024), (128, 256, 64), (4096, 1236, 1024), (77, 100, 40)]
-    for (M, N, K) in shapes:
-        Kp = (K + 7) // 8 * 8
-        Mp = (M + 7) // 8 * 8
-        Np = (N + 7) // 8 * 8
-        if kind in ('kk256', 'kk320'):
-            a = torch.randn(M, Kp, device=dev).to(dtype)[:, :K]
-            b = torch.randn(N, Kp, device=dev).to(dtype)[:, :K]
-            ref = a.double() @ b.double().t()
-            got = ops.gemm_probe(a, False, b, False, M, N, K, block_n=int(kind[2:]), epi=0)
-        elif kind == 'kmn':   # dX-like: A [M,K] K-major, B stored [K,N]
-            a = torch.randn(M, Kp, device=dev).to(dtype)[:, :K]
-            b = torch.randn(K, Np, device=dev).to(dtype)[:, :N]
-            ref = a.double() @ b.double()
-            got = ops.gemm_probe(a, False, b, True, M, N, K, block_n=256, epi=1 if dt == 'bf16' else 0)
-        elif kind == 'mnmn':  # dW-like: A stored [K,M], B stored [K,N], split-K reduce
-            a = torch.randn(K, Mp, device=dev).to(dtype)[:, :M]
-            b = torch.randn(K, Np, device=dev).to(dtype)[:, :N]
-            ref = a.double().t() @ b.double()
-            got = ops.gemm_probe(a, True, b, True, M, N, K, block_n=256, splits=3, epi=2)
-        torch.cuda.synchronize()
-        r = rel(got, ref)
-        t = tol if got.dtype == torch.float32 else 5e-3
-        out['%dx%dx%d' % (M, N, K)] = r
-        assert r < t, 'rel err %g >= %g for %s %s' % (r, t, name, (M, N, K))
-    return out
-
-
 def _problem(N, K=1024, seed=0, wstd=0.05):
     np, torch, ops, synthetic_tables, O = _setup()
     t = synthetic_tables()
@@ -307,9 +272,6 @@ def case_timing(name):
 
 CASES = {
     'group_ce': case_group_ce, 'sampler': case_sampler, 'merge': case_merge,
-    'gemm.kk256.bf16': case_gemm, 'gemm.kmn.bf16': case_gemm,
-    'gemm.mnmn.bf16': case_gemm,
-    'gemm.kk256.f32': case_gemm, 'gemm.kmn.f32': case_gemm, 'gemm.mnmn.f32': case_gemm,
     'fused.bf16': case_fused, 'fused.f32': case_fused, 'fusedk.bf16': case_fusedk, 'fusedk.f32': case_fusedk,
     'timing': case_timing,
 }

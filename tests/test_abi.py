@@ -72,6 +72,18 @@ def test_unknown_weights_dtype_is_rejected():
     rc = lib.bags_group_ce(p, 8, p, p, sl, p, 2, None, 1, 8, 2, 4, p, None, None, 0, 0, None, p, ws, None)
     assert rc == -1 and b'weights dtype 2' in lib.bags_last_error()
 
+def test_cast_bf16_rejects_misaligned_pointers():
+    """bags_cast_bf16 reads float4 from src and writes 8-byte groups to dst: a misaligned pointer is a bad argument,
+    reported before any launch."""
+    lib = nat.lib()
+    buf = (C.c_char * 256)()
+    base = (C.addressof(buf) + 15) // 16 * 16
+    rc = lib.bags_cast_bf16(base + 4, 4, base + 128, 4, 1, 4, None)   # src 4 bytes past a 16-byte boundary
+    assert rc == -1 and b'aligned' in lib.bags_last_error()
+    rc = lib.bags_cast_bf16(base, 4, base + 130, 4, 1, 4, None)       # dst 2 bytes past an 8-byte boundary
+    assert rc == -1 and b'aligned' in lib.bags_last_error()
+
+
 def test_ops_refuse_cpu_tensors():
     """No CPU fallback: handing the product a CPU tensor is an error, not a slow path."""
     import torch

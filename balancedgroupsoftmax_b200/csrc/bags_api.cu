@@ -10,6 +10,7 @@
 #include <mutex>
 #include <string>
 #include <utility>
+#include <vector>
 
 #include "../../include/bags_b200.h"
 #include "bags_gemm.cuh"
@@ -62,7 +63,8 @@ static std::mutex g_mutex;
 static DeviceInfo g_dev[64];
 static bool g_dev_ok[64] = {false};
 
-// test hook: device buffer [ctas][8] int64 that the next launches stamp with %globaltimer values
+// test hook: device buffer [rows][8] int64 that the next launches stamp with %globaltimer values (row ranges: see
+// bags_debug_set_timing in bags_b200.h)
 static long long* g_timing = nullptr;
 extern "C" int bags_debug_set_timing(void* dev_ptr) {
   g_timing = reinterpret_cast<long long*>(dev_ptr);
@@ -707,12 +709,48 @@ static int launch_bwd_merged(const void* dz, long long ldd, const void* x, long 
   if ((rc = make_tmap(&t_dz, dz, dtype, C, N, ldd, CX::BLOCK_K, CX::BLOCK_M))) return rc;  // dX: A = dz
   if ((rc = make_tmap(&t_w, w, dtype, K, C, ldw, CX::SLAB, CX::BLOCK_K))) return rc;      // dX: B = W^T
   if ((rc = make_tmap(&t_wp, wb, dtype, K, C, ldw, CX::SLAB, CX::BLOCK_K))) return rc;    // dX: B = W'^T
+  CUtensorMap t_dx = t_dz;   // (unused unless bp.dx_tma)
+  if (bp.dx_tma && (rc = make_tmap(&t_dx, bp.dx.out, dtype, K, N, bp.dx.ldo, 64, 64))) return rc;   // dX store boxes
   auto kernel = bags_bwd_merged_kernel<TF32>;
-  BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, CW::SMEM_BYTES));
+  constexpr int smem = bwd_merged_smem_bytes<TF32>();
+  BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const int units = bp.dw_units + bp.dx_units;
   const int grid = units < di.num_sms ? units : di.num_sms;
-  BAGS_CUDA(launch(kernel, dim3(grid), dim3(CW::NUM_THREADS), CW::SMEM_BYTES, stream, true, false, t_dzT, t_xT, t_dz, t_w, t_wp, bp));
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(CW::NUM_THREADS), smem, stream, true, false, t_dzT, t_xT, t_dz, t_w, t_wp,
+                   t_dx, bp));
   return BAGS_OK;
+}
+
+// Split-K factor of the merged backward's dW units.  The kernel deals its work list (dW units split-major, then the
+// dX units) round-robin to min(units, SMs) CTAs, and a CTA runs its units back to back, so the backward ends with the
+// CTA that holds the most work.  The cost of a split factor is exactly that: the largest sum over one CTA's units of
+// (k-blocks + kUnitOverheadKb), where the overhead stands for a unit's epilogue and pipeline fill.  Ties go to fewer
+// splits (less split-K red.add traffic).  A pure function of the shape and the SM count.
+static constexpr int kUnitOverheadKb = 2;
+static int merged_dw_splits(int dw_tiles, int dw_kblocks, int dx_units, int dx_kblocks, int num_sms) {
+  // the walk over the work list is O(16 units); a training loop asks for the same shape every step
+  thread_local int memo_key[5] = {-1, -1, -1, -1, -1}, memo_splits = 1;
+  const int key[5] = {dw_tiles, dw_kblocks, dx_units, dx_kblocks, num_sms};
+  if (std::memcmp(key, memo_key, sizeof(key)) == 0) return memo_splits;
+  int splits = 1;
+  long long best = -1;
+  std::vector<long long> load;
+  for (int sp = 1; sp <= 16 && sp <= dw_kblocks; ++sp) {
+    const int units = dw_tiles * sp + dx_units;
+    const int ctas = units < num_sms ? units : num_sms;
+    load.assign(ctas, 0);
+    const int base = dw_kblocks / sp, rem = dw_kblocks % sp;
+    for (int u = 0; u < units; ++u) {
+      const int kb = u < dw_tiles * sp ? base + (u / dw_tiles < rem ? 1 : 0) : dx_kblocks;
+      load[u % ctas] += kb + kUnitOverheadKb;
+    }
+    long long cost = 0;
+    for (long long l : load) cost = l > cost ? l : cost;
+    if (best < 0 || cost < best) { best = cost; splits = sp; }
+  }
+  std::memcpy(memo_key, key, sizeof(key));
+  memo_splits = splits;
+  return splits;
 }
 
 static constexpr int kColsumTiles = 8;   // row groups of the bias-gradient partial sums made by bwd_prep
@@ -786,6 +824,7 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
     pp.s_ctas = want_scale ? di.num_sms : 0;
     pp.c_ctas = want_colpart ? ((C + 63) / 64) * kColsumTiles : 0;
     pp.skip_scale_if_uniform = (merged && no_gaps) ? 1 : 0;   // the merged kernel reads W itself (see bp.uniform_ok)
+    pp.timing = g_timing ? g_timing + 2048 * 8 : nullptr;       // rows [2048, 4096)
     const int grid = pp.z_ctas + pp.s_ctas + pp.c_ctas;
     if (grid > 0) {
       BAGS_CUDA(launch(bf ? bwd_prep_kernel<false> : bwd_prep_kernel<true>, dim3(grid), dim3(256), 0, stream, true, false, pp));
@@ -808,16 +847,8 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
     px.M = N; px.N = K; px.K = C;
     px.num_m_tiles = (N + 127) / 128; px.num_n_tiles = (K + 255) / 256; px.kblocks_total = (C + bk - 1) / bk;
     px.num_splits = 1;
-    // split-K factor of the dW units: fewest (rounds of the work list over the SMs x longest unit), in k-blocks
     const int dw_tiles = pw.num_m_tiles * pw.num_n_tiles, dx_units = px.num_m_tiles * px.num_n_tiles;
-    int splits = 1;
-    long best = -1;
-    for (int sp = 1; sp <= 16 && sp <= pw.kblocks_total; ++sp) {
-      const long rounds = (dw_tiles * sp + dx_units + di.num_sms - 1) / di.num_sms;
-      const int dwk = (pw.kblocks_total + sp - 1) / sp;
-      const long cost = rounds * (dwk > px.kblocks_total ? dwk : px.kblocks_total);
-      if (best < 0 || cost < best) { best = cost; splits = sp; }
-    }
+    int splits = merged_dw_splits(dw_tiles, pw.kblocks_total, dx_units, px.kblocks_total, di.num_sms);
     splits = env_int("BAGS_DW_SPLITS", splits);
     if (splits < 1) splits = 1;
     if (splits > pw.kblocks_total) splits = pw.kblocks_total;
@@ -839,6 +870,11 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
     bp.gout = gout;
     bp.G = gt.G;
     bp.uniform_ok = no_gaps ? 1 : 0;
+    bp.inputs_ready = prep_launched ? 1 : 0;
+    bp.wprime_prepared = want_scale ? 1 : 0;
+    // TMA-stored bf16 dX: a store box writes whole 16-byte pieces at the right edge, so K must end on one
+    bp.dx_tma = (bf && (K % 8) == 0 && (lddx % 8) == 0) ? 1 : 0;
+    bp.timing = g_timing ? g_timing + 1024 * 8 : nullptr;   // rows [1024, 1024 + 2 grid)
     return bf ? launch_bwd_merged<false>(dz, ldd, x, ldx, w, wb, ldw, bp, di, stream)
               : launch_bwd_merged<true>(dz, ldd, x, ldx, w, wb, ldw, bp, di, stream);
   }

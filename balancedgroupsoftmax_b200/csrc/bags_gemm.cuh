@@ -188,7 +188,10 @@ __device__ __forceinline__ void produce_unit(const CUtensorMap* tmap_a, const CU
   }
 }
 
-// Consumer side of one unit: the mainloop of warpgroup `cw` (rows 64 cw .. 64 cw + 63 of the tile).
+// Consumer side of one unit: the mainloop of warpgroup `cw` (rows 64 cw .. 64 cw + 63 of the tile).  One k-block of
+// wgmma stays in flight: after committing k-block kb the warpgroup waits for kb - 1 only and releases that stage, so
+// the tensor pipe does not drain between k-blocks.  The unit ends with everything complete and every stage it used
+// released; pp.stage / pp.phase then name the next unit's first stage, as on the producer's side.
 template <class Cfg, bool A_MN, bool B_MN, bool TF32>
 __device__ __forceinline__ void consume_unit(float (&acc)[128], int cw, int kb0, int kb1, Pipe& pp, int lane) {
   constexpr int STAGES = Cfg::STAGES_;
@@ -198,6 +201,7 @@ __device__ __forceinline__ void consume_unit(float (&acc)[128], int cw, int kb0,
   constexpr uint32_t A_KSTEP = A_T ? 2048 : 32, B_KSTEP = B_T ? 2048 : 32;
   // this warpgroup's 64 A rows: the second MN slab (MN-major) / rows 64..127 (K-major) -- 8 KB either way
   const uint32_t a_off = cw * 8192;
+  int prev = 0;   // stage of k-block kb - 1
   for (int kb = kb0; kb < kb1; ++kb) {
     mbar_wait(&pp.full_bar[pp.stage], pp.phase);
     const uint32_t sa = smem_u32(pp.smem_a + pp.stage * Cfg::A_BYTES) + a_off;
@@ -213,11 +217,21 @@ __device__ __forceinline__ void consume_unit(float (&acc)[128], int cw, int kb0,
       else      wgmma_bf16_n256<A_T ? 1 : 0, B_T ? 1 : 0>(acc, adesc, bdesc, accum);
     }
     wgmma_commit();
-    wgmma_wait<0>();
+    // keep this k-block's MMAs in flight; the previous k-block's are complete, so its stage can be refilled
+    wgmma_wait<1>();
     fence_regs(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&pp.empty_bar[pp.stage]);   // frees the smem slot
+    if (kb > kb0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&pp.empty_bar[prev]);
+    }
+    prev = pp.stage;
     if (++pp.stage == STAGES) { pp.stage = 0; pp.phase ^= 1u; }
+  }
+  wgmma_wait<0>();
+  fence_regs(acc);
+  if (kb1 > kb0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&pp.empty_bar[prev]);   // the last k-block's stage
   }
 }
 
@@ -352,6 +366,17 @@ bags_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 // bins tile [0, C) and all gout[g] are equal (the reference's setting) the dX units read W itself and scale their
 // output by gout[0]: the preparation kernel then skips the scaled copy W' (it makes the same device-side decision).
 // With gaps between the bins W' is always built, since its gap rows are 0 while W's are not.
+//
+// Programmatic dependent launch: the preparation kernel (when it runs) triggers only after its own griddepcontrol.wait,
+// so at this kernel's start dz (the forward's output) and x are complete, and W was never written on the device side.
+// Each access waits only for what it reads:
+//   - the producer's dW units (dz^T, x): no wait, unless no preparation kernel ran (inputs_ready = 0);
+//   - the producer's dX units (dz, W or W'): a wait before the first load of W' (wprime_prepared and gout not
+//     uniform); none when they read W itself;
+//   - the consumers: a wait before their first epilogue, since dW may still be being zeroed and db's column-sum
+//     partials are the preparation kernel's;
+//   - gout is read before any wait: the preparation kernel does not write it, and it is nullptr when none ran.
+// So the mainloop of the first units runs under the preparation kernel's tail.
 // ---------------------------------------------------------------------------------------------------------------------
 struct BwdMergedParams {
   GemmParams dw;     // tile counts, splits and epilogue fields of the dW problem
@@ -361,6 +386,14 @@ struct BwdMergedParams {
   const float* gout; // [G] per-bin upstream gradients, or nullptr (dX reads b_ptr unscaled)
   int G;
   int uniform_ok;    // the bins tile [0, C): a uniform gout may take the W shortcut
+  int inputs_ready;     // a preparation kernel ran between the forward and this launch: dz and x are complete at launch
+  int wprime_prepared;  // dx.b_ptr is W', written by that preparation kernel (else it is W)
+  int dx_tma;           // bf16 dX with K and its row stride multiples of 8: stored through t_dx (dx_epilogue_tma)
+  // optional debug timeline (bags_debug_set_timing), two rows of 8 int64 per CTA, or nullptr.  Row 0, %globaltimer
+  // of the first consumer thread: CTA start, griddepcontrol.wait returned, then for each of the first three units
+  // the end of its mainloop and the end of its epilogue.  Row 1: slots 0-2 the k-blocks of those units (negative
+  // for a dX unit), slot 7 the producer's first load.
+  long long* timing;
 };
 
 template <bool TF32>
@@ -368,11 +401,54 @@ using BwdDwCfg = GemmCfg<256, true, true, EPI_RED_F32, TF32, 4>;
 template <bool TF32>
 using BwdDxCfg = GemmCfg<256, false, true, TF32 ? EPI_STORE_F32 : EPI_STORE_BF16, TF32, 4>;
 
+// The bf16 dX tile leaves through shared memory and TMA stores: each consumer warpgroup stages its 64 x 256 rows in
+// two halves of 64 x 128 (two 128B-swizzled boxes of 64 columns, 16 KB), after the ring and its barriers.
+constexpr int kDxStageBytes = 2 * 16384;
+template <bool TF32>
+constexpr int bwd_merged_smem_bytes() {
+  return 4 * BwdDwCfg<TF32>::STAGE_BYTES + 1024 /*align slack*/ + 1024 /*barriers*/ + kDxStageBytes;
+}
+static_assert(bwd_merged_smem_bytes<false>() <= 232448, "exceeds 227 KB of shared memory");
+
+// bf16 dX epilogue of warpgroup `cw` through its 16 KB staging buffer `stg`: the same values as epilogue_unit's
+// (bf16 of scale * acc), written with one TMA store per 64 x 64 box instead of 8-row scattered 4-byte stores.
+// The tensor map spans [N, K] with K % 8 == 0, so the clipped boxes at the edges never write past column K.
+// Thread 0 of the warpgroup issues the stores and, before the buffer is refilled, waits until they have read it.
+__device__ __forceinline__ void dx_epilogue_tma(const float (&acc)[128], const CUtensorMap* tmap, uint8_t* stg,
+                                                int M, int N, int m0, int n0, int cw, int warp, int lane, int tid,
+                                                float scale) {
+  const int rw = m0 + 64 * cw;   // first row of this warpgroup
+#pragma unroll
+  for (int hc = 0; hc < 2; ++hc) {
+    if (tid == 0) tma_store_wait_read<0>();   // the previous half's (or unit's) stores have read the buffer
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const int j = 16 * hc + jj;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = warp * 16 + (lane >> 2) + 8 * h;
+        *reinterpret_cast<uint32_t*>(stg + (jj >> 3) * 8192 + r * 128 + (((jj & 7) ^ (r & 7)) << 4) + 4 * (lane & 3)) =
+            pack_bf16x2(acc[4 * j + 2 * h] * scale, acc[4 * j + 2 * h + 1] * scale);
+      }
+    }
+    fence_proxy_async_smem();   // the staged half is read by the TMA (async proxy)
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+    if (tid == 0 && rw < M) {
+#pragma unroll
+      for (int b = 0; b < 2; ++b)
+        if (n0 + 128 * hc + 64 * b < N) tma_store_2d(tmap, stg + b * 8192, n0 + 128 * hc + 64 * b, rw);
+      tma_store_commit();
+    }
+  }
+}
+
 template <bool TF32>
 __global__ void __launch_bounds__(384, 1)
 bags_bwd_merged_kernel(const __grid_constant__ CUtensorMap t_dzT, const __grid_constant__ CUtensorMap t_xT,
                        const __grid_constant__ CUtensorMap t_dz, const __grid_constant__ CUtensorMap t_w,
-                       const __grid_constant__ CUtensorMap t_wp, const BwdMergedParams p) {
+                       const __grid_constant__ CUtensorMap t_wp, const __grid_constant__ CUtensorMap t_dx,
+                       const BwdMergedParams p) {
   using CW = BwdDwCfg<TF32>;
   using CX = BwdDxCfg<TF32>;
   static_assert(CW::STAGE_BYTES == CX::STAGE_BYTES && CW::A_BYTES == CX::A_BYTES, "one ring serves both problems");
@@ -380,10 +456,14 @@ bags_bwd_merged_kernel(const __grid_constant__ CUtensorMap t_dzT, const __grid_c
   extern __shared__ uint8_t smem_raw[];
   const int wg = threadIdx.x >> 7;
   const int tid = threadIdx.x & 127;
+  // debug timeline: row 0 belongs to the first consumer thread, row 1 slot 7 to the producer thread
+  long long* const tl = (p.timing != nullptr && (threadIdx.x == 128 || threadIdx.x == 0))
+                            ? p.timing + blockIdx.x * 16ll + (threadIdx.x == 0 ? 8 : 0) : nullptr;
+  if (tl != nullptr && threadIdx.x == 128) tl[0] = global_timer_ns();
   pdl_trigger();
   Pipe pp = setup_pipe(smem_raw, 4, CW::A_BYTES, CW::STAGE_BYTES, CW::ANY_MANUAL);
-  // dz, the zeroed dW, W' and the bias-gradient partials all come from the preceding kernels
-  pdl_wait();
+  uint8_t* const stg = reinterpret_cast<uint8_t*>(pp.full_bar) + 1024;   // dX staging (1024-byte aligned)
+  // gout is never written by the preparation kernel, and without one it is nullptr here (see inputs_ready)
   float g0 = 1.0f;
   const bool uniform = p.uniform_ok && p.gout != nullptr && gout_uniform(p.gout, p.G, g0);
   const float* xb = uniform ? p.w : p.dx.b_ptr;
@@ -395,6 +475,12 @@ bags_bwd_merged_kernel(const __grid_constant__ CUtensorMap t_dzT, const __grid_c
   if (wg == 0) {
     setmaxnreg_dec<40>();
     if (CW::ANY_MANUAL || tid == 0) {
+      // dz and x: ready at launch when the preparation kernel ran (it triggers only after its own wait); W' is the
+      // preparation kernel's output, W itself is not
+      bool waited = false;
+      if (!p.inputs_ready) { pdl_wait(); waited = true; }
+      const bool wait_dx = !uniform && p.wprime_prepared;
+      if (tl != nullptr) tl[7] = global_timer_ns();
       for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
         if (u < p.dw_units) {
           const int split = u / dw_per_split, t = u - split * dw_per_split;
@@ -405,6 +491,7 @@ bags_bwd_merged_kernel(const __grid_constant__ CUtensorMap t_dzT, const __grid_c
         } else {
           const int t = u - p.dw_units;
           const int m_tile = t / p.dx.num_n_tiles, n_tile = t - m_tile * p.dx.num_n_tiles;
+          if (wait_dx && !waited) { pdl_wait(); waited = true; }
           produce_unit<CX, false, true>(&t_dz, txb, p.dx, xb, m_tile * 128, n_tile * 256, 0, p.dx.kblocks_total, pp, tid);
         }
       }
@@ -412,22 +499,38 @@ bags_bwd_merged_kernel(const __grid_constant__ CUtensorMap t_dzT, const __grid_c
   } else {
     setmaxnreg_inc<232>();
     const int cw = wg - 1, warp = tid >> 5, lane = tid & 31;
+    // first epilogue: dW may still be being zeroed, and db's column-sum partials come from the preparation kernel
+    auto epilogue_wait = [&]() {
+      pdl_wait();
+      if (tl != nullptr) tl[1] = global_timer_ns();
+    };
     float acc[128];
-    for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
+    int i = 0;   // the CTA's unit count (timeline slots)
+    for (int u = blockIdx.x; u < num_units; u += gridDim.x, ++i) {
       if (u < p.dw_units) {
         const int split = u / dw_per_split, t = u - split * dw_per_split;
         const int m_tile = t / p.dw.num_n_tiles, n_tile = t - m_tile * p.dw.num_n_tiles;
         int kb0, kb1;
         split_range(p.dw, split, kb0, kb1);
         consume_unit<CW, true, true, TF32>(acc, cw, kb0, kb1, pp, lane);
+        if (tl != nullptr && i < 3) { tl[2 + 2 * i] = global_timer_ns(); tl[8 + i] = kb1 - kb0; }
+        if (i == 0) epilogue_wait();
         epilogue_unit<256, EPI_RED_F32>(acc, p.dw, m_tile, n_tile, split, cw, warp, lane, 1.0f);
       } else {
         const int t = u - p.dw_units;
         const int m_tile = t / p.dx.num_n_tiles, n_tile = t - m_tile * p.dx.num_n_tiles;
         consume_unit<CX, false, true, TF32>(acc, cw, 0, p.dx.kblocks_total, pp, lane);
-        epilogue_unit<256, TF32 ? EPI_STORE_F32 : EPI_STORE_BF16>(acc, p.dx, m_tile, n_tile, 0, cw, warp, lane, xscale);
+        if (tl != nullptr && i < 3) { tl[2 + 2 * i] = global_timer_ns(); tl[8 + i] = -p.dx.kblocks_total; }
+        if (i == 0) epilogue_wait();
+        if (!TF32 && p.dx_tma)
+          dx_epilogue_tma(acc, &t_dx, stg + cw * (kDxStageBytes / 2), p.dx.M, p.dx.N, m_tile * 128, n_tile * 256, cw,
+                          warp, lane, tid, xscale);
+        else
+          epilogue_unit<256, TF32 ? EPI_STORE_F32 : EPI_STORE_BF16>(acc, p.dx, m_tile, n_tile, 0, cw, warp, lane, xscale);
       }
+      if (tl != nullptr && i < 3) tl[3 + 2 * i] = global_timer_ns();
     }
+    if (!TF32 && p.dx_tma && tid == 0) tma_store_wait_all();   // the staging buffer stays valid until the stores end
   }
 }
 

@@ -570,6 +570,7 @@ struct BwdPrepParams {
   const void* dz; long long ldd; int N; float* colpart; int ctiles;
   int z_ctas, s_ctas, c_ctas;   // CTA ranges of the three jobs (0 = job disabled)
   int skip_scale_if_uniform;    // the consumer reads W itself and scales its output when all gout[g] are equal
+  long long* timing;            // debug timeline rows [0, 2048), one per CTA: start, wait returned, end; or nullptr
 };
 
 // all per-bin upstream gradients equal?  (then diag(gout) W == gout[0] W: no scaled copy of W is needed)
@@ -721,9 +722,14 @@ template <bool F32>
 __global__ void __launch_bounds__(256)
 bwd_prep_kernel(const BwdPrepParams p) {
   __shared__ float s_part[8][64];
+  long long* const tl = (p.timing != nullptr && threadIdx.x == 0 && blockIdx.x < 2048) ? p.timing + blockIdx.x * 8ll
+                                                                                        : nullptr;
+  if (tl != nullptr) tl[0] = global_timer_ns();
   pdl_wait();      // dz comes from the forward kernel; nothing before it may still be running either
-  pdl_trigger();   // from here on the dW GEMM may start: its mainloop only reads dz and x
+  pdl_trigger();   // from here on the backward GEMMs may start: their mainloops only read dz, x and W
+  if (tl != nullptr) tl[1] = global_timer_ns();
   bwd_prep_job<F32, -1>(p, blockIdx.x, threadIdx.x, s_part);
+  if (tl != nullptr) tl[2] = global_timer_ns();
 }
 
 // ----------------------------------------------------------------------------

@@ -251,9 +251,10 @@ int bags_gemm_probe(const void* a, long long lda, int a_mn, const void* b, long 
 
 /* Test hook: point the fused forward (bags_fwd / bags_ce_fwd without logits) and the gradient-exchange kernel
  * (bags_grad_allreduce) at a device buffer of int64 %globaltimer stamps, [blocks][8] slots per kernel.  The fused
- * forward writes rows [0, blocks) (at most 256 CTAs; tools/fused_fwd_phases.py reads its phases), the gradient
- * exchange rows from 4096 on.  The GEMM and backward kernels do not stamp it.  NULL (the default) disables it.
- * Not thread-safe; for profiling only. */
+ * forward writes rows [0, blocks) (at most 256 CTAs; tools/fused_fwd_phases.py reads its phases), the merged
+ * backward two rows per CTA from row 1024 on, the backward's preparation kernel rows [2048, 4096) (one per CTA;
+ * tools/bwd_phases.py reads both), the gradient exchange rows from 4096 on.  The GEMM kernels do not stamp it.
+ * NULL (the default) disables it.  Not thread-safe; for profiling only. */
 int bags_debug_set_timing(void* dev_ptr);
 
 /* The library reads its tuning / experiment switches (BAGS_* environment variables) once per name and caches them;

@@ -3,6 +3,7 @@
 // No torch, no allocations, no device synchronisation.
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
@@ -491,7 +492,7 @@ extern "C" int bags_fused_eligible(const int32_t* slices_host, int G, int C) {
 
 template <bool TF32>
 static int launch_fused_fwd(const void* x, long long ldx, const void* w, long long ldw, const FusedFwdParams& p0,
-                            void* dz, long long ldd, int num_sms, cudaStream_t stream, bool wf) {
+                            void* dz, long long ldd, int num_sms, cudaStream_t stream, bool wf, bool focal = false) {
   using Cfg = FusedCfg<TF32>;
   const int dtype = TF32 ? BAGS_DTYPE_F32 : BAGS_DTYPE_BF16;
   CUtensorMap tx, tw;
@@ -518,7 +519,7 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   p.kblocks = (p.K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
   p.want_dz = dz != nullptr ? 1 : 0;
   p.timing = g_timing;   // rows [0, grid) (grid <= 4 * kFusedMaxGroups); the gradient exchange stamps from row 4096
-  auto kernel = wf ? bags_fwd_fused_kernel<TF32, true> : bags_fwd_fused_kernel<TF32, false>;
+  auto kernel = focal ? bags_focal_fwd_kernel<TF32> : wf ? bags_fwd_fused_kernel<TF32, true> : bags_fwd_fused_kernel<TF32, false>;
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   // persistent grid of CTA groups, all resident at once: the four CTAs of a group wait for each other's softmax
   // partials.  At 4096 RoIs on 132 SMs this is 32 groups, i.e. 128 CTAs in one wave.
@@ -666,6 +667,66 @@ extern "C" int bags_ce_fwd(const void* x, long long ldx, const void* w, long lon
   p.clear_vecs = static_cast<long long>(clear_bytes / 16);
   return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true)
                                   : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true);
+}
+
+// fc_cls + the sigmoid focal loss over all C logits (FocalLoss, focal_loss.py:29-88 with sigmoid_focal_loss_cuda.cu:23-96):
+// the fused kernel's focal variant with one bin (0, C) and fp32 per-RoI weights.  Argument rules as bags_ce_fwd.
+extern "C" int bags_focal_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
+                              const int64_t* targets, const int64_t* labels, const float* weights, float norm,
+                              float gamma, float alpha, int N, int K, int C, int dtype, float* loss, float* acc,
+                              void* dz, long long ldd, float* colsum, int colsum_tiles, void* workspace,
+                              size_t workspace_bytes, void* clear, size_t clear_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  constexpr int kMaxC = FusedCfg<false>::RANKS * FusedCfg<false>::BLOCK_N;
+  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "bags_focal_fwd: bad dtype %d", dtype);
+  BAGS_REQUIRE(N >= 0 && K >= 1 && C >= 1 && C <= kMaxC, "bags_focal_fwd: bad shape N=%d K=%d C=%d (1 <= C <= %d)", N,
+               K, C, kMaxC);
+  BAGS_REQUIRE(loss && workspace && (N == 0 || (x && w && targets)) && (acc == nullptr || N == 0 || labels),
+               "bags_focal_fwd: NULL argument");
+  BAGS_REQUIRE(norm > 0.f && std::isfinite(norm), "bags_focal_fwd: norm=%g must be positive and finite",
+               static_cast<double>(norm));
+  BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "bags_focal_fwd: workspace too small (%zu < %zu)",
+               workspace_bytes, bags_workspace_bytes());
+  BAGS_REQUIRE(acc == nullptr || N <= (1 << 24),
+               "bags_focal_fwd: N=%d: the accuracy count is exact up to 2^24 rows only", N);
+  if (dz != nullptr)
+    BAGS_REQUIRE(ldd >= C && (ldd % 8) == 0, "bags_focal_fwd: ldd=%lld must be a multiple of 8 and >= C", ldd);
+  if (colsum != nullptr)
+    BAGS_REQUIRE(colsum_tiles == (N + 127) / 128 || (N == 0 && colsum_tiles >= 1),
+                 "bags_focal_fwd: colsum must hold ceil(N/128) = %d row tiles of C floats (got %d)", (N + 127) / 128,
+                 colsum_tiles);
+  if (clear != nullptr)
+    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(clear) & 15) == 0 && (clear_bytes % 16) == 0,
+                 "bags_focal_fwd: the buffer to clear must be 16-byte aligned and a multiple of 16 bytes");
+  const int32_t slices[2] = {0, C};
+  GroupTable gt;
+  if (int rc = make_group_table(gt, slices, 1, C)) return rc;
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  if (N == 0) {
+    BAGS_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), stream));
+    if (acc != nullptr) BAGS_CUDA(cudaMemsetAsync(acc, 0, sizeof(float), stream));
+    if (colsum != nullptr) BAGS_CUDA(cudaMemsetAsync(colsum, 0, sizeof(float) * C * colsum_tiles, stream));
+    if (clear != nullptr) BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, stream));
+    return BAGS_OK;
+  }
+  FusedFwdParams p{};
+  p.N = N; p.C = C; p.K = K; p.gt = gt; p.bias = bias;
+  p.labels = reinterpret_cast<const long long*>(labels);
+  p.targets = reinterpret_cast<const long long*>(targets);
+  p.l2b = nullptr; p.classes = C;
+  p.wmask = reinterpret_cast<const uint8_t*>(weights);
+  p.norm = norm; p.gamma = gamma; p.alpha = alpha;
+  p.loss = loss; p.acc = acc; p.acc_scale = static_cast<float>(100.0 / N);   // accuracy.py: correct * (100.0 / N)
+  p.lse = nullptr; p.colsum = colsum;
+  p.counter = reinterpret_cast<unsigned int*>(workspace);
+  p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  p.xch_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes);
+  p.xch = reinterpret_cast<float2*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes + kFusedXchCounterBytes);
+  p.clear = reinterpret_cast<float4*>(clear);
+  p.clear_vecs = static_cast<long long>(clear_bytes / 16);
+  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true, true)
+                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true, true);
 }
 
 extern "C" int bags_reweight(const int64_t* labels, const int32_t* label2bin, const uint8_t* wmask,

@@ -42,6 +42,12 @@
 // The same kernel is the plain softmax-CE head (bags_ce_fwd, reweight_bbox_head.py / bbox_head.py:97-129): one bin
 // (0, C), l2b == nullptr (the label is the target column), fp32 per-RoI weights, and optionally the top-1 accuracy,
 // counted where the loss is formed (z[target] == row max) and reduced with the loss partials.
+//
+// bags_focal_fwd_kernel is the sigmoid focal loss on the same body (bags_focal_fwd; focal_loss.py:29-88,
+// sigmoid_focal_loss_cuda.cu:23-96): one bin (0, C), fp32 per-RoI weights, and per element
+//   pass F  : z := w/norm * grad(z, t) in place, loss += w/norm * l(z, t) (focal_element); z[label] for the accuracy
+// in place of passes A-C's softmax.  Only the accuracy needs the row max, so without it pass A and the exchange are
+// skipped and the CTAs of a group never wait for each other.
 #pragma once
 #include "bags_kernels.cuh"
 #include "bags_ptx.cuh"
@@ -85,7 +91,37 @@ struct FusedFwdParams {
   // 0 start, 1 end of the mainloop, 2 after pass A, 3 after pass B, 4 exchange wait done, 5 end of pass C, 6 end of
   // the CTA.  Slots 1-5 are those of the CTA's last row tile.
   long long* timing;
+  // focal variant only: per-row targets in the op's convention ([N] int64, read as int: column t - 1 is positive, every
+  // other column negative, t < 0 ignores the row), the normaliser (coef = w / norm) and the focal parameters
+  const long long* targets;
+  float norm, gamma, alpha;
 };
+
+// log(FLT_MIN): the op clamps p to FLT_MIN before its log
+constexpr float kLogFltMin = -87.33654475f;
+
+// One element of the sigmoid focal loss, sigmoid_focal_loss_cuda.cu:23-96 in fp32: the loss l and the op's own analytic
+// gradient g (:79-93, not autograd of l) of logit z as a positive (pos) or a negative element.
+//   positive: l = -alpha (1-p)^gamma log(max(p, FLT_MIN))
+//             g = -alpha (1-p)^gamma (1 - p - gamma p log(max(p, FLT_MIN)))
+//   negative: l = -(1-alpha) p^gamma log1m
+//             g = -(1-alpha) p^gamma (gamma (1-p) log1m - p)
+// with p = sigmoid(z) and the op's stable log(1 - p), log1m = -z [z >= 0] - log(1 + exp(-|z|)).  p and 1 - p both come
+// from e = exp(-|z|), so neither loses its relative precision where the other approaches 1; log p = min(z, 0) -
+// log(1 + e) is clamped at log(FLT_MIN) as the op clamps p.  powf(x, 0) = 1 for every x, 0 included.  Both bracketed
+// gradient terms are sums of same-signed parts: no cancellation.
+__device__ __forceinline__ void focal_element(float z, bool pos, float gamma, float alpha, float& l, float& g) {
+  const float e = expf(-fabsf(z));
+  const float r = __frcp_rn(1.f + e);
+  const float p = z >= 0.f ? r : e * r, q = z >= 0.f ? e * r : r;   // p = sigmoid(z), q = 1 - p
+  const float lg = log1pf(e);
+  const float log1m = -fmaxf(z, 0.f) - lg;
+  const float logp = fmaxf(fminf(z, 0.f) - lg, kLogFltMin);
+  const float s = pos ? -alpha : -(1.f - alpha);
+  const float pw = powf(pos ? q : p, gamma);
+  l = s * pw * (pos ? logp : log1m);
+  g = s * pw * (pos ? q - gamma * p * logp : gamma * q * log1m - p);
+}
 
 template <bool TF32>
 struct FusedCfg {
@@ -137,13 +173,15 @@ __device__ __forceinline__ unsigned int ld_acquire_gpu(const unsigned int* addr)
   return v;
 }
 
+// The body of both kernels below.  (The parameters are taken by value: with a reference, the existing instantiations
+// compile to different SASS than as kernels of their own.)
 // WF = true: p.wmask points at fp32 per-(bin, RoI) weights instead of 0/1 bytes (the reweight head variant,
 // gs_bbox_head_with0_reweight.py:57-85)
+// FOCAL = true: the sigmoid focal loss (pass F) instead of the softmax CE (passes A-C); one bin, WF
 // tmap_dz: dz [N, C] in the operand dtype (row stride ldd), boxes of BOX_COLS x 128, 128B swizzle; unused without dz
-template <bool TF32, bool WF = false>
-__global__ void __launch_bounds__(FusedCfg<TF32>::NUM_THREADS, 1)
-bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                      const __grid_constant__ CUtensorMap tmap_dz, const FusedFwdParams p) {
+template <bool TF32, bool WF, bool FOCAL>
+__device__ __forceinline__ void fused_fwd_body(const CUtensorMap& tmap_x, const CUtensorMap& tmap_w,
+                                               const CUtensorMap& tmap_dz, const FusedFwdParams p) {
   using Cfg = FusedCfg<TF32>;
   constexpr int BLOCK_M = Cfg::BLOCK_M, BLOCK_N = Cfg::BLOCK_N, BLOCK_K = Cfg::BLOCK_K, STAGES = Cfg::STAGES;
   constexpr int MAXG = Cfg::MAXG, HALF_N = Cfg::HALF_N, RANKS = Cfg::RANKS;
@@ -253,7 +291,15 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   static_assert(Cfg::NUM_THREADS == 2 * BLOCK_M && MAXG == 6, "row information: two threads per row, three bins each");
   const int info_row = tid & (BLOCK_M - 1), info_g0 = tid / BLOCK_M;
   const bool info_ok = m0 + info_row < p.N;
-  {
+  if constexpr (FOCAL) {
+    // slot 0: the label column of the accuracy (-1: none); slot 1: the target t (the op reads `int t = targets[n]`)
+    if (info_g0 == 0) {
+      const long long lab = (info_ok && p.labels != nullptr) ? __ldg(p.labels + m0 + info_row) : -1;
+      s_tcol[info_row] = (lab >= 0 && lab < p.C) ? static_cast<int>(lab) : -1;
+    } else {
+      s_tcol[BLOCK_M + info_row] = info_ok ? static_cast<int>(__ldg(p.targets + m0 + info_row)) : -1;
+    }
+  } else {
     const long long lab = info_ok ? __ldg(p.labels + m0 + info_row) : -1;
     const bool lab_ok = info_ok && lab >= 0 && lab < p.classes;
     for (int g = info_g0; g < G; g += 2) {
@@ -329,7 +375,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
                 ? (WF ? __ldg(reinterpret_cast<const float*>(p.wmask) + static_cast<long long>(g) * p.N + row)
                       : static_cast<float>(__ldg(p.wmask + static_cast<long long>(g) * p.N + row)))
                 : 1.0f;
-      inv_avg = 1.0f / (p.avg != nullptr ? __ldg(p.avg + g) : fmaxf(static_cast<float>(p.N), 1.0f));
+      inv_avg = 1.0f / (FOCAL ? p.norm : (p.avg != nullptr ? __ldg(p.avg + g) : fmaxf(static_cast<float>(p.N), 1.0f)));
     }
     info_coef[i] = w * inv_avg;
   }
@@ -349,40 +395,44 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   // per-thread partials of (bin, row slot) -> s_part; the running pair is flushed where the bin changes
 #define BAGS_PART(g, rr) s_part[((g) * 2 + (rr)) * 256 + tid]
 
+  // the row max and the group's exchange: always for the softmax, for the focal loss only for its accuracy
+  const bool xchg = !FOCAL || p.acc != nullptr;
   // ---- pass A: per-bin max over this thread's columns, then over the quad ----
+  if (xchg) {
 #pragma unroll
-  for (int g = 0; g < MAXG; ++g) BAGS_PART(g, 0) = BAGS_PART(g, 1) = -INFINITY;
-  {
-    int gc = -1;
-    float mc[2] = {-INFINITY, -INFINITY};
-    auto stepA = [&](float z0, float z1, int c) {
-      const int b = s_colbin[c];
-      if (b != gc) {
-        if (gc >= 0) { BAGS_PART(gc, 0) = mc[0]; BAGS_PART(gc, 1) = mc[1]; }
-        gc = b; mc[0] = mc[1] = -INFINITY;
-      }
-      mc[0] = fmaxf(mc[0], z0);
-      mc[1] = fmaxf(mc[1], z1);
-    };
-    auto chunkA = [&](float (&a)[80], int j, int J, int c) {
-      if (BAGS_IS_SLOW(J)) {
-        stepA(a[4 * j], a[4 * j + 2], c);
-        stepA(a[4 * j + 1], a[4 * j + 3], c + 1);
-      } else {
-        mc[0] = fmaxf(fmaxf(mc[0], a[4 * j]), a[4 * j + 1]);
-        mc[1] = fmaxf(fmaxf(mc[1], a[4 * j + 2]), a[4 * j + 3]);
-      }
-    };
-    BAGS_CHUNKS(chunkA);
-    if (gc >= 0) { BAGS_PART(gc, 0) = mc[0]; BAGS_PART(gc, 1) = mc[1]; }
-  }
-  for (int g = 0; g < G; ++g) {
+    for (int g = 0; g < MAXG; ++g) BAGS_PART(g, 0) = BAGS_PART(g, 1) = -INFINITY;
+    {
+      int gc = -1;
+      float mc[2] = {-INFINITY, -INFINITY};
+      auto stepA = [&](float z0, float z1, int c) {
+        const int b = s_colbin[c];
+        if (b != gc) {
+          if (gc >= 0) { BAGS_PART(gc, 0) = mc[0]; BAGS_PART(gc, 1) = mc[1]; }
+          gc = b; mc[0] = mc[1] = -INFINITY;
+        }
+        mc[0] = fmaxf(mc[0], z0);
+        mc[1] = fmaxf(mc[1], z1);
+      };
+      auto chunkA = [&](float (&a)[80], int j, int J, int c) {
+        if (BAGS_IS_SLOW(J)) {
+          stepA(a[4 * j], a[4 * j + 2], c);
+          stepA(a[4 * j + 1], a[4 * j + 3], c + 1);
+        } else {
+          mc[0] = fmaxf(fmaxf(mc[0], a[4 * j]), a[4 * j + 1]);
+          mc[1] = fmaxf(fmaxf(mc[1], a[4 * j + 2]), a[4 * j + 3]);
+        }
+      };
+      BAGS_CHUNKS(chunkA);
+      if (gc >= 0) { BAGS_PART(gc, 0) = mc[0]; BAGS_PART(gc, 1) = mc[1]; }
+    }
+    for (int g = 0; g < G; ++g) {
 #pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      float m = BAGS_PART(g, rr);
-      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
-      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
-      if (q == 0) s_mrow[g * BLOCK_M + row_l0 + 8 * rr] = m;
+      for (int rr = 0; rr < 2; ++rr) {
+        float m = BAGS_PART(g, rr);
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+        if (q == 0) s_mrow[g * BLOCK_M + row_l0 + 8 * rr] = m;
+      }
     }
   }
 #pragma unroll
@@ -391,71 +441,117 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   __syncthreads();   // s_tcol / s_coef of every row; s_mrow of the quad
   if (tid == 0) stamp(p.timing, 2);
 
-  // ---- pass B: z := e = exp(z - max) in place, per-bin sum of e; z[target] for the loss ----
+  if constexpr (FOCAL) {
+    // ---- pass F: z := w/norm * grad(z, t) in place, loss += w/norm * l(z, t); z[label] for the accuracy.
+    // Columns >= C (the slow chunks' s_colbin < 0) get dz = 0 and no loss.  The loss goes per warp to
+    // s_loss[8 + warp] and is added to s_loss[0] in warp order below, so that it does not depend on the warps' timing.
+    // ----
+    const float gamma = p.gamma, alpha = p.alpha;
+    float cf[2], zl[2] = {0.f, 0.f}, ls = 0.f;
+    int tp[2], tl[2];
 #pragma unroll
-  for (int g = 0; g < MAXG; ++g) BAGS_PART(g, 0) = BAGS_PART(g, 1) = 0.f;
-  {
-    int gc = -1;
-    float mb[2] = {0.f, 0.f}, sc[2] = {0.f, 0.f}, zt[2] = {0.f, 0.f};
-    int tc[2] = {-1, -1};
-    // z[target] is picked into a register on the way and stored where the bin ends, by the lane that holds the
-    // target column (the target lies inside its bin)
-    auto flushB = [&]() {
-      if (gc >= 0) {
-        BAGS_PART(gc, 0) = sc[0]; BAGS_PART(gc, 1) = sc[1];
+    for (int rr = 0; rr < 2; ++rr) {
+      const int row_l = row_l0 + 8 * rr, t = s_tcol[BLOCK_M + row_l];
+      cf[rr] = t >= 0 ? s_coef[row_l] : 0.f;
+      tp[rr] = t >= 0 ? t - 1 - n0 : -1;   // local positive column (never matched when outside this CTA)
+      tl[rr] = s_tcol[row_l] - n0;          // local label column
+    }
+    auto elemF = [&](float& z, int rr, int c, bool in) {
+      zl[rr] = (c == tl[rr]) ? z : zl[rr];
+      float l, g;
+      focal_element(z, c == tp[rr], gamma, alpha, l, g);
+      ls += in ? cf[rr] * l : 0.f;
+      z = in ? cf[rr] * g : 0.f;
+    };
+    auto chunkF = [&](float (&a)[80], int j, int J, int c) {
+      const bool lookup = BAGS_IS_SLOW(J);
 #pragma unroll
-        for (int rr = 0; rr < 2; ++rr)
-          if (tc[rr] >= 0 && tc[rr] < BLOCK_N && ((tc[rr] >> 1) & 3) == q) s_zt[gc * BLOCK_M + row_l0 + 8 * rr] = zt[rr];
+      for (int e = 0; e < 2; ++e) {
+        const bool in = !lookup || s_colbin[c + e] >= 0;
+        elemF(a[4 * j + e], 0, c + e, in);
+        elemF(a[4 * j + 2 + e], 1, c + e, in);
       }
     };
-    auto expB = [&](float& z0, float& z1, int c) {
-      zt[0] = (c == tc[0]) ? z0 : zt[0];
-      zt[1] = (c == tc[1]) ? z1 : zt[1];
-      z0 = exp2f(fmaf(z0, kLog2e, -mb[0]));
-      z1 = exp2f(fmaf(z1, kLog2e, -mb[1]));
-      sc[0] += z0;
-      sc[1] += z1;
-    };
-    auto stepB = [&](float& z0, float& z1, int c) {
-      const int b = s_colbin[c];
-      if (b != gc) {
-        flushB();
-        gc = b; sc[0] = sc[1] = 0.f;
-        if (b >= 0) {
+    BAGS_CHUNKS(chunkF);
+    if (xchg) {
 #pragma unroll
-          for (int rr = 0; rr < 2; ++rr) {
-            mb[rr] = s_mrow[b * BLOCK_M + row_l0 + 8 * rr] * kLog2e;
-            tc[rr] = s_tcol[b * BLOCK_M + row_l0 + 8 * rr] - n0;   // local column of the target
+      for (int rr = 0; rr < 2; ++rr)
+        if (tl[rr] >= 0 && tl[rr] < BLOCK_N && ((tl[rr] >> 1) & 3) == q) s_zt[row_l0 + 8 * rr] = zl[rr];
+    }
+    ls = warp_sum(ls);
+    if (lane == 0) s_loss[8 + (tid >> 5)] = ls;
+  } else {
+    // ---- pass B: z := e = exp(z - max) in place, per-bin sum of e; z[target] for the loss ----
+#pragma unroll
+    for (int g = 0; g < MAXG; ++g) BAGS_PART(g, 0) = BAGS_PART(g, 1) = 0.f;
+    {
+      int gc = -1;
+      float mb[2] = {0.f, 0.f}, sc[2] = {0.f, 0.f}, zt[2] = {0.f, 0.f};
+      int tc[2] = {-1, -1};
+      // z[target] is picked into a register on the way and stored where the bin ends, by the lane that holds the
+      // target column (the target lies inside its bin)
+      auto flushB = [&]() {
+        if (gc >= 0) {
+          BAGS_PART(gc, 0) = sc[0]; BAGS_PART(gc, 1) = sc[1];
+#pragma unroll
+          for (int rr = 0; rr < 2; ++rr)
+            if (tc[rr] >= 0 && tc[rr] < BLOCK_N && ((tc[rr] >> 1) & 3) == q)
+              s_zt[gc * BLOCK_M + row_l0 + 8 * rr] = zt[rr];
+        }
+      };
+      auto expB = [&](float& z0, float& z1, int c) {
+        zt[0] = (c == tc[0]) ? z0 : zt[0];
+        zt[1] = (c == tc[1]) ? z1 : zt[1];
+        z0 = exp2f(fmaf(z0, kLog2e, -mb[0]));
+        z1 = exp2f(fmaf(z1, kLog2e, -mb[1]));
+        sc[0] += z0;
+        sc[1] += z1;
+      };
+      auto stepB = [&](float& z0, float& z1, int c) {
+        const int b = s_colbin[c];
+        if (b != gc) {
+          flushB();
+          gc = b; sc[0] = sc[1] = 0.f;
+          if (b >= 0) {
+#pragma unroll
+            for (int rr = 0; rr < 2; ++rr) {
+              mb[rr] = s_mrow[b * BLOCK_M + row_l0 + 8 * rr] * kLog2e;
+              tc[rr] = s_tcol[b * BLOCK_M + row_l0 + 8 * rr] - n0;   // local column of the target
+            }
           }
         }
-      }
-      if (b >= 0) expB(z0, z1, c);
-    };
-    auto chunkB = [&](float (&a)[80], int j, int J, int c) {
-      if (BAGS_IS_SLOW(J)) {
-        stepB(a[4 * j], a[4 * j + 2], c);
-        stepB(a[4 * j + 1], a[4 * j + 3], c + 1);
-      } else {
-        expB(a[4 * j], a[4 * j + 2], c);
-        expB(a[4 * j + 1], a[4 * j + 3], c + 1);
-      }
-    };
-    BAGS_CHUNKS(chunkB);
-    flushB();
+        if (b >= 0) expB(z0, z1, c);
+      };
+      auto chunkB = [&](float (&a)[80], int j, int J, int c) {
+        if (BAGS_IS_SLOW(J)) {
+          stepB(a[4 * j], a[4 * j + 2], c);
+          stepB(a[4 * j + 1], a[4 * j + 3], c + 1);
+        } else {
+          expB(a[4 * j], a[4 * j + 2], c);
+          expB(a[4 * j + 1], a[4 * j + 3], c + 1);
+        }
+      };
+      BAGS_CHUNKS(chunkB);
+      flushB();
+    }
   }
 
-  // ---- exchange: publish (max, sum) of every (row, bin) to the group's slot of this tile's parity ----
+  // ---- exchange: publish (max, sum) of every (row, bin) to the group's slot of this tile's parity (the focal loss:
+  // (max, 0)) ----
   // Two slots suffice: a CTA writes the slot of its tile i + 2 only after it has seen all four arrivals of tile i + 1,
   // and a peer arrives for tile i + 1 only after it has read its partials of tile i.
   float2* xch = p.xch + static_cast<size_t>(group * 2 + (tile_i & 1)) * Cfg::SLOT_ELEMS;   // [4 ranks][MAXG][128]
-  {
+  if (xchg) {
     float2* mine = xch + rank * MAXG * BLOCK_M;
     for (int g = 0; g < G; ++g) {
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
-        float s = BAGS_PART(g, rr);
-        s += __shfl_xor_sync(0xffffffffu, s, 1);
-        s += __shfl_xor_sync(0xffffffffu, s, 2);
+        float s = 0.f;
+        if constexpr (!FOCAL) {
+          s = BAGS_PART(g, rr);
+          s += __shfl_xor_sync(0xffffffffu, s, 1);
+          s += __shfl_xor_sync(0xffffffffu, s, 2);
+        }
         if (q == 0) {
           const int row_l = row_l0 + 8 * rr;
           mine[g * BLOCK_M + row_l] = make_float2(s_mrow[g * BLOCK_M + row_l], s);
@@ -468,10 +564,14 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   unsigned int xch_target = 0;
   if (tid == 0) {
     stamp(p.timing, 3);
+    if constexpr (FOCAL) s_loss[0] += ((s_loss[8] + s_loss[9]) + (s_loss[10] + s_loss[11])) +
+                                      ((s_loss[12] + s_loss[13]) + (s_loss[14] + s_loss[15]));
     // Arrival counters are never reset: every tile adds four arrivals, so a tile's four arrivals are the ones that
     // take the counter to the next multiple of 4 -- across tiles, launches and graph replays on one stream.
-    __threadfence();
-    xch_target = (atom_add_release_gpu(xch_counter, 1u) & ~3u) + 4u;
+    if (xchg) {
+      __threadfence();
+      xch_target = (atom_add_release_gpu(xch_counter, 1u) & ~3u) + 4u;
+    }
   }
   // The optional buffer clear (a write: only after the wait -- the buffer may still be in use by an earlier kernel) is
   // issued while the peers' partials are awaited.
@@ -481,7 +581,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     for (long long i = static_cast<long long>(blockIdx.x) * Cfg::NUM_THREADS + tid; i < p.clear_vecs; i += stride)
       p.clear[i] = zero4;
   }
-  if (tid == 0) {
+  if (tid == 0 && xchg) {
     uint32_t spins = 0, ns = 32;
     while (static_cast<int>(ld_acquire_gpu(xch_counter) - xch_target) < 0) {
       if (++spins > BAGS_WAIT_LIMIT) __trap();
@@ -497,7 +597,7 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
   // rather than at the start of the kernel made the 4096-RoI benchmark step about 3 % faster on an H100 80GB HBM3 at
   // 400 W.)  Dependents guard their first dependent access with griddepcontrol.wait.
   if (tile_i == 0) pdl_trigger();
-  {
+  if (xchg) {
     // The quad's 2 x G (row, bin) pairs k = 2 g + rr are spread over its four lanes (lane q: k = q, q + 4, q + 8), and
     // every lane issues all its L2 loads before it uses any.
     constexpr int PAIRS = 2 * MAXG / 4;
@@ -512,7 +612,11 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
 #pragma unroll
     for (int i = 0; i < PAIRS; ++i) {
       const int k = q + 4 * i, g = k >> 1, row_l = row_l0 + 8 * (k & 1), row = m0 + row_l;
-      if (g < G) {
+      if (FOCAL && g < G) {   // the accuracy only
+        const float M = fmaxf(fmaxf(v[i][0].x, v[i][1].x), fmaxf(v[i][2].x, v[i][3].x));
+        const int tcol = s_tcol[row_l];
+        if (tcol >= n0 && tcol < n0 + BLOCK_N && row < p.N && s_zt[row_l] == M) atomicAdd(&s_loss[kMaxG - 1], 1.f);
+      } else if (g < G) {
         const float M = fmaxf(fmaxf(v[i][0].x, v[i][1].x), fmaxf(v[i][2].x, v[i][3].x));
         float S = 0.f;
 #pragma unroll
@@ -575,7 +679,13 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     };
     auto chunkC = [&](float (&a)[80], int j, int J, int c) {
       float d[2][2];
-      if (BAGS_IS_SLOW(J)) {
+      if (FOCAL) {   // pass F left dz in the accumulators
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          d[0][e] = a[4 * j + e];
+          d[1][e] = a[4 * j + 2 + e];
+        }
+      } else if (BAGS_IS_SLOW(J)) {
         stepC(a[4 * j], a[4 * j + 2], c, d[0][0], d[1][0]);
         stepC(a[4 * j + 1], a[4 * j + 3], c + 1, d[0][1], d[1][1]);
       } else {
@@ -671,6 +781,22 @@ bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_c
     tma_store_wait_all();   // the dz stores have read the stages and are complete
     stamp(p.timing, 6);
   }
+}
+
+// the grouped softmax CE (bags_fwd) and the plain softmax CE (bags_ce_fwd, WF)
+template <bool TF32, bool WF = false>
+__global__ void __launch_bounds__(FusedCfg<TF32>::NUM_THREADS, 1)
+bags_fwd_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+                      const __grid_constant__ CUtensorMap tmap_dz, const FusedFwdParams p) {
+  fused_fwd_body<TF32, WF, false>(tmap_x, tmap_w, tmap_dz, p);
+}
+
+// the sigmoid focal loss (bags_focal_fwd)
+template <bool TF32>
+__global__ void __launch_bounds__(FusedCfg<TF32>::NUM_THREADS, 1)
+bags_focal_fwd_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
+                      const __grid_constant__ CUtensorMap tmap_dz, const FusedFwdParams p) {
+  fused_fwd_body<TF32, true, true>(tmap_x, tmap_w, tmap_dz, p);
 }
 
 }  // namespace bags

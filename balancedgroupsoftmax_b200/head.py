@@ -37,7 +37,8 @@ from torch.nn.modules.utils import _pair
 
 from . import ops
 from .fp16 import auto_fp16, force_fp32
-from .losses import CrossEntropyLoss, SmoothL1Loss, accuracy  # noqa: F401  (registers them)
+from .losses import CrossEntropyLoss, FocalLoss, SmoothL1Loss, accuracy  # noqa: F401  (registers them)
+from .losses import FOCAL_ONE_HOT_CLASSES, focal_targets
 from .registry import HEADS, build_loss, register
 from .tables import GroupTables, load_reference_files
 
@@ -810,9 +811,9 @@ class ReweightBBoxHead(NativeFcClsHead):
 
     In training with a softmax ``CrossEntropyLoss`` (reduction 'mean') as ``loss_cls``, fc_cls, the weighted CE and the
     accuracy run in one fused kernel (``ops.SoftmaxCEFunction``: the [N, C] logits never reach memory) and the
-    backward in one bags_bwd call; dX is computed only when the RoI features need a gradient.  Any other ``loss_cls``
-    (e.g. the FocalLoss of reweighthead_bfocal) or ``reduction_override`` runs the reference's op sequence on
-    materialised logits."""
+    backward in one bags_bwd call; dX is computed only when the RoI features need a gradient.  A sigmoid ``FocalLoss``
+    with reduction 'mean' (reweighthead_bfocal) takes the same fused route (``ops.SigmoidFocalFunction``).  Any other
+    ``loss_cls`` or ``reduction_override`` runs the reference's op sequence on materialised logits."""
 
     def __init__(self, num_fcs=2, fc_out_channels=1024, reweight_cfg=None, *args, **kwargs):
         super().__init__(num_fcs=num_fcs, fc_out_channels=fc_out_channels, *args, **kwargs)
@@ -837,10 +838,19 @@ class ReweightBBoxHead(NativeFcClsHead):
             w = self._cls_weight_dev[idx] = self.cls_weight.to(labels.device)
         return w[labels]
 
-    def _fused_loss_ok(self) -> bool:
+    def _fused_loss_ok(self) -> Optional[str]:
+        """'ce' for a softmax CrossEntropyLoss, 'focal' for a sigmoid FocalLoss, both with reduction 'mean' (recognised
+        by type name and attributes, so mmdet's own classes qualify too); None: the materialised route."""
         lc = self.loss_cls
-        return (type(lc).__name__ == 'CrossEntropyLoss' and not getattr(lc, 'use_sigmoid', False)
-                and not getattr(lc, 'use_mask', False) and getattr(lc, 'reduction', None) == 'mean')
+        if getattr(lc, 'reduction', None) != 'mean':
+            return None
+        name = type(lc).__name__
+        if name == 'CrossEntropyLoss' and not getattr(lc, 'use_sigmoid', False) and not getattr(lc, 'use_mask', False):
+            return 'ce'
+        if (name == 'FocalLoss' and getattr(lc, 'use_sigmoid', False) is True
+                and all(isinstance(getattr(lc, k, None), (int, float)) for k in ('gamma', 'alpha', 'loss_weight'))):
+            return 'focal'
+        return None
 
     @force_fp32(apply_to=('cls_score', 'bbox_pred'))
     def loss(self, cls_score, bbox_pred, labels, label_weights, bbox_targets, bbox_weights, reduction_override=None):
@@ -848,12 +858,21 @@ class ReweightBBoxHead(NativeFcClsHead):
         if cls_score is not None:
             assert reduction_override in (None, 'none', 'mean', 'sum')
             weight = self._reweight(labels)
-            if (reduction_override in (None, 'mean') and self._fused_loss_ok() and isinstance(cls_score, ClsScoreHandle)
+            kind = self._fused_loss_ok()
+            if (reduction_override in (None, 'mean') and kind is not None and isinstance(cls_score, ClsScoreHandle)
                     and cls_score._logits is None):
-                avg = (label_weights > 0).sum(dtype=torch.float32).clamp_min(1.0).reshape(1)
                 acc = torch.empty((1,), dtype=torch.float32, device=labels.device)
-                loss = ops.SoftmaxCEFunction.apply(cls_score.x_cls, self.fc_cls.weight, self.fc_cls.bias, labels,
-                                                   weight, avg, self.compute_dtype, acc)[0]
+                if kind == 'focal':
+                    # FocalLoss.forward: the one-hot targets' quirk, and avg_factor = N * 1231 whatever the caller passes
+                    lc, N = self.loss_cls, labels.numel()
+                    loss = ops.SigmoidFocalFunction.apply(
+                        cls_score.x_cls, self.fc_cls.weight, self.fc_cls.bias, focal_targets(labels, N), weight,
+                        max(float(N * FOCAL_ONE_HOT_CLASSES), 1.), float(lc.gamma), float(lc.alpha), self.compute_dtype,
+                        labels, acc)[0]
+                else:
+                    avg = (label_weights > 0).sum(dtype=torch.float32).clamp_min(1.0).reshape(1)
+                    loss = ops.SoftmaxCEFunction.apply(cls_score.x_cls, self.fc_cls.weight, self.fc_cls.bias, labels,
+                                                       weight, avg, self.compute_dtype, acc)[0]
                 lw = self.loss_cls.loss_weight
                 losses['loss_cls'] = loss if lw == 1.0 else loss * lw
                 losses['acc'] = acc

@@ -278,11 +278,57 @@ def ce_fwd(x, w, bias, labels, weights=None, avg=None, want_acc: bool = False, w
     ``want_acc``: also the top-1 accuracy in percent (ties with the row maximum count as correct), written into
     ``acc_out`` when given.  ``clear``: as in ``fused_fwd``."""
     _require_cuda(x, w, bias, labels, weights, avg, clear, acc_out)
+    x, w, bias, weights, loss, acc, dz, ldd, colsum = _single_bin_args(x, w, bias, weights, want_acc, want_dz,
+                                                                       want_colsum, clear, acc_out)
+    labels = labels.contiguous()
+    N, K = x.shape
+    if avg is not None:
+        assert avg.dtype == torch.float32 and avg.numel() >= 1
+    ws = _workspace(x.device)
+    nat.check(nat.lib().bags_ce_fwd(
+        x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(), nat.ptr(weights),
+        nat.ptr(avg), N, K, w.shape[0], _dtype_code(x.dtype), loss.data_ptr(), nat.ptr(acc), nat.ptr(dz), ldd,
+        nat.ptr(colsum), colsum.shape[0] if colsum is not None else 0, ws.data_ptr(), ws.numel(), nat.ptr(clear),
+        clear.numel() * clear.element_size() if clear is not None else 0, _stream_ptr(x.device)), 'bags_ce_fwd')
+    return loss, acc, dz, colsum
+
+
+def focal_fwd(x, w, bias, targets, norm: float, gamma: float = 2.0, alpha: float = 0.25, labels=None, weights=None,
+              want_acc: bool = False, want_dz: bool = True, want_colsum: bool = False,
+              clear: Optional[torch.Tensor] = None, acc_out: Optional[torch.Tensor] = None):
+    """bags_focal_fwd: fc_cls + the sigmoid focal loss over all C logits in the fused kernel (FocalLoss with
+    ReweightBBoxHead).  Returns (loss [1], acc [1] | None, dz [N, pad_cols(C)] | None, colsum [ceil(N/128), C] | None).
+
+    ``targets``: int64 [N] in the focal-loss op's convention (column t - 1 positive, t < 0 ignores the row; see
+    ``losses.focal_targets``); ``norm``: the host-known divisor (N * 1231 for FocalLoss); ``labels``: int64 [N], for the
+    accuracy only.  ``weights``, ``want_acc``, ``clear``, ``acc_out``: as in ``ce_fwd``."""
+    _require_cuda(x, w, bias, targets, labels, weights, clear, acc_out)
+    x, w, bias, weights, loss, acc, dz, ldd, colsum = _single_bin_args(x, w, bias, weights, want_acc, want_dz,
+                                                                       want_colsum, clear, acc_out)
+    targets = targets.contiguous()
+    assert targets.dtype == torch.int64 and targets.numel() == x.shape[0]
+    if want_acc:
+        if labels is None:
+            raise nat.BagsNativeError('focal_fwd: the accuracy needs the labels')
+        labels = labels.contiguous()
+        assert labels.dtype == torch.int64 and labels.numel() == x.shape[0]
+    N, K = x.shape
+    ws = _workspace(x.device)
+    nat.check(nat.lib().bags_focal_fwd(
+        x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), targets.data_ptr(),
+        nat.ptr(labels) if want_acc else None, nat.ptr(weights), float(norm), float(gamma), float(alpha), N, K,
+        w.shape[0], _dtype_code(x.dtype), loss.data_ptr(), nat.ptr(acc), nat.ptr(dz), ldd, nat.ptr(colsum),
+        colsum.shape[0] if colsum is not None else 0, ws.data_ptr(), ws.numel(), nat.ptr(clear),
+        clear.numel() * clear.element_size() if clear is not None else 0, _stream_ptr(x.device)), 'bags_focal_fwd')
+    return loss, acc, dz, colsum
+
+
+def _single_bin_args(x, w, bias, weights, want_acc, want_dz, want_colsum, clear, acc_out):
+    """Operands and outputs shared by ce_fwd and focal_fwd: (x, w, bias, weights, loss, acc, dz, ldd, colsum)."""
     x, w = _row_major(x), _row_major(w)
     if x.dtype != w.dtype:
         raise nat.BagsNativeError('x (%s) and w (%s) must share a dtype' % (x.dtype, w.dtype))
-    labels = labels.contiguous()
-    N, K = x.shape
+    N = x.shape[0]
     Cc = w.shape[0]
     dev = x.device
     if bias is not None:
@@ -291,8 +337,6 @@ def ce_fwd(x, w, bias, labels, weights=None, avg=None, want_acc: bool = False, w
     if weights is not None:
         weights = weights.to(torch.float32).contiguous()
         assert weights.numel() == N
-    if avg is not None:
-        assert avg.dtype == torch.float32 and avg.numel() >= 1
     loss = torch.empty((1,), dtype=torch.float32, device=dev)
     acc = None
     if want_acc:
@@ -307,13 +351,7 @@ def ce_fwd(x, w, bias, labels, weights=None, avg=None, want_acc: bool = False, w
             colsum = torch.empty((max((N + 127) // 128, 1), Cc), dtype=torch.float32, device=dev)
     if clear is not None:
         assert clear.is_contiguous() and (clear.numel() * clear.element_size()) % 16 == 0
-    ws = _workspace(dev)
-    nat.check(nat.lib().bags_ce_fwd(
-        x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(), nat.ptr(weights),
-        nat.ptr(avg), N, K, Cc, _dtype_code(x.dtype), loss.data_ptr(), nat.ptr(acc), nat.ptr(dz), ldd, nat.ptr(colsum),
-        colsum.shape[0] if colsum is not None else 0, ws.data_ptr(), ws.numel(), nat.ptr(clear),
-        clear.numel() * clear.element_size() if clear is not None else 0, _stream_ptr(dev)), 'bags_ce_fwd')
-    return loss, acc, dz, colsum
+    return x, w, bias, weights, loss, acc, dz, ldd, colsum
 
 
 _scratch_cache: Dict[Tuple, torch.Tensor] = {}
@@ -723,14 +761,51 @@ class SoftmaxCEFunction(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_loss):
-        xc, wc, dz = ctx.saved_tensors
-        need_dx, need_dw, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-        dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
-        dW, db, dX = fused_bwd(dz, xc, wc, _gout(grad_loss), _single_slice_tables(ctx.num_cols, xc.device), None,
-                               need_dw=need_dw, need_db=(need_db and ctx.has_bias), need_dx=need_dx,
-                               dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None)
-        dX, dW, db = _grads_in_param_dtypes(ctx, dX, dW, db)
-        return dX, dW, db, None, None, None, None, None
+        return _single_bin_bwd(ctx, grad_loss) + (None,) * 5
+
+
+def _single_bin_bwd(ctx, grad_loss):
+    """(dX, dW, db) in the parameters' dtypes from the dz~ a single-bin fused forward saved: one bags_bwd over the slice
+    (0, C); dX only when x needs a gradient, dW zeroed by the forward kernel when ``ctx.dW`` is set."""
+    xc, wc, dz = ctx.saved_tensors
+    need_dx, need_dw, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+    dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
+    dW, db, dX = fused_bwd(dz, xc, wc, _gout(grad_loss), _single_slice_tables(ctx.num_cols, xc.device), None,
+                           need_dw=need_dw, need_db=(need_db and ctx.has_bias), need_dx=need_dx,
+                           dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None)
+    return _grads_in_param_dtypes(ctx, dX, dW, db)
+
+
+class SigmoidFocalFunction(torch.autograd.Function):
+    """loss[1] = sigmoid focal loss of fc_cls(x) over all C logits, per-RoI weighted, divided by ``norm``
+    (FocalLoss(use_sigmoid=True) in ReweightBBoxHead.loss) -- the focal counterpart of ``SoftmaxCEFunction``:
+
+    forward : bags_focal_fwd (fused fc_cls GEMM + the focal loss and the op's analytic gradient per element; logits stay
+              on chip; saves dz~; optional top-1 accuracy of ``labels`` into ``acc_out``)
+    backward: bags_bwd over the single slice (0, C), as SoftmaxCEFunction.  ``norm`` is a host number (from shapes): no
+              host sync."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, targets, weights, norm, gamma, alpha, compute_dtype, labels=None, acc_out=None):
+        _require_cuda(x, weight, bias, targets)
+        xc, wc, b32 = _fc_cls_operands(x, weight, bias, compute_dtype)
+        need_grad = any(ctx.needs_input_grad[:3])
+        dW = None
+        if need_grad and ctx.needs_input_grad[1] and PREP_IN_FORWARD:
+            dW = torch.empty((wc.shape[0], wc.shape[1]), dtype=torch.float32, device=xc.device)
+        loss, _, dz, _ = focal_fwd(xc, wc, b32, targets, norm, gamma, alpha, labels=labels, weights=weights,
+                                   want_acc=acc_out is not None, want_dz=need_grad, clear=dW, acc_out=acc_out)
+        ctx.dW = dW
+        ctx.num_cols = wc.shape[0]
+        _save_param_dtypes(ctx, x, weight, bias)
+        if need_grad:
+            ctx.save_for_backward(xc, wc, dz)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss):
+        return _single_bin_bwd(ctx, grad_loss) + (None,) * 8
 
 
 class GroupCEFunction(torch.autograd.Function):

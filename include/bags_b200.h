@@ -20,6 +20,8 @@
  *   fc_cls + loss in one call                             bags_fwd
  *   ReweightBBoxHead.loss: fc_cls + weighted softmax CE   bags_ce_fwd
  *     + accuracy (reweight_bbox_head.py:36-55)
+ *   fc_cls + FocalLoss (sigmoid) + accuracy              bags_focal_fwd
+ *     focal_loss.py:29-88, sigmoid_focal_loss_cuda.cu:23-96
  *   autograd backward of the above (dW, db, dX)           bags_bwd
  *     triggered at mmdet/core/utils/dist_utils.py:53
  *   GSBBoxHeadWith0._merge_score                          bags_merge_scores
@@ -141,6 +143,29 @@ int bags_ce_fwd(const void* x, long long ldx, const void* w, long long ldw, cons
                 const float* weights, const float* avg, int N, int K, int C, int dtype, float* loss, float* acc,
                 void* dz, long long ldd, float* colsum, int colsum_tiles, void* workspace, size_t workspace_bytes,
                 void* clear, size_t clear_bytes, void* stream);
+
+/* fc_cls + the sigmoid focal loss over all C logits, logits kept on chip -- replaces FocalLoss.forward
+ * (mmdet/models/losses/focal_loss.py:63-88), sigmoid_focal_loss + weight_reduce_loss (:29-43, losses/utils.py:26-53) and
+ * the op's forward and backward kernels (mmdet/ops/sigmoid_focal_loss/src/sigmoid_focal_loss_cuda.cu:23-96), with the
+ * fused kernel of bags_ce_fwd in its focal variant:
+ *   loss[0] = sum_n sum_c w[n] * l(z[n,c], t[n]) / norm                          (weights NULL => w = 1)
+ *   dz      = w[n] / norm * g(z[n,c], t[n])                                      (the op's analytic gradient)
+ *   acc[0]  = 100 * #{n : z[n, labels[n]] == max_c z[n, c]} / N                  (optional; as bags_ce_fwd)
+ * targets: int64 [N] in the op's convention, read as int: column t - 1 is positive, every other column negative, and a
+ *          row with t < 0 contributes nothing.  FocalLoss.forward passes F.one_hot(labels, 1231) as the targets and the
+ *          op reads its first N entries: t[n] = (labels[n / 1231] == n % 1231).
+ * With p = sigmoid(z) and log1m = -z [z >= 0] - log(1 + exp(-|z|)):
+ *   positive: l = -alpha (1-p)^gamma log(max(p, FLT_MIN))   g = -alpha (1-p)^gamma (1 - p - gamma p log(max(p, FLT_MIN)))
+ *   negative: l = -(1-alpha) p^gamma log1m                  g = -(1-alpha) p^gamma (gamma (1-p) log1m - p)
+ * norm: the host-known divisor, N * 1231 for FocalLoss (which ignores the caller's avg_factor); no device read.
+ * labels: int64 [N], needed only for acc (a label outside [0, C) never counts as correct).  Without acc the CTAs of the
+ * kernel do not wait for each other.
+ * weights, dz, colsum, clear, workspace: as bags_ce_fwd; dW, db and dX then come from bags_bwd with the single slice
+ * (0, C) and gout = dL/dloss[0].  1 <= C <= 1280.  N == 0: loss = 0, acc = 0. */
+int bags_focal_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias, const int64_t* targets,
+                   const int64_t* labels, const float* weights, float norm, float gamma, float alpha, int N, int K, int C,
+                   int dtype, float* loss, float* acc, void* dz, long long ldd, float* colsum, int colsum_tiles,
+                   void* workspace, size_t workspace_bytes, void* clear, size_t clear_bytes, void* stream);
 
 /* ---- reweight head variant (GSBBoxHeadWith0Reweight, mmdet/models/bbox_heads/gs_bbox_head_with0_reweight.py:57-109):
  * per-(bin, RoI) fp32 weights instead of 0/1 masks, consumed by bags_fwd / bags_group_ce as BAGS_WEIGHTS_F32. ----

@@ -43,6 +43,9 @@ SIGNATURES = {
                          _vp, _sz, _vp]),
     'bags_focal_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _vp, _vp, C.c_float, C.c_float, C.c_float, _i, _i, _i, _i,
                             _vp, _vp, _vp, _ll, _vp, _i, _vp, _sz, _vp, _sz, _vp]),
+    'bags_box_fwd': (_i, [_vp, _ll, _i, _vp, _ll, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _i, _i, _i, _vp, _vp, _vp,
+                          _vp, _vp, _sz, _vp]),
+    'bags_box_bwd': (_i, [_vp, _vp, _vp, _ll, _i, _vp, _ll, _vp, _vp, _i, _i, _i, _vp, _ll, _vp, _vp, _ll, _vp]),
     'bags_reweight': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     'bags_bwd_scratch_bytes': (_sz, [_i, _ll, _i]),
     'bags_bwd': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _ll, _vp, _sz, _i, _i,

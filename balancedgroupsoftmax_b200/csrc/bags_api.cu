@@ -19,6 +19,7 @@
 #include "bags_kernels.cuh"
 #include "bags_allreduce.cuh"
 #include "bags_nms.cuh"
+#include "bags_box.cuh"
 
 using namespace bags;
 
@@ -727,6 +728,105 @@ extern "C" int bags_focal_fwd(const void* x, long long ldx, const void* w, long 
   p.clear_vecs = static_cast<long long>(clear_bytes / 16);
   return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true, true)
                                   : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true, true);
+}
+
+// ----------------------------------------------------------------------------
+// class-specific box regression + SmoothL1 (bbox_head.py:118-128, smooth_l1_loss.py)
+// ----------------------------------------------------------------------------
+static bool aligned(const void* ptr, int bytes) { return (reinterpret_cast<uintptr_t>(ptr) % bytes) == 0; }
+
+// x rows are read 4 elements at a time (8 bytes bf16, 16 bytes fp32), W rows as float4
+static int check_box_operands(const char* who, const void* x, long long ldx, int dtype, const float* w, long long ldw,
+                              int K, int classes) {
+  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "%s: bad dtype %d", who, dtype);
+  BAGS_REQUIRE(K >= 4 && (K % 4) == 0, "%s: K=%d must be a positive multiple of 4", who, K);
+  BAGS_REQUIRE(classes >= 1 && classes <= kBoxMaxClasses, "%s: classes=%d outside [1,%d]", who, classes, kBoxMaxClasses);
+  if (x != nullptr)
+    BAGS_REQUIRE(aligned(x, dtype == BAGS_DTYPE_BF16 ? 8 : 16) && ldx >= K && (ldx % 4) == 0,
+                 "%s: x rows must be %d-byte aligned with ldx >= K and ldx %% 4 == 0 (ldx=%lld)", who,
+                 dtype == BAGS_DTYPE_BF16 ? 8 : 16, ldx);
+  if (w != nullptr)
+    BAGS_REQUIRE(aligned(w, 16) && ldw >= K && (ldw % 4) == 0,
+                 "%s: W rows must be 16-byte aligned with ldw >= K and ldw %% 4 == 0 (ldw=%lld)", who, ldw);
+  return BAGS_OK;
+}
+
+extern "C" int bags_box_fwd(const void* x, long long ldx, int dtype, const float* w, long long ldw, const float* bias,
+                            const int64_t* labels, const float* targets, const float* weights, float beta, float avg,
+                            int N, int K, int classes, float* loss, float* g, float* pred, int32_t* index,
+                            void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  BAGS_REQUIRE(N >= 0, "bags_box_fwd: bad shape N=%d", N);
+  BAGS_REQUIRE(loss && index && workspace && w && (N == 0 || (x && labels && targets && weights && g)),
+               "bags_box_fwd: NULL argument");
+  if (int rc = check_box_operands("bags_box_fwd", x, ldx, dtype, w, ldw, K, classes)) return rc;
+  BAGS_REQUIRE(beta > 0.f && std::isfinite(beta), "bags_box_fwd: beta=%g must be positive and finite",
+               static_cast<double>(beta));
+  BAGS_REQUIRE(N == 0 || (avg > 0.f && std::isfinite(avg)), "bags_box_fwd: avg=%g must be positive and finite",
+               static_cast<double>(avg));
+  BAGS_REQUIRE(aligned(targets, 16) && aligned(weights, 16) && aligned(g, 16) && aligned(pred, 16),
+               "bags_box_fwd: targets, weights, g and pred must be 16-byte aligned [N, 4] arrays");
+  BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "bags_box_fwd: workspace too small (%zu < %zu)",
+               workspace_bytes, bags_workspace_bytes());
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  BoxFwdParams p{};
+  p.x = x; p.ldx = ldx; p.w = w; p.ldw = ldw; p.bias = bias;
+  p.labels = reinterpret_cast<const long long*>(labels);
+  p.targets = targets; p.weights = weights;
+  p.beta = beta; p.avg = N > 0 ? avg : 1.f;
+  p.N = N; p.K = K; p.classes = classes;
+  p.loss = loss; p.g = g; p.pred = pred; p.index = index;
+  p.counter = reinterpret_cast<unsigned int*>(workspace) + kBoxCounterWord;
+  p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  // one warp per RoI; the grid depends only on N and the SM count, so the loss's summation order does too
+  int workers = (N + kBoxThreads / 32 - 1) / (kBoxThreads / 32);
+  if (workers > 4 * di.num_sms) workers = 4 * di.num_sms;
+  if (workers < 1) workers = 1;
+  const dim3 grid(workers + 1);   // + the class-sort CTA
+  if (dtype == BAGS_DTYPE_BF16) bags_box_fwd_kernel<true><<<grid, kBoxThreads, 0, stream>>>(p);
+  else                          bags_box_fwd_kernel<false><<<grid, kBoxThreads, 0, stream>>>(p);
+  BAGS_CUDA(cudaGetLastError());
+  return BAGS_OK;
+}
+
+extern "C" int bags_box_bwd(const float* g, const float* gout, const void* x, long long ldx, int dtype, const float* w,
+                            long long ldw, const int64_t* labels, const int32_t* index, int N, int K, int classes,
+                            float* dW, long long lddw, float* db, void* dX, long long lddx, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  BAGS_REQUIRE(N >= 0, "bags_box_bwd: bad shape N=%d", N);
+  BAGS_REQUIRE(index && (N == 0 || g) && (dW == nullptr || N == 0 || x) && (dX == nullptr || (w && (N == 0 || labels))),
+               "bags_box_bwd: NULL argument");
+  if (int rc = check_box_operands("bags_box_bwd", dW != nullptr ? x : nullptr, ldx, dtype, dX != nullptr ? w : nullptr,
+                                  ldw, K, classes))
+    return rc;
+  BAGS_REQUIRE(aligned(g, 16), "bags_box_bwd: g must be a 16-byte aligned [N, 4] array");
+  if (dW != nullptr)
+    BAGS_REQUIRE(aligned(dW, 16) && lddw >= K && (lddw % 4) == 0,
+                 "bags_box_bwd: dW rows must be 16-byte aligned with lddw >= K and lddw %% 4 == 0 (lddw=%lld)", lddw);
+  if (dX != nullptr)
+    BAGS_REQUIRE(aligned(dX, dtype == BAGS_DTYPE_BF16 ? 8 : 16) && lddx >= K && (lddx % 4) == 0,
+                 "bags_box_bwd: dX rows must be aligned like x with lddx >= K and lddx %% 4 == 0 (lddx=%lld)", lddx);
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  BoxBwdParams p{};
+  p.g = g; p.gout = gout; p.x = x; p.ldx = ldx; p.w = w; p.ldw = ldw;
+  p.labels = reinterpret_cast<const long long*>(labels);
+  p.index = index;
+  p.N = N; p.K = K; p.classes = classes;
+  p.kslices = (K + kBoxSlice - 1) / kBoxSlice;
+  p.dW = dW; p.lddw = lddw; p.db = db; p.dX = dX; p.lddx = lddx;
+  // work list: class units (dW rows, db) first, then RoI units (dX rows)
+  const long long class_units = (dW != nullptr) ? 1LL * classes * p.kslices : (db != nullptr ? classes : 0);
+  const long long roi_units = (dX != nullptr) ? 1LL * N * p.kslices : 0;
+  BAGS_REQUIRE(class_units + roi_units < (1LL << 31), "bags_box_bwd: N=%d K=%d is too large", N, K);
+  p.class_units = static_cast<int>(class_units);
+  if (class_units + roi_units == 0) return BAGS_OK;
+  const dim3 grid(static_cast<unsigned>(class_units + roi_units));
+  if (dtype == BAGS_DTYPE_BF16) bags_box_bwd_kernel<true><<<grid, kBoxBwdThreads, 0, stream>>>(p);
+  else                          bags_box_bwd_kernel<false><<<grid, kBoxBwdThreads, 0, stream>>>(p);
+  BAGS_CUDA(cudaGetLastError());
+  return BAGS_OK;
 }
 
 extern "C" int bags_reweight(const int64_t* labels, const int32_t* label2bin, const uint8_t* wmask,

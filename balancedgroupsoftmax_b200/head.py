@@ -21,7 +21,9 @@ What differs is the execution of the hot path:
   * ``_merge_score`` (gs_bbox_head_with0.py:239-273) is one kernel (``bags_merge_scores``).
 
 The shared FCs, ``fc_reg`` and the SmoothL1 box loss are neighbours of the path and stay
-plain ``nn.Linear`` / PyTorch, exactly as scopes them.
+plain ``nn.Linear`` / PyTorch, exactly as scopes them -- unless the execution key ``fuse_bbox_loss`` is set: then
+``forward`` returns a lazy ``BoxPredHandle`` for the class-specific ``bbox_pred`` and the box loss computes only the
+positive RoIs' four deltas (``ops.SmoothL1BoxFunction``), with no host sync.
 """
 from __future__ import annotations
 
@@ -128,8 +130,42 @@ def delta2bbox(rois, deltas, means=(0, 0, 0, 0), stds=(1, 1, 1, 1), max_shape=No
     return torch.stack([x1, y1, x2, y2], dim=-1).view_as(deltas)
 
 
-# --------------------------------------------------------------------------- lazy cls_score
-class ClsScoreHandle(object):
+# --------------------------------------------------------------------------- lazy projections
+class _LazyHandle(object):
+    """A projection a training ``forward`` records instead of launching, so that ``loss`` can fuse it with its loss.
+    Subclasses give ``shape``, ``device`` and ``tensor()`` (the materialised, autograd-connected output); indexing, any
+    other attribute and any torch function handed a handle see ``tensor()``, so every other consumer keeps working."""
+
+    def size(self, dim=None):
+        return self.shape if dim is None else self.shape[dim]
+
+    def dim(self):
+        return 2
+
+    def __getattr__(self, name):  # argmax, float, detach, ... -> materialise
+        if name.startswith('_'):
+            raise AttributeError(name)
+        return getattr(self.tensor(), name)
+
+    def __getitem__(self, idx):
+        return self.tensor()[idx]
+
+    @classmethod
+    def __torch_function__(cls, func, types, args=(), kwargs=None):
+        """torch.cat([cls_score, ...]), torch.softmax(cls_score, 1), F.cross_entropy(cls_score, ...) ...: any torch
+        function handed a handle sees the materialised tensor (callers written for the reference's plain tensor)."""
+        def unwrap(a):
+            if isinstance(a, _LazyHandle):
+                return a.tensor()
+            if isinstance(a, (list, tuple)):
+                return type(a)(unwrap(v) for v in a)
+            if isinstance(a, dict):
+                return {k: unwrap(v) for k, v in a.items()}
+            return a
+        return func(*unwrap(tuple(args)), **unwrap(kwargs or {}))
+
+
+class ClsScoreHandle(_LazyHandle):
     """What ``GSBBoxHeadWith0.forward`` returns for ``cls_score`` in training mode.
 
     It records the fc_cls input instead of launching the projection, so that ``loss`` can run
@@ -147,12 +183,6 @@ class ClsScoreHandle(object):
     def shape(self):
         return torch.Size((self.x_cls.shape[0], self._head.fc_cls.out_features))
 
-    def size(self, dim=None):
-        return self.shape if dim is None else self.shape[dim]
-
-    def dim(self):
-        return 2
-
     @property
     def device(self):
         return self.x_cls.device
@@ -162,27 +192,32 @@ class ClsScoreHandle(object):
             self._logits = self._head._fc_cls_logits(self.x_cls)
         return self._logits
 
-    def __getattr__(self, name):  # argmax, float, detach, ... -> materialise
-        if name.startswith('_'):
-            raise AttributeError(name)
-        return getattr(self.tensor(), name)
 
-    def __getitem__(self, idx):
-        return self.tensor()[idx]
+class BoxPredHandle(_LazyHandle):
+    """What a head with ``fuse_bbox_loss`` returns for the class-specific ``bbox_pred`` in training mode.
 
-    @classmethod
-    def __torch_function__(cls, func, types, args=(), kwargs=None):
-        """torch.cat([cls_score, ...]), torch.softmax(cls_score, 1), F.cross_entropy(cls_score, ...) ...: any torch
-        function handed a handle sees the materialised logits (callers written for the reference's plain tensor)."""
-        def unwrap(a):
-            if isinstance(a, ClsScoreHandle):
-                return a.tensor()
-            if isinstance(a, (list, tuple)):
-                return type(a)(unwrap(v) for v in a)
-            if isinstance(a, dict):
-                return {k: unwrap(v) for k, v in a.items()}
-            return a
-        return func(*unwrap(tuple(args)), **unwrap(kwargs or {}))
+    It records the fc_reg input, so that ``loss`` can compute only the four box deltas of each positive RoI inside its
+    SmoothL1 loss (``ops.SmoothL1BoxFunction``) instead of the [N, 4 * num_classes] projection.  ``tensor()`` (or any
+    tensor attribute access) materialises that projection through ``_fc_reg``, autograd-connected.
+    """
+
+    def __init__(self, head: 'NativeFcClsHead', x_reg: torch.Tensor):
+        self._head = head
+        self.x_reg = x_reg
+        self._pred = None
+
+    @property
+    def shape(self):
+        return torch.Size((self.x_reg.shape[0], self._head.fc_reg.out_features))
+
+    @property
+    def device(self):
+        return self.x_reg.device
+
+    def tensor(self) -> torch.Tensor:
+        if self._pred is None:
+            self._pred = self._head._fc_reg(self.x_reg)
+        return self._pred
 
 
 def _as_tensor(cls_score):
@@ -484,6 +519,10 @@ class NativeFcClsHead(SharedFCBBoxHead):
         eval_compute_dtype 'fp32' (default) / 'bf16' for the test-time logits
         native_trunk       True (default): shared FCs / fc_reg on this library's wgmma GEMMs
         fuse_loss          True (default): training forward returns a ClsScoreHandle
+        fuse_bbox_loss     False (default).  True: with class-specific regression, the training forward returns a
+                           ``BoxPredHandle`` for ``bbox_pred`` and a 'mean' SmoothL1 ``loss_bbox`` computes only each
+                           positive RoI's four deltas, with fp32 products, and no host sync
+                           (``ops.SmoothL1BoxFunction``).  ``loss_bbox`` then differs from the default route by rounding
     """
 
     def _init_execution(self, cfg):
@@ -496,6 +535,7 @@ class NativeFcClsHead(SharedFCBBoxHead):
         # shared FCs + fc_reg on this library's wgmma GEMMs (bias + ReLU in the epilogue) instead of nn.Linear / cuBLAS
         self.native_trunk = bool(_cfg_get(cfg, 'native_trunk', os.environ.get('BAGS_NATIVE_TRUNK', '1') != '0'))
         self.fuse_loss = bool(_cfg_get(cfg, 'fuse_loss', True))
+        self.fuse_bbox_loss = bool(_cfg_get(cfg, 'fuse_bbox_loss', False))
 
     @staticmethod
     def _cuda_index(device) -> int:
@@ -534,10 +574,37 @@ class NativeFcClsHead(SharedFCBBoxHead):
                                                torch.float32)
         return self.fc_reg(x_reg)
 
+    def _fused_bbox_loss_ok(self, reduction_override) -> bool:
+        """True for a SmoothL1Loss with reduction 'mean' and no other reduction asked (recognised by type name and
+        attributes, so mmdet's own class qualifies too)."""
+        lb = self.loss_bbox
+        return (reduction_override in (None, 'mean') and type(lb).__name__ == 'SmoothL1Loss'
+                and getattr(lb, 'reduction', None) == 'mean'
+                and all(isinstance(getattr(lb, k, None), (int, float)) for k in ('beta', 'loss_weight')))
+
+    def _bbox_loss(self, bbox_pred, labels, bbox_targets, bbox_weights, reduction_override):
+        """An unmaterialised ``BoxPredHandle`` with a 'mean' SmoothL1 takes the fused route (avg_factor =
+        bbox_targets.size(0) from the shape); anything else the reference's op sequence on the materialised deltas."""
+        if isinstance(bbox_pred, BoxPredHandle):
+            if bbox_pred._pred is None and self._fused_bbox_loss_ok(reduction_override):
+                lb = self.loss_bbox
+                loss = ops.SmoothL1BoxFunction.apply(bbox_pred.x_reg, self.fc_reg.weight, self.fc_reg.bias, labels,
+                                                     bbox_targets, bbox_weights, float(lb.beta),
+                                                     float(bbox_targets.size(0)))[0]
+                return loss if lb.loss_weight == 1.0 else loss * lb.loss_weight
+            bbox_pred = bbox_pred.tensor()
+        return super()._bbox_loss(bbox_pred, labels, bbox_targets, bbox_weights, reduction_override)
+
     @auto_fp16()
     def forward(self, x):
         x_cls, x_reg = self._trunk(x)
-        bbox_pred = self._fc_reg(x_reg) if self.with_reg else None
+        bbox_pred = None
+        if self.with_reg:
+            if (self.fuse_bbox_loss and self.training and torch.is_grad_enabled() and not self.reg_class_agnostic
+                    and x_reg.is_cuda):
+                bbox_pred = BoxPredHandle(self, x_reg)
+            else:
+                bbox_pred = self._fc_reg(x_reg)
         if not self.with_cls:
             return None, bbox_pred
         if self.training and self.fuse_loss and torch.is_grad_enabled():
@@ -559,6 +626,7 @@ class GSBBoxHeadWith0(NativeFcClsHead):
                           (``api.GraphCachedHeadLoss``) -- graph-replay host cost with a data-dependent N
         native_trunk      True (default): shared FCs / fc_reg on this library's wgmma GEMMs
         eval_compute_dtype 'fp32' (default) / 'bf16' for the test-time logits
+        fuse_bbox_loss    False (default).  True: fc_reg + the SmoothL1 box loss in one fused op (see NativeFcClsHead)
     """
 
     def __init__(self, num_fcs=2, fc_out_channels=1024, gs_config=None, *args, **kwargs):

@@ -323,6 +323,59 @@ def focal_fwd(x, w, bias, targets, norm: float, gamma: float = 2.0, alpha: float
     return loss, acc, dz, colsum
 
 
+def box_fwd(x, w, bias, labels, targets, weights, beta: float, avg: float, want_pred: bool = False):
+    """bags_box_fwd: the class-specific fc_reg columns of the positive RoIs fused with SmoothL1 'mean' (BBoxHead's box
+    loss).  Returns (loss [1], g [N, 4], index int32 [classes + 1 + N], pred [N, 4] | None); ``g`` and ``index`` feed
+    ``box_bwd``.  ``w``: the fp32 [4 * classes, K] weight (never cast to bf16); ``x``: bf16 or fp32 [N, K];
+    ``avg``: the host normaliser (bbox_targets.size(0))."""
+    _require_cuda(x, w, bias, labels, targets, weights)
+    x, w = _row_major(x), _row_major(w)
+    if w.dtype != torch.float32:
+        raise nat.BagsNativeError('box_fwd: the fc_reg weight must be float32 (got %s)' % w.dtype)
+    if bias is not None:
+        assert bias.dtype == torch.float32
+        bias = bias.contiguous()
+    labels = labels.contiguous()
+    targets = targets.to(torch.float32).contiguous()
+    weights = weights.to(torch.float32).contiguous()
+    N, K = x.shape
+    classes = w.shape[0] // 4
+    assert w.shape[0] == 4 * classes and w.shape[1] == K
+    assert labels.dtype == torch.int64 and labels.numel() == N and targets.shape == (N, 4) and weights.shape == (N, 4)
+    dev = x.device
+    loss = torch.empty((1,), dtype=torch.float32, device=dev)
+    g = torch.empty((N, 4), dtype=torch.float32, device=dev)
+    index = torch.empty((classes + 1 + N,), dtype=torch.int32, device=dev)
+    pred = torch.empty((N, 4), dtype=torch.float32, device=dev) if want_pred else None
+    ws = _workspace(dev)
+    nat.check(nat.lib().bags_box_fwd(
+        x.data_ptr(), x.stride(0), _dtype_code(x.dtype), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(),
+        targets.data_ptr(), weights.data_ptr(), float(beta), float(avg), N, K, classes, loss.data_ptr(), g.data_ptr(),
+        nat.ptr(pred), index.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr(dev)), 'bags_box_fwd')
+    return loss, g, index, pred
+
+
+def box_bwd(g, gout, x, w, labels, index, need_dw: bool = True, need_db: bool = True, need_dx: bool = True):
+    """bags_box_bwd: (dW fp32 [4 * classes, K] | None, db fp32 [4 * classes] | None, dX [N, K] x's dtype | None) from
+    the ``g`` and ``index`` of ``box_fwd``; ``gout``: dL/dloss as a device fp32 [1] tensor, or None for 1."""
+    _require_cuda(g, gout, x, w, labels, index)
+    x, w = _row_major(x), _row_major(w)
+    N, K = x.shape
+    classes = w.shape[0] // 4
+    dev = x.device
+    if gout is not None:
+        gout = _gout(gout)
+        assert gout.numel() == 1
+    dW = torch.empty((4 * classes, K), dtype=torch.float32, device=dev) if need_dw else None
+    db = torch.empty((4 * classes,), dtype=torch.float32, device=dev) if need_db else None
+    dX = torch.empty((N, K), dtype=x.dtype, device=dev) if need_dx else None
+    nat.check(nat.lib().bags_box_bwd(
+        g.data_ptr(), nat.ptr(gout), x.data_ptr(), x.stride(0), _dtype_code(x.dtype), w.data_ptr(), w.stride(0),
+        labels.contiguous().data_ptr(), index.data_ptr(), N, K, classes, nat.ptr(dW), K, nat.ptr(db), nat.ptr(dX), K,
+        _stream_ptr(dev)), 'bags_box_bwd')
+    return dW, db, dX
+
+
 def _single_bin_args(x, w, bias, weights, want_acc, want_dz, want_colsum, clear, acc_out):
     """Operands and outputs shared by ce_fwd and focal_fwd: (x, w, bias, weights, loss, acc, dz, ldd, colsum)."""
     x, w = _row_major(x), _row_major(w)
@@ -806,6 +859,37 @@ class SigmoidFocalFunction(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_loss):
         return _single_bin_bwd(ctx, grad_loss) + (None,) * 8
+
+
+class SmoothL1BoxFunction(torch.autograd.Function):
+    """loss[1] = SmoothL1 'mean' of the class-specific box deltas of the positive RoIs, fc_reg included
+    (BBoxHead._bbox_loss on fc_reg(x) with loss_weight 1) -- only the four columns each positive RoI's loss reads:
+
+    forward : bags_box_fwd (fp32 products from the fp32 master weight, the loss, its gradient g and the class index;
+              no host sync: ``avg`` is a host number, bbox_targets.size(0))
+    backward: bags_box_bwd (dW fully written -- zero rows for absent classes --, db, dX), only what autograd needs."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, labels, targets, weights, beta, avg):
+        _require_cuda(x, weight, bias, labels, targets, weights)
+        xc = x if x.dtype in (torch.bfloat16, torch.float32) else x.float()
+        wc = weight if weight.dtype == torch.float32 else weight.float()
+        b32 = None if bias is None else (bias if bias.dtype == torch.float32 else bias.float())
+        labels = labels.contiguous()
+        loss, g, index, _ = box_fwd(xc, wc, b32, labels, targets, weights, beta, avg)
+        _save_param_dtypes(ctx, x, weight, bias)
+        if any(ctx.needs_input_grad[:3]):
+            ctx.save_for_backward(g, index, _row_major(xc), _row_major(wc), labels)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss):
+        g, index, xc, wc, labels = ctx.saved_tensors
+        dW, db, dX = box_bwd(g, grad_loss, xc, wc, labels, index, need_dw=ctx.needs_input_grad[1],
+                             need_db=ctx.needs_input_grad[2] and ctx.has_bias, need_dx=ctx.needs_input_grad[0])
+        dX, dW, db = _grads_in_param_dtypes(ctx, dX, dW, db)
+        return dX, dW, db, None, None, None, None, None
 
 
 class GroupCEFunction(torch.autograd.Function):

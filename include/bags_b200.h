@@ -22,6 +22,8 @@
  *     + accuracy (reweight_bbox_head.py:36-55)
  *   fc_cls + FocalLoss (sigmoid) + accuracy              bags_focal_fwd
  *     focal_loss.py:29-88, sigmoid_focal_loss_cuda.cu:23-96
+ *   fc_reg + gather + SmoothL1Loss (class-specific)       bags_box_fwd / bags_box_bwd
+ *     bbox_head.py:118-128, smooth_l1_loss.py
  *   autograd backward of the above (dW, db, dX)           bags_bwd
  *     triggered at mmdet/core/utils/dist_utils.py:53
  *   GSBBoxHeadWith0._merge_score                          bags_merge_scores
@@ -166,6 +168,40 @@ int bags_focal_fwd(const void* x, long long ldx, const void* w, long long ldw, c
                    const int64_t* labels, const float* weights, float norm, float gamma, float alpha, int N, int K, int C,
                    int dtype, float* loss, float* acc, void* dz, long long ldd, float* colsum, int colsum_tiles,
                    void* workspace, size_t workspace_bytes, void* clear, size_t clear_bytes, void* stream);
+
+/* Class-specific box regression fused with its SmoothL1 loss -- replaces, for the training loss, fc_reg's
+ * [N, 4 * classes] GEMM (convfc_bbox_head.py:167), the gather bbox_pred.view(N, -1, 4)[pos_inds, labels[pos_inds]] of
+ * BBoxHead.loss (bbox_head.py:118-128, with its nonzero() host sync) and SmoothL1Loss 'mean'
+ * (mmdet/models/losses/smooth_l1_loss.py, losses/utils.py:26-53).  A RoI n is positive when 0 < l = labels[n] < classes;
+ * only its four columns are computed, with fp32 products and accumulation, from the fp32 master W:
+ *   pred[n,j] = sum_k x[n,k] W[4l+j, k] + bias[4l+j]          d = pred[n,j] - targets[n,j]
+ *   sl1(d)    = |d| < beta ? 0.5 d^2 / beta : |d| - 0.5 beta
+ *   loss[0]   = sum_{n positive, j} weights[n,j] sl1(d) / avg  (summed in a fixed order: bit-identical across runs)
+ *   g[n,j]    = weights[n,j] sl1'(d) / avg, sl1' = d / beta for |d| < beta, sign(d) otherwise; 0 for other rows
+ * x: [N, K] (ldx) bf16 or fp32 (dtype), rows 8- (bf16) or 16-byte (fp32) aligned, ldx % 4 == 0, K % 4 == 0.
+ * W: [4 * classes, K] fp32 (ldw % 4 == 0, 16-byte aligned); bias: [4 * classes] fp32 or NULL.  labels: int64 [N]; a
+ * label >= classes (or <= 0) contributes nothing.  targets, weights, g, pred: contiguous fp32 [N, 4], 16-byte aligned.
+ * pred (optional, NULL to skip) holds the four predictions of each positive row and 0 elsewhere.
+ * avg: the host-known normaliser (bbox_targets.size(0)), never read from the device; beta > 0.  1 <= classes <= 8192.
+ * index: int32 [classes + 1 + N], written for bags_box_bwd -- offsets [classes + 1] of each class's positives, then the
+ * positive RoIs sorted by class, ascending RoI id inside a class (a stable counting sort built on the device).
+ * workspace: as bags_fwd (its counter is left at zero).  One launch, no host sync.  N == 0: loss = 0. */
+int bags_box_fwd(const void* x, long long ldx, int dtype, const float* w, long long ldw, const float* bias,
+                 const int64_t* labels, const float* targets, const float* weights, float beta, float avg, int N, int K,
+                 int classes, float* loss, float* g, float* pred, int32_t* index, void* workspace,
+                 size_t workspace_bytes, void* stream);
+
+/* Backward of bags_box_fwd (the autograd backward of the gather + SmoothL1, scatter and fc_reg's dW / db / dX GEMMs),
+ * given its g, index and gout = dL/dloss[0] (device fp32 [1]; NULL => 1):
+ *   dW[4c+j, :] = sum_{n of class c, ascending} gout g[n,j] x[n,:]   fp32 [4 * classes, K] (lddw), FULLY overwritten:
+ *                                                                   rows of classes without a positive are zero
+ *   db[4c+j]    = sum_{n of class c, ascending} gout g[n,j]          fp32 [4 * classes]
+ *   dX[n, :]    = sum_j gout g[n,j] W[4l+j, :]                       x's dtype [N, K] (lddx); 0 for non-positive rows
+ * Each output is optional (NULL to skip).  One launch; no atomics, so every output is bit-identical across runs and
+ * CUDA-graph replays.  Operand rules as bags_box_fwd; dW 16-byte aligned rows, dX aligned like x. */
+int bags_box_bwd(const float* g, const float* gout, const void* x, long long ldx, int dtype, const float* w, long long ldw,
+                 const int64_t* labels, const int32_t* index, int N, int K, int classes, float* dW, long long lddw,
+                 float* db, void* dX, long long lddx, void* stream);
 
 /* ---- reweight head variant (GSBBoxHeadWith0Reweight, mmdet/models/bbox_heads/gs_bbox_head_with0_reweight.py:57-109):
  * per-(bin, RoI) fp32 weights instead of 0/1 masks, consumed by bags_fwd / bags_group_ce as BAGS_WEIGHTS_F32. ----

@@ -491,9 +491,22 @@ extern "C" int bags_fused_eligible(const int32_t* slices_host, int G, int C) {
   return fused_eligible(slices_host, G, C) ? 1 : 0;
 }
 
+static bool aligned(const void* ptr, int bytes) { return (reinterpret_cast<uintptr_t>(ptr) % bytes) == 0; }
+
+// the buffer a forward sets to zero (typically the caller's dW): 16-byte aligned, a multiple of 16 bytes
+static int check_clear(const char* who, const void* clear, size_t clear_bytes) {
+  BAGS_REQUIRE(clear == nullptr || (aligned(clear, 16) && (clear_bytes % 16) == 0),
+               "%s: the buffer to clear must be 16-byte aligned and a multiple of 16 bytes", who);
+  return BAGS_OK;
+}
+
+// The fused kernel's loss variants: the softmax CE with 0/1 byte weights (bags_fwd with the sampler's masks) or with
+// fp32 weights (bags_fwd with BAGS_WEIGHTS_F32, bags_ce_fwd), and the sigmoid focal loss (bags_focal_fwd, fp32 weights).
+enum class FusedLoss { kCeMask, kCeWeighted, kFocal };
+
 template <bool TF32>
-static int launch_fused_fwd(const void* x, long long ldx, const void* w, long long ldw, const FusedFwdParams& p0,
-                            void* dz, long long ldd, int num_sms, cudaStream_t stream, bool wf, bool focal = false) {
+static int launch_fused_fwd(const char* who, FusedLoss loss, const void* x, long long ldx, const void* w, long long ldw,
+                            const FusedFwdParams& p0, void* dz, long long ldd, int num_sms, cudaStream_t stream) {
   using Cfg = FusedCfg<TF32>;
   const int dtype = TF32 ? BAGS_DTYPE_F32 : BAGS_DTYPE_BF16;
   CUtensorMap tx, tw;
@@ -501,8 +514,6 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   if (rc) return rc;
   rc = make_tmap(&tw, w, dtype, p0.K, p0.C, ldw, Cfg::BLOCK_K, Cfg::HALF_N);
   if (rc) return rc;
-  if (dz != nullptr && (reinterpret_cast<uintptr_t>(dz) & 15) != 0)
-    return fail(BAGS_ERR_INVALID, "bags_fwd: dz must be 16-byte aligned");
   // dz [N, C] with row stride ldd: the kernel stages each tile's dz in shared memory and stores it with TMA in boxes
   // of 128 bytes x 128 rows.  A TMA store writes whole 16-byte pieces at the tensor's right edge, so the map spans the
   // columns up to the last 16-byte boundary at or before C; the kernel writes the rest, and the padding columns
@@ -520,7 +531,9 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   p.kblocks = (p.K + Cfg::BLOCK_K - 1) / Cfg::BLOCK_K;
   p.want_dz = dz != nullptr ? 1 : 0;
   p.timing = g_timing;   // rows [0, grid) (grid <= 4 * kFusedMaxGroups); the gradient exchange stamps from row 4096
-  auto kernel = focal ? bags_focal_fwd_kernel<TF32> : wf ? bags_fwd_fused_kernel<TF32, true> : bags_fwd_fused_kernel<TF32, false>;
+  auto kernel = loss == FusedLoss::kFocal       ? bags_focal_fwd_kernel<TF32>
+                : loss == FusedLoss::kCeWeighted ? bags_fwd_fused_kernel<TF32, true>
+                                                 : bags_fwd_fused_kernel<TF32, false>;
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
   // persistent grid of CTA groups, all resident at once: the four CTAs of a group wait for each other's softmax
   // partials.  At 4096 RoIs on 132 SMs this is 32 groups, i.e. 128 CTAs in one wave.
@@ -531,7 +544,7 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   if (groups > row_tiles) groups = row_tiles;
   if (groups > kFusedMaxGroups) groups = kFusedMaxGroups;
   if (groups < 1)
-    return fail(BAGS_ERR_CUDA, "bags_fwd: the fused kernel cannot keep %d CTAs resident (%d SMs, %d CTA(s) per SM)",
+    return fail(BAGS_ERR_CUDA, "%s: the fused kernel cannot keep %d CTAs resident (%d SMs, %d CTA(s) per SM)", who,
                 Cfg::RANKS, num_sms, per_sm);
   const int grid = Cfg::RANKS * groups;
   // PDL INVARIANT (also the sampler's): this kernel reads x, W, bias, labels and label2bin BEFORE its
@@ -548,6 +561,49 @@ static int launch_fused_fwd(const void* x, long long ldx, const void* w, long lo
   return BAGS_OK;
 }
 
+// The fused route of bags_fwd, bags_ce_fwd and bags_focal_fwd: the argument rules they share, the outputs of N == 0,
+// the per-stream workspace and the launch.  The caller has checked its own arguments and filled p's N, C, K and loss
+// fields (bias, labels, l2b, classes, wmask, avg, loss, acc, lse, colsum and the focal parameters); slices_host / G is
+// its bin table.  Every argument check comes before device_info(), so a bad argument is reported without a GPU.
+static int fused_fwd(const char* who, FusedLoss loss, const void* x, long long ldx, const void* w, long long ldw,
+                     int dtype, FusedFwdParams p, const int32_t* slices_host, int G, void* dz, long long ldd,
+                     int colsum_tiles, void* workspace, size_t workspace_bytes, void* clear, size_t clear_bytes,
+                     cudaStream_t stream) {
+  const int N = p.N, C = p.C;
+  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "%s: bad dtype %d", who, dtype);
+  BAGS_REQUIRE(N >= 0 && p.K >= 1, "%s: bad shape N=%d K=%d", who, N, p.K);
+  BAGS_REQUIRE(p.loss && workspace && (N == 0 || (x && w)), "%s: NULL argument", who);
+  BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "%s: workspace too small (%zu < %zu)", who, workspace_bytes,
+               bags_workspace_bytes());
+  BAGS_REQUIRE(p.acc == nullptr || N <= (1 << 24), "%s: N=%d: the accuracy count is exact up to 2^24 rows only", who, N);
+  if (dz != nullptr) BAGS_REQUIRE(ldd >= C && (ldd % 8) == 0, "%s: ldd=%lld must be a multiple of 8 and >= C", who, ldd);
+  BAGS_REQUIRE(dz == nullptr || N == 0 || aligned(dz, 16), "%s: dz must be 16-byte aligned", who);
+  if (p.colsum != nullptr)
+    BAGS_REQUIRE(colsum_tiles == (N + 127) / 128 || (N == 0 && colsum_tiles >= 1),
+                 "%s: colsum must hold ceil(N/128) = %d row tiles of C floats (got %d)", who, (N + 127) / 128,
+                 colsum_tiles);
+  if (int rc = check_clear(who, clear, clear_bytes)) return rc;
+  if (int rc = make_group_table(p.gt, slices_host, G, C)) return rc;
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  if (N == 0) {
+    BAGS_CUDA(cudaMemsetAsync(p.loss, 0, sizeof(float) * G, stream));
+    if (p.acc != nullptr) BAGS_CUDA(cudaMemsetAsync(p.acc, 0, sizeof(float), stream));
+    if (p.colsum != nullptr) BAGS_CUDA(cudaMemsetAsync(p.colsum, 0, sizeof(float) * C * colsum_tiles, stream));
+    if (clear != nullptr) BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, stream));
+    return BAGS_OK;
+  }
+  p.acc_scale = static_cast<float>(100.0 / N);   // accuracy.py: correct * (100.0 / N)
+  p.counter = reinterpret_cast<unsigned int*>(workspace);
+  p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+  p.xch_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes);
+  p.xch = reinterpret_cast<float2*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes + kFusedXchCounterBytes);
+  p.clear = reinterpret_cast<float4*>(clear);
+  p.clear_vecs = static_cast<long long>(clear_bytes / 16);
+  auto launch_for_dtype = dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false> : launch_fused_fwd<true>;
+  return launch_for_dtype(who, loss, x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream);
+}
+
 extern "C" int bags_fwd(const void* x, long long ldx, const void* w, long long ldw,
                         const float* bias, const int64_t* labels, const int32_t* label2bin,
                         const int32_t* slices_host, const void* weights, int weights_dtype, const float* avg,
@@ -558,20 +614,13 @@ extern "C" int bags_fwd(const void* x, long long ldx, const void* w, long long l
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   BAGS_REQUIRE(weights_dtype == BAGS_WEIGHTS_U8 || weights_dtype == BAGS_WEIGHTS_F32,
                "bags_fwd: bad weights dtype %d", weights_dtype);
-  if (clear != nullptr) {
-    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(clear) & 15) == 0 && (clear_bytes % 16) == 0,
-                 "bags_fwd: the buffer to clear must be 16-byte aligned and a multiple of 16 bytes");
-    if (logits != nullptr || N == 0) {   // not the fused kernel: a plain memset
-      BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, stream));
-      clear = nullptr;
-    }
-  }
-  if (colsum != nullptr)
-    BAGS_REQUIRE(colsum_tiles >= 1 && (logits != nullptr || colsum_tiles == (N + 127) / 128 || N == 0),
-                 "bags_fwd: colsum must hold ceil(N/128) = %d row tiles of C floats (got %d)", (N + 127) / 128, colsum_tiles);
   if (logits != nullptr) {
     // caller wants materialised logits: GEMM with fp32 store, then the stand-alone grouped CE (tile 0 holds
-    // the column sums, the other tiles are zero)
+    // the column sums, the other tiles are zero); `clear` is a plain memset
+    BAGS_REQUIRE(colsum == nullptr || colsum_tiles >= 1, "bags_fwd: colsum must hold at least one row tile (got %d)",
+                 colsum_tiles);
+    if (int rc = check_clear("bags_fwd", clear, clear_bytes)) return rc;
+    if (clear != nullptr) BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, stream));
     if (colsum != nullptr && colsum_tiles > 1)
       BAGS_CUDA(cudaMemsetAsync(colsum, 0, sizeof(float) * C * colsum_tiles, stream));
     if (int rc = bags_linear_act_fwd(x, ldx, w, ldw, bias, logits, ldz, N, K, C, dtype, BAGS_DTYPE_F32, 0, stream_))
@@ -583,35 +632,16 @@ extern "C" int bags_fwd(const void* x, long long ldx, const void* w, long long l
   BAGS_REQUIRE(fused_eligible(slices_host, G, C),
                "bags_fwd: logits == NULL requests the fused kernel, but this bin table / C=%d / G=%d is not eligible "
                "(see bags_fused_eligible); pass a logits workspace", C, G);
-  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "bags_fwd: bad dtype %d", dtype);
-  BAGS_REQUIRE(label2bin && loss && workspace && (N == 0 || (x && w && labels)), "bags_fwd: NULL argument");
-  BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "bags_fwd: workspace too small");
-  BAGS_REQUIRE(N >= 0 && K >= 1, "bags_fwd: bad shape");
-  if (dz != nullptr) BAGS_REQUIRE(ldd >= C && (ldd % 8) == 0, "bags_fwd: ldd=%lld must be a multiple of 8 and >= C", ldd);
-  GroupTable gt;
-  if (int rc = make_group_table(gt, slices_host, G, C)) return rc;
-  DeviceInfo di;
-  if (int rc = device_info(di)) return rc;
-  if (N == 0) {
-    BAGS_CUDA(cudaMemsetAsync(loss, 0, sizeof(float) * G, stream));
-    if (colsum != nullptr) BAGS_CUDA(cudaMemsetAsync(colsum, 0, sizeof(float) * C * colsum_tiles, stream));
-    return BAGS_OK;
-  }
-  if (bias != nullptr) BAGS_REQUIRE((reinterpret_cast<uintptr_t>(bias) & 15) == 0, "bags_fwd: bias must be 16-byte aligned");
+  BAGS_REQUIRE(label2bin && (N == 0 || labels), "bags_fwd: NULL argument");
+  BAGS_REQUIRE(N == 0 || bias == nullptr || aligned(bias, 16), "bags_fwd: bias must be 16-byte aligned");
   FusedFwdParams p{};
-  p.N = N; p.C = C; p.K = K; p.gt = gt; p.bias = bias;
+  p.N = N; p.C = C; p.K = K; p.bias = bias;
   p.labels = reinterpret_cast<const long long*>(labels);
   p.l2b = label2bin; p.classes = classes; p.wmask = static_cast<const uint8_t*>(weights); p.avg = avg;
   p.loss = loss; p.lse = lse; p.colsum = colsum;
-  p.counter = reinterpret_cast<unsigned int*>(workspace);
-  p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  p.xch_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes);
-  p.xch = reinterpret_cast<float2*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes + kFusedXchCounterBytes);
-  p.clear = reinterpret_cast<float4*>(clear);
-  p.clear_vecs = static_cast<long long>(clear_bytes / 16);
-  const bool wf = weights_dtype == BAGS_WEIGHTS_F32;
-  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, wf)
-                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, wf);
+  return fused_fwd("bags_fwd", weights_dtype == BAGS_WEIGHTS_F32 ? FusedLoss::kCeWeighted : FusedLoss::kCeMask, x, ldx,
+                   w, ldw, dtype, p, slices_host, G, dz, ldd, colsum_tiles, workspace, workspace_bytes, clear,
+                   clear_bytes, stream);
 }
 
 // fc_cls + plain softmax CE over all C logits (ReweightBBoxHead, BBoxHead.loss): the fused kernel with one bin (0, C),
@@ -623,118 +653,49 @@ extern "C" int bags_ce_fwd(const void* x, long long ldx, const void* w, long lon
                            int dtype, float* loss, float* acc, void* dz, long long ldd, float* colsum,
                            int colsum_tiles, void* workspace, size_t workspace_bytes, void* clear, size_t clear_bytes,
                            void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   constexpr int kMaxC = FusedCfg<false>::RANKS * FusedCfg<false>::BLOCK_N;
-  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "bags_ce_fwd: bad dtype %d", dtype);
-  BAGS_REQUIRE(N >= 0 && K >= 1 && C >= 1 && C <= kMaxC, "bags_ce_fwd: bad shape N=%d K=%d C=%d (1 <= C <= %d)", N, K,
-               C, kMaxC);
-  BAGS_REQUIRE(loss && workspace && (N == 0 || (x && w && labels)), "bags_ce_fwd: NULL argument");
-  BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "bags_ce_fwd: workspace too small (%zu < %zu)",
-               workspace_bytes, bags_workspace_bytes());
-  BAGS_REQUIRE(acc == nullptr || N <= (1 << 24),
-               "bags_ce_fwd: N=%d: the accuracy count is exact up to 2^24 rows only", N);
-  if (dz != nullptr) BAGS_REQUIRE(ldd >= C && (ldd % 8) == 0, "bags_ce_fwd: ldd=%lld must be a multiple of 8 and >= C", ldd);
-  if (colsum != nullptr)
-    BAGS_REQUIRE(colsum_tiles == (N + 127) / 128 || (N == 0 && colsum_tiles >= 1),
-                 "bags_ce_fwd: colsum must hold ceil(N/128) = %d row tiles of C floats (got %d)", (N + 127) / 128,
-                 colsum_tiles);
-  if (clear != nullptr)
-    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(clear) & 15) == 0 && (clear_bytes % 16) == 0,
-                 "bags_ce_fwd: the buffer to clear must be 16-byte aligned and a multiple of 16 bytes");
-  const int32_t slices[2] = {0, C};
-  GroupTable gt;
-  if (int rc = make_group_table(gt, slices, 1, C)) return rc;
-  DeviceInfo di;
-  if (int rc = device_info(di)) return rc;
-  if (N == 0) {
-    BAGS_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), stream));
-    if (acc != nullptr) BAGS_CUDA(cudaMemsetAsync(acc, 0, sizeof(float), stream));
-    if (colsum != nullptr) BAGS_CUDA(cudaMemsetAsync(colsum, 0, sizeof(float) * C * colsum_tiles, stream));
-    if (clear != nullptr) BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, stream));
-    return BAGS_OK;
-  }
+  BAGS_REQUIRE(C >= 1 && C <= kMaxC, "bags_ce_fwd: bad shape C=%d (1 <= C <= %d)", C, kMaxC);
+  BAGS_REQUIRE(N == 0 || labels, "bags_ce_fwd: NULL argument");
   FusedFwdParams p{};
-  p.N = N; p.C = C; p.K = K; p.gt = gt; p.bias = bias;
+  p.N = N; p.C = C; p.K = K; p.bias = bias;
   p.labels = reinterpret_cast<const long long*>(labels);
   p.l2b = nullptr; p.classes = C;
   p.wmask = reinterpret_cast<const uint8_t*>(weights); p.avg = avg;
-  p.loss = loss; p.acc = acc; p.acc_scale = static_cast<float>(100.0 / N);   // accuracy.py: correct * (100.0 / N)
-  p.lse = nullptr; p.colsum = colsum;
-  p.counter = reinterpret_cast<unsigned int*>(workspace);
-  p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  p.xch_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes);
-  p.xch = reinterpret_cast<float2*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes + kFusedXchCounterBytes);
-  p.clear = reinterpret_cast<float4*>(clear);
-  p.clear_vecs = static_cast<long long>(clear_bytes / 16);
-  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true)
-                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true);
+  p.loss = loss; p.acc = acc; p.colsum = colsum;
+  const int32_t slices[2] = {0, C};
+  return fused_fwd("bags_ce_fwd", FusedLoss::kCeWeighted, x, ldx, w, ldw, dtype, p, slices, 1, dz, ldd, colsum_tiles,
+                   workspace, workspace_bytes, clear, clear_bytes, static_cast<cudaStream_t>(stream_));
 }
 
 // fc_cls + the sigmoid focal loss over all C logits (FocalLoss, focal_loss.py:29-88 with sigmoid_focal_loss_cuda.cu:23-96):
-// the fused kernel's focal variant with one bin (0, C) and fp32 per-RoI weights.  Argument rules as bags_ce_fwd.
+// the fused kernel's focal variant with one bin (0, C) and fp32 per-RoI weights.  Argument rules as bags_ce_fwd, plus
+// non-NULL targets, the labels when acc is asked for, and a finite norm > 0.
 extern "C" int bags_focal_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
                               const int64_t* targets, const int64_t* labels, const float* weights, float norm,
                               float gamma, float alpha, int N, int K, int C, int dtype, float* loss, float* acc,
                               void* dz, long long ldd, float* colsum, int colsum_tiles, void* workspace,
                               size_t workspace_bytes, void* clear, size_t clear_bytes, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   constexpr int kMaxC = FusedCfg<false>::RANKS * FusedCfg<false>::BLOCK_N;
-  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "bags_focal_fwd: bad dtype %d", dtype);
-  BAGS_REQUIRE(N >= 0 && K >= 1 && C >= 1 && C <= kMaxC, "bags_focal_fwd: bad shape N=%d K=%d C=%d (1 <= C <= %d)", N,
-               K, C, kMaxC);
-  BAGS_REQUIRE(loss && workspace && (N == 0 || (x && w && targets)) && (acc == nullptr || N == 0 || labels),
-               "bags_focal_fwd: NULL argument");
+  BAGS_REQUIRE(C >= 1 && C <= kMaxC, "bags_focal_fwd: bad shape C=%d (1 <= C <= %d)", C, kMaxC);
+  BAGS_REQUIRE((N == 0 || targets) && (acc == nullptr || N == 0 || labels), "bags_focal_fwd: NULL argument");
   BAGS_REQUIRE(norm > 0.f && std::isfinite(norm), "bags_focal_fwd: norm=%g must be positive and finite",
                static_cast<double>(norm));
-  BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "bags_focal_fwd: workspace too small (%zu < %zu)",
-               workspace_bytes, bags_workspace_bytes());
-  BAGS_REQUIRE(acc == nullptr || N <= (1 << 24),
-               "bags_focal_fwd: N=%d: the accuracy count is exact up to 2^24 rows only", N);
-  if (dz != nullptr)
-    BAGS_REQUIRE(ldd >= C && (ldd % 8) == 0, "bags_focal_fwd: ldd=%lld must be a multiple of 8 and >= C", ldd);
-  if (colsum != nullptr)
-    BAGS_REQUIRE(colsum_tiles == (N + 127) / 128 || (N == 0 && colsum_tiles >= 1),
-                 "bags_focal_fwd: colsum must hold ceil(N/128) = %d row tiles of C floats (got %d)", (N + 127) / 128,
-                 colsum_tiles);
-  if (clear != nullptr)
-    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(clear) & 15) == 0 && (clear_bytes % 16) == 0,
-                 "bags_focal_fwd: the buffer to clear must be 16-byte aligned and a multiple of 16 bytes");
-  const int32_t slices[2] = {0, C};
-  GroupTable gt;
-  if (int rc = make_group_table(gt, slices, 1, C)) return rc;
-  DeviceInfo di;
-  if (int rc = device_info(di)) return rc;
-  if (N == 0) {
-    BAGS_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), stream));
-    if (acc != nullptr) BAGS_CUDA(cudaMemsetAsync(acc, 0, sizeof(float), stream));
-    if (colsum != nullptr) BAGS_CUDA(cudaMemsetAsync(colsum, 0, sizeof(float) * C * colsum_tiles, stream));
-    if (clear != nullptr) BAGS_CUDA(cudaMemsetAsync(clear, 0, clear_bytes, stream));
-    return BAGS_OK;
-  }
   FusedFwdParams p{};
-  p.N = N; p.C = C; p.K = K; p.gt = gt; p.bias = bias;
+  p.N = N; p.C = C; p.K = K; p.bias = bias;
   p.labels = reinterpret_cast<const long long*>(labels);
   p.targets = reinterpret_cast<const long long*>(targets);
   p.l2b = nullptr; p.classes = C;
   p.wmask = reinterpret_cast<const uint8_t*>(weights);
   p.norm = norm; p.gamma = gamma; p.alpha = alpha;
-  p.loss = loss; p.acc = acc; p.acc_scale = static_cast<float>(100.0 / N);   // accuracy.py: correct * (100.0 / N)
-  p.lse = nullptr; p.colsum = colsum;
-  p.counter = reinterpret_cast<unsigned int*>(workspace);
-  p.part = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
-  p.xch_counter = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes);
-  p.xch = reinterpret_cast<float2*>(reinterpret_cast<char*>(workspace) + kLossWorkspaceBytes + kFusedXchCounterBytes);
-  p.clear = reinterpret_cast<float4*>(clear);
-  p.clear_vecs = static_cast<long long>(clear_bytes / 16);
-  return dtype == BAGS_DTYPE_BF16 ? launch_fused_fwd<false>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true, true)
-                                  : launch_fused_fwd<true>(x, ldx, w, ldw, p, dz, ldd, di.num_sms, stream, true, true);
+  p.loss = loss; p.acc = acc; p.colsum = colsum;
+  const int32_t slices[2] = {0, C};
+  return fused_fwd("bags_focal_fwd", FusedLoss::kFocal, x, ldx, w, ldw, dtype, p, slices, 1, dz, ldd, colsum_tiles,
+                   workspace, workspace_bytes, clear, clear_bytes, static_cast<cudaStream_t>(stream_));
 }
 
 // ----------------------------------------------------------------------------
 // class-specific box regression + SmoothL1 (bbox_head.py:118-128, smooth_l1_loss.py)
 // ----------------------------------------------------------------------------
-static bool aligned(const void* ptr, int bytes) { return (reinterpret_cast<uintptr_t>(ptr) % bytes) == 0; }
-
 // x rows are read 4 elements at a time (8 bytes bf16, 16 bytes fp32), W rows as float4
 static int check_box_operands(const char* who, const void* x, long long ldx, int dtype, const float* w, long long ldw,
                               int K, int classes) {

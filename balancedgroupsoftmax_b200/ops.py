@@ -15,7 +15,6 @@ raises if the inputs are not CUDA tensors or the extension is missing.
 from __future__ import annotations
 
 import ctypes as C
-import os
 from dataclasses import dataclass
 from typing import Dict, Optional, Tuple
 
@@ -220,6 +219,53 @@ def fused_eligible(dt: DeviceTables) -> bool:
     return bool(nat.lib().bags_fused_eligible(dt.slices_host, dt.G, dt.num_logits))
 
 
+def _fused_outputs(x, w, bias, G: int, want_acc: bool, want_dz: bool, want_colsum: bool,
+                   clear: Optional[torch.Tensor], acc_out: Optional[torch.Tensor] = None):
+    """Operands and outputs shared by bags_fwd, bags_ce_fwd and bags_focal_fwd: row-major x and w of one dtype, the
+    fp32 bias, loss [G], acc [1] (``acc_out`` when given), dz [N, pad_cols(C)] in the operand dtype, the per-row-tile
+    colsum [ceil(N/128), C] and the buffer to ``clear``.  Returns (x, w, bias, loss, acc, dz, colsum, tail), ``tail``
+    being the calls' common last arguments (dz, ldd, colsum, colsum_tiles, workspace, workspace_bytes, clear,
+    clear_bytes, stream)."""
+    x, w = _row_major(x), _row_major(w)
+    if x.dtype != w.dtype:
+        raise nat.BagsNativeError('x (%s) and w (%s) must share a dtype' % (x.dtype, w.dtype))
+    N = x.shape[0]
+    Cc = w.shape[0]
+    dev = x.device
+    if bias is not None:
+        assert bias.dtype == torch.float32
+        bias = bias.contiguous()
+    loss = torch.empty((G,), dtype=torch.float32, device=dev)
+    acc = None
+    if want_acc:
+        acc = acc_out if acc_out is not None else torch.empty((1,), dtype=torch.float32, device=dev)
+        assert acc.dtype == torch.float32 and acc.numel() == 1
+    dz = colsum = None
+    ldd = 0
+    if want_dz:
+        ldd = pad_cols(Cc)
+        dz = torch.empty((N, ldd), dtype=x.dtype, device=dev)
+        if want_colsum:   # per-row-tile partials; by default the backward recomputes them from dz instead
+            colsum = torch.empty((max((N + 127) // 128, 1), Cc), dtype=torch.float32, device=dev)
+    if clear is not None:
+        # ``clear``: a contiguous buffer (the caller's dW) that the forward zeroes, on the fused route while its CTAs
+        # exchange their softmax partials
+        assert clear.is_contiguous() and (clear.numel() * clear.element_size()) % 16 == 0
+    ws = _workspace(dev)
+    tail = (nat.ptr(dz), ldd, nat.ptr(colsum), colsum.shape[0] if colsum is not None else 0, ws.data_ptr(), ws.numel(),
+            nat.ptr(clear), clear.numel() * clear.element_size() if clear is not None else 0, _stream_ptr(dev))
+    return x, w, bias, loss, acc, dz, colsum, tail
+
+
+def _roi_weights(weights: Optional[torch.Tensor], N: int) -> Optional[torch.Tensor]:
+    """fp32 [N] per-RoI weights of the single-bin losses (None: 1)."""
+    if weights is None:
+        return None
+    weights = weights.to(torch.float32).contiguous()
+    assert weights.numel() == N
+    return weights
+
+
 def fused_fwd(x, w, bias, labels, dt: DeviceTables, wmask, avg, logits: Optional[torch.Tensor] = None,
               want_dz: bool = True, want_lse: bool = False, materialize: Optional[bool] = None,
               want_colsum: bool = False, clear: Optional[torch.Tensor] = None):
@@ -231,41 +277,23 @@ def fused_fwd(x, w, bias, labels, dt: DeviceTables, wmask, avg, logits: Optional
     (fused_bwd recomputes them from dz when they are not supplied).
     """
     _require_cuda(x, w, bias, labels, wmask, avg)
-    x, w = _row_major(x), _row_major(w)
-    if x.dtype != w.dtype:
-        raise nat.BagsNativeError('x (%s) and w (%s) must share a dtype' % (x.dtype, w.dtype))
+    x, w, bias, loss, _, dz, colsum, tail = _fused_outputs(x, w, bias, dt.G, False, want_dz, want_colsum, clear)
     labels = labels.contiguous()
     N, K = x.shape
     Cc = w.shape[0]
-    dev = x.device
     if materialize is None:
         materialize = (logits is not None) or not fused_eligible(dt)
     if materialize and logits is None:
-        logits = torch.empty((N, Cc), dtype=torch.float32, device=dev)
+        logits = torch.empty((N, Cc), dtype=torch.float32, device=x.device)
     if not materialize:
         logits = None
-    loss = torch.empty((dt.G,), dtype=torch.float32, device=dev)
-    lse = torch.empty((N, dt.G), dtype=torch.float32, device=dev) if want_lse else None
-    dz = colsum = None
-    ldd = 0
-    if want_dz:
-        ldd = pad_cols(Cc)
-        dz = torch.empty((N, ldd), dtype=x.dtype, device=dev)
-        if want_colsum:   # per-row-tile partials; by default the backward recomputes them from dz instead
-            colsum = torch.empty((max((N + 127) // 128, 1), Cc), dtype=torch.float32, device=dev)
-    ws = _workspace(dev)
+    lse = torch.empty((N, dt.G), dtype=torch.float32, device=x.device) if want_lse else None
     wmask, wcode = _weights_arg(wmask)
-    if clear is not None:
-        # ``clear``: a contiguous buffer (the caller's dW) that the forward zeroes, on the fused route while its CTAs
-        # exchange their softmax partials
-        assert clear.is_contiguous() and (clear.numel() * clear.element_size()) % 16 == 0
     nat.check(nat.lib().bags_fwd(
         x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(),
         dt.label2bin.data_ptr(), dt.slices_host, nat.ptr(wmask), wcode, nat.ptr(avg), N, K, Cc, dt.G, dt.num_classes,
         _dtype_code(x.dtype), nat.ptr(logits), logits.stride(0) if logits is not None else 0, loss.data_ptr(),
-        nat.ptr(lse), nat.ptr(dz), ldd, nat.ptr(colsum), colsum.shape[0] if colsum is not None else 0, ws.data_ptr(),
-        ws.numel(), nat.ptr(clear), clear.numel() * clear.element_size() if clear is not None else 0,
-        _stream_ptr(dev)), 'bags_fwd')
+        nat.ptr(lse), *tail), 'bags_fwd')
     return loss, logits, lse, dz, colsum
 
 
@@ -278,18 +306,16 @@ def ce_fwd(x, w, bias, labels, weights=None, avg=None, want_acc: bool = False, w
     ``want_acc``: also the top-1 accuracy in percent (ties with the row maximum count as correct), written into
     ``acc_out`` when given.  ``clear``: as in ``fused_fwd``."""
     _require_cuda(x, w, bias, labels, weights, avg, clear, acc_out)
-    x, w, bias, weights, loss, acc, dz, ldd, colsum = _single_bin_args(x, w, bias, weights, want_acc, want_dz,
-                                                                       want_colsum, clear, acc_out)
+    x, w, bias, loss, acc, dz, colsum, tail = _fused_outputs(x, w, bias, 1, want_acc, want_dz, want_colsum, clear,
+                                                             acc_out)
     labels = labels.contiguous()
     N, K = x.shape
+    weights = _roi_weights(weights, N)
     if avg is not None:
         assert avg.dtype == torch.float32 and avg.numel() >= 1
-    ws = _workspace(x.device)
     nat.check(nat.lib().bags_ce_fwd(
         x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(), nat.ptr(weights),
-        nat.ptr(avg), N, K, w.shape[0], _dtype_code(x.dtype), loss.data_ptr(), nat.ptr(acc), nat.ptr(dz), ldd,
-        nat.ptr(colsum), colsum.shape[0] if colsum is not None else 0, ws.data_ptr(), ws.numel(), nat.ptr(clear),
-        clear.numel() * clear.element_size() if clear is not None else 0, _stream_ptr(x.device)), 'bags_ce_fwd')
+        nat.ptr(avg), N, K, w.shape[0], _dtype_code(x.dtype), loss.data_ptr(), nat.ptr(acc), *tail), 'bags_ce_fwd')
     return loss, acc, dz, colsum
 
 
@@ -303,23 +329,21 @@ def focal_fwd(x, w, bias, targets, norm: float, gamma: float = 2.0, alpha: float
     ``losses.focal_targets``); ``norm``: the host-known divisor (N * 1231 for FocalLoss); ``labels``: int64 [N], for the
     accuracy only.  ``weights``, ``want_acc``, ``clear``, ``acc_out``: as in ``ce_fwd``."""
     _require_cuda(x, w, bias, targets, labels, weights, clear, acc_out)
-    x, w, bias, weights, loss, acc, dz, ldd, colsum = _single_bin_args(x, w, bias, weights, want_acc, want_dz,
-                                                                       want_colsum, clear, acc_out)
+    x, w, bias, loss, acc, dz, colsum, tail = _fused_outputs(x, w, bias, 1, want_acc, want_dz, want_colsum, clear,
+                                                             acc_out)
+    N, K = x.shape
+    weights = _roi_weights(weights, N)
     targets = targets.contiguous()
-    assert targets.dtype == torch.int64 and targets.numel() == x.shape[0]
+    assert targets.dtype == torch.int64 and targets.numel() == N
     if want_acc:
         if labels is None:
             raise nat.BagsNativeError('focal_fwd: the accuracy needs the labels')
         labels = labels.contiguous()
-        assert labels.dtype == torch.int64 and labels.numel() == x.shape[0]
-    N, K = x.shape
-    ws = _workspace(x.device)
+        assert labels.dtype == torch.int64 and labels.numel() == N
     nat.check(nat.lib().bags_focal_fwd(
         x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(bias), targets.data_ptr(),
         nat.ptr(labels) if want_acc else None, nat.ptr(weights), float(norm), float(gamma), float(alpha), N, K,
-        w.shape[0], _dtype_code(x.dtype), loss.data_ptr(), nat.ptr(acc), nat.ptr(dz), ldd, nat.ptr(colsum),
-        colsum.shape[0] if colsum is not None else 0, ws.data_ptr(), ws.numel(), nat.ptr(clear),
-        clear.numel() * clear.element_size() if clear is not None else 0, _stream_ptr(x.device)), 'bags_focal_fwd')
+        w.shape[0], _dtype_code(x.dtype), loss.data_ptr(), nat.ptr(acc), *tail), 'bags_focal_fwd')
     return loss, acc, dz, colsum
 
 
@@ -374,37 +398,6 @@ def box_bwd(g, gout, x, w, labels, index, need_dw: bool = True, need_db: bool = 
         labels.contiguous().data_ptr(), index.data_ptr(), N, K, classes, nat.ptr(dW), K, nat.ptr(db), nat.ptr(dX), K,
         _stream_ptr(dev)), 'bags_box_bwd')
     return dW, db, dX
-
-
-def _single_bin_args(x, w, bias, weights, want_acc, want_dz, want_colsum, clear, acc_out):
-    """Operands and outputs shared by ce_fwd and focal_fwd: (x, w, bias, weights, loss, acc, dz, ldd, colsum)."""
-    x, w = _row_major(x), _row_major(w)
-    if x.dtype != w.dtype:
-        raise nat.BagsNativeError('x (%s) and w (%s) must share a dtype' % (x.dtype, w.dtype))
-    N = x.shape[0]
-    Cc = w.shape[0]
-    dev = x.device
-    if bias is not None:
-        assert bias.dtype == torch.float32
-        bias = bias.contiguous()
-    if weights is not None:
-        weights = weights.to(torch.float32).contiguous()
-        assert weights.numel() == N
-    loss = torch.empty((1,), dtype=torch.float32, device=dev)
-    acc = None
-    if want_acc:
-        acc = acc_out if acc_out is not None else torch.empty((1,), dtype=torch.float32, device=dev)
-        assert acc.dtype == torch.float32 and acc.numel() == 1
-    dz = colsum = None
-    ldd = 0
-    if want_dz:
-        ldd = pad_cols(Cc)
-        dz = torch.empty((N, ldd), dtype=x.dtype, device=dev)
-        if want_colsum:
-            colsum = torch.empty((max((N + 127) // 128, 1), Cc), dtype=torch.float32, device=dev)
-    if clear is not None:
-        assert clear.is_contiguous() and (clear.numel() * clear.element_size()) % 16 == 0
-    return x, w, bias, weights, loss, acc, dz, ldd, colsum
 
 
 _scratch_cache: Dict[Tuple, torch.Tensor] = {}
@@ -657,14 +650,6 @@ class LinearActFunction(torch.autograd.Function):
 
 
 # --------------------------------------------------------------------------- autograd
-# where the backward's preparation work runs: 1 = dW is zeroed by the fused forward kernel (idle producer warps)
-PREP_IN_FORWARD = os.environ.get('BAGS_PREP_IN_FORWARD', '1') != '0'
-# 1 = the bias-gradient column sums come from the forward's epilogue as well (otherwise a job of the backward's
-# preparation kernel).  Off by default on one GPU; with a grad_bucket (data-parallel schedule)
-# it is always on: the dW + db launch -- on the critical path before the exchange -- then has nothing to prepare.
-FWD_COLSUM = os.environ.get('BAGS_FWD_COLSUM', '0') == '1'
-
-
 def _fc_cls_operands(x, weight, bias, compute_dtype):
     """(xc, wc, b32): the fc_cls operands the fused forward reads.  bf16: fp32 masters are cast (the weight only when
     it changed); float32: fp32 operands, TF32 products.  The bias is always fp32."""
@@ -682,6 +667,40 @@ def _fc_cls_operands(x, weight, bias, compute_dtype):
     else:
         b32 = bias.float().contiguous()
     return xc, wc, b32
+
+
+def _fused_loss_prologue(ctx, x, weight, bias, compute_dtype, clear_dw: bool = True):
+    """Forward prologue of the fused-loss Functions: (xc, wc, b32, dW).  xc, wc, b32: the fc_cls operands
+    (``_fc_cls_operands``); dW: when the weight needs a gradient and ``clear_dw``, its fp32 [C, K] buffer for the fused
+    forward to zero (its ``clear``), so that the backward's split-K red.add needs no zeroing job; None otherwise."""
+    xc, wc, b32 = _fc_cls_operands(x, weight, bias, compute_dtype)
+    _save_param_dtypes(ctx, x, weight, bias)
+    dW = None
+    if ctx.needs_input_grad[1] and clear_dw:
+        dW = torch.empty((wc.shape[0], wc.shape[1]), dtype=torch.float32, device=xc.device)
+    return xc, wc, b32, dW
+
+
+def _fused_loss_saved(ctx, xc, wc, dz, dW) -> None:
+    """What ``_fused_loss_bwd`` reads: the dW the forward zeroed, and dz~ with the operands when a gradient is needed."""
+    ctx.dW = dW
+    if any(ctx.needs_input_grad[:3]):
+        ctx.save_for_backward(xc, wc, dz)
+
+
+def _fused_loss_bwd(ctx, grad_loss, dt: Optional[DeviceTables] = None, colsum: Optional[torch.Tensor] = None):
+    """(dX, dW, db) in the parameters' dtypes from the dz~ a fused-loss forward saved: one bags_bwd over the bin table
+    ``dt`` (None: the single slice (0, C)), with the forward's column-sum partials ``colsum`` when it took them; dX only
+    when x needs a gradient, dW zeroed by the forward kernel when ``ctx.dW`` is set."""
+    xc, wc, dz = ctx.saved_tensors
+    need_dx, need_dw, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+    dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
+    if dt is None:
+        dt = _single_slice_tables(wc.shape[0], xc.device)
+    dW, db, dX = fused_bwd(dz, xc, wc, _gout(grad_loss), dt, colsum, need_dw=need_dw,
+                           need_db=(need_db and ctx.has_bias), need_dx=need_dx,
+                           dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None)
+    return _grads_in_param_dtypes(ctx, dX, dW, db)
 
 
 def _save_param_dtypes(ctx, x, weight, bias) -> None:
@@ -730,57 +749,47 @@ class GroupSoftmaxFunction(torch.autograd.Function):
         the returned weight / bias gradients ARE the bucket views, holding the mean over ranks."""
         _require_cuda(x, weight, bias, labels)
         # (autograd does not record inside Function.forward: the inputs are used as they are, no detach() round trips)
-        xc, wc, b32 = _fc_cls_operands(x, weight, bias, compute_dtype)
-        need_grad = any(ctx.needs_input_grad[:3])
-        # dW is allocated here and zeroed by the forward kernel (its split-K red.add in the
-        # backward then needs no zeroing job); BAGS_FWD_COLSUM=1 also takes the bias-gradient partials from the forward
-        dW = None
-        ctx.grad_bucket = grad_bucket if (grad_bucket is not None and need_grad and ctx.needs_input_grad[1]) else None
+        ctx.grad_bucket = grad_bucket if (grad_bucket is not None and ctx.needs_input_grad[1]) else None
+        xc, wc, b32, dW = _fused_loss_prologue(ctx, x, weight, bias, compute_dtype,
+                                               clear_dw=ctx.grad_bucket is None and logits_out is None)
         if ctx.grad_bucket is not None:
+            # the forward zeroes the bucket's dW as well, and takes the bias-gradient partials: the dW + db launch -- on
+            # the critical path before the exchange -- then has nothing to prepare
             dW = grad_bucket.views[0]
             assert dW.dtype == torch.float32 and tuple(dW.shape) == (wc.shape[0], wc.shape[1]) and dW.is_contiguous()
-            if logits_out is not None or not PREP_IN_FORWARD:
+            if logits_out is not None:
                 dW.zero_()
-        elif need_grad and ctx.needs_input_grad[1] and logits_out is None and PREP_IN_FORWARD:
-            dW = torch.empty((wc.shape[0], wc.shape[1]), dtype=torch.float32, device=xc.device)
         loss, _, _, dz, colsum = fused_fwd(xc, wc, b32, labels, dt, wmask, avg, logits=logits_out,
-                                           want_dz=need_grad, clear=dW,
-                                           want_colsum=(dW is not None and bias is not None and
-                                                        (FWD_COLSUM or ctx.grad_bucket is not None)))
-        ctx.dW = dW
-        ctx.colsum = colsum if dW is not None else None
+                                           want_dz=any(ctx.needs_input_grad[:3]), clear=dW,
+                                           want_colsum=ctx.grad_bucket is not None and bias is not None)
         ctx.dt = dt
-        _save_param_dtypes(ctx, x, weight, bias)
-        if need_grad:
-            ctx.save_for_backward(xc, wc, dz)
+        ctx.colsum = colsum
+        _fused_loss_saved(ctx, xc, wc, dz, dW)
         return loss
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_loss):
+        bucket = ctx.grad_bucket
+        if bucket is None or not ctx.needs_input_grad[1]:
+            return _fused_loss_bwd(ctx, grad_loss, ctx.dt, ctx.colsum) + (None,) * 7
         xc, wc, dz = ctx.saved_tensors
-        need_dx, need_dw, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        need_dx, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[2]
         gout = _gout(grad_loss)
         dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
-        bucket = ctx.grad_bucket
-        if bucket is not None and need_dw:
-            # dW + db first, straight into the exchange bucket; the exchange starts when they are complete and runs
-            # while the dX contraction does
-            if dW0 is None:
-                bucket.views[0].zero_()
-            db_view = bucket.views[1] if (need_db and ctx.has_bias and len(bucket.views) > 1) else None
-            dW, db, _ = fused_bwd(dz, xc, wc, gout, ctx.dt, ctx.colsum, need_dw=True,
-                                  need_db=(need_db and ctx.has_bias), need_dx=False, dW=bucket.views[0], db=db_view,
-                                  dw_prezeroed=True)
-            join = bucket.exchange_overlapped()
-            dX = None
-            if need_dx:
-                _, _, dX = fused_bwd(dz, xc, wc, gout, ctx.dt, None, need_dw=False, need_db=False, need_dx=True)
-            join()
-        else:
-            dW, db, dX = fused_bwd(dz, xc, wc, gout, ctx.dt, ctx.colsum, need_dw=need_dw,
-                                   need_db=(need_db and ctx.has_bias), need_dx=need_dx,
-                                   dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None)
+        # dW + db first, straight into the exchange bucket; the exchange starts when they are complete and runs
+        # while the dX contraction does
+        if dW0 is None:
+            bucket.views[0].zero_()
+        db_view = bucket.views[1] if (need_db and ctx.has_bias and len(bucket.views) > 1) else None
+        dW, db, _ = fused_bwd(dz, xc, wc, gout, ctx.dt, ctx.colsum, need_dw=True,
+                              need_db=(need_db and ctx.has_bias), need_dx=False, dW=bucket.views[0], db=db_view,
+                              dw_prezeroed=True)
+        join = bucket.exchange_overlapped()
+        dX = None
+        if need_dx:
+            _, _, dX = fused_bwd(dz, xc, wc, gout, ctx.dt, None, need_dw=False, need_db=False, need_dx=True)
+        join()
         dX, dW, db = _grads_in_param_dtypes(ctx, dX, dW, db)
         return dX, dW, db, None, None, None, None, None, None, None
 
@@ -797,36 +806,16 @@ class SoftmaxCEFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, labels, weights, avg, compute_dtype, acc_out=None):
         _require_cuda(x, weight, bias, labels)
-        xc, wc, b32 = _fc_cls_operands(x, weight, bias, compute_dtype)
-        need_grad = any(ctx.needs_input_grad[:3])
-        dW = None
-        if need_grad and ctx.needs_input_grad[1] and PREP_IN_FORWARD:
-            dW = torch.empty((wc.shape[0], wc.shape[1]), dtype=torch.float32, device=xc.device)
-        loss, _, dz, _ = ce_fwd(xc, wc, b32, labels, weights, avg, want_acc=acc_out is not None, want_dz=need_grad,
-                                clear=dW, acc_out=acc_out)
-        ctx.dW = dW
-        ctx.num_cols = wc.shape[0]
-        _save_param_dtypes(ctx, x, weight, bias)
-        if need_grad:
-            ctx.save_for_backward(xc, wc, dz)
+        xc, wc, b32, dW = _fused_loss_prologue(ctx, x, weight, bias, compute_dtype)
+        loss, _, dz, _ = ce_fwd(xc, wc, b32, labels, weights, avg, want_acc=acc_out is not None,
+                                want_dz=any(ctx.needs_input_grad[:3]), clear=dW, acc_out=acc_out)
+        _fused_loss_saved(ctx, xc, wc, dz, dW)
         return loss
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_loss):
-        return _single_bin_bwd(ctx, grad_loss) + (None,) * 5
-
-
-def _single_bin_bwd(ctx, grad_loss):
-    """(dX, dW, db) in the parameters' dtypes from the dz~ a single-bin fused forward saved: one bags_bwd over the slice
-    (0, C); dX only when x needs a gradient, dW zeroed by the forward kernel when ``ctx.dW`` is set."""
-    xc, wc, dz = ctx.saved_tensors
-    need_dx, need_dw, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
-    dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
-    dW, db, dX = fused_bwd(dz, xc, wc, _gout(grad_loss), _single_slice_tables(ctx.num_cols, xc.device), None,
-                           need_dw=need_dw, need_db=(need_db and ctx.has_bias), need_dx=need_dx,
-                           dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None)
-    return _grads_in_param_dtypes(ctx, dX, dW, db)
+        return _fused_loss_bwd(ctx, grad_loss) + (None,) * 5
 
 
 class SigmoidFocalFunction(torch.autograd.Function):
@@ -841,24 +830,17 @@ class SigmoidFocalFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, targets, weights, norm, gamma, alpha, compute_dtype, labels=None, acc_out=None):
         _require_cuda(x, weight, bias, targets)
-        xc, wc, b32 = _fc_cls_operands(x, weight, bias, compute_dtype)
-        need_grad = any(ctx.needs_input_grad[:3])
-        dW = None
-        if need_grad and ctx.needs_input_grad[1] and PREP_IN_FORWARD:
-            dW = torch.empty((wc.shape[0], wc.shape[1]), dtype=torch.float32, device=xc.device)
+        xc, wc, b32, dW = _fused_loss_prologue(ctx, x, weight, bias, compute_dtype)
         loss, _, dz, _ = focal_fwd(xc, wc, b32, targets, norm, gamma, alpha, labels=labels, weights=weights,
-                                   want_acc=acc_out is not None, want_dz=need_grad, clear=dW, acc_out=acc_out)
-        ctx.dW = dW
-        ctx.num_cols = wc.shape[0]
-        _save_param_dtypes(ctx, x, weight, bias)
-        if need_grad:
-            ctx.save_for_backward(xc, wc, dz)
+                                   want_acc=acc_out is not None, want_dz=any(ctx.needs_input_grad[:3]), clear=dW,
+                                   acc_out=acc_out)
+        _fused_loss_saved(ctx, xc, wc, dz, dW)
         return loss
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_loss):
-        return _single_bin_bwd(ctx, grad_loss) + (None,) * 8
+        return _fused_loss_bwd(ctx, grad_loss) + (None,) * 8
 
 
 class SmoothL1BoxFunction(torch.autograd.Function):

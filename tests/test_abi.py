@@ -72,6 +72,40 @@ def test_unknown_weights_dtype_is_rejected():
     rc = lib.bags_group_ce(p, 8, p, p, sl, p, 2, None, 1, 8, 2, 4, p, None, None, 0, 0, None, p, ws, None)
     assert rc == -1 and b'weights dtype 2' in lib.bags_last_error()
 
+def test_fwd_invalid_arguments_return_error_codes():
+    """bags_fwd's argument rules on both routes (fused: logits NULL; materialised: a logits buffer), reported before
+    anything touches a device -- the fused route shares them with bags_ce_fwd and bags_focal_fwd."""
+    lib = nat.lib()
+    buf = (C.c_char * 256)()
+    base = (C.addressof(buf) + 15) // 16 * 16
+    ws = lib.bags_workspace_bytes()
+    tiles = nat.int32_array([0, 4, 4, 4])   # two bins tiling C = 8: eligible for the fused kernel
+    assert lib.bags_fused_eligible(tiles, 2, 8) == 1
+
+    def call(slices=tiles, l2b=base, wdt=nat.WEIGHTS_U8, N=4, K=8, dtype=nat.DTYPE_BF16, bias=None, logits=None,
+             dz=None, ldd=0, colsum=None, ntiles=0, wsb=ws, clear=None, clear_bytes=0):
+        return lib.bags_fwd(base, K, base, K, bias, base, l2b, slices, None, wdt, None, N, K, 8, 2, 4, dtype, logits,
+                            8 if logits else 0, base, None, dz, ldd, colsum, ntiles, base, wsb, clear, clear_bytes, None)
+
+    gap = nat.int32_array([0, 2, 4, 4])     # columns 2 and 3 lie in no bin
+    assert lib.bags_fused_eligible(gap, 2, 8) == 0
+    assert call(slices=gap) == -1 and b'eligible' in lib.bags_last_error()
+    assert call(wdt=2) == -1 and b'weights dtype 2' in lib.bags_last_error()
+    assert call(dtype=7) == -1 and b'dtype' in lib.bags_last_error()
+    assert call(l2b=None) == -1 and b'NULL' in lib.bags_last_error()
+    assert call(K=0) == -1 and b'bad shape' in lib.bags_last_error()
+    assert call(bias=base + 4) == -1 and b'bias' in lib.bags_last_error()
+    assert call(dz=base, ldd=12) == -1 and b'ldd' in lib.bags_last_error()     # not a multiple of 8
+    assert call(dz=base, ldd=0) == -1 and b'ldd' in lib.bags_last_error()      # < C
+    assert call(colsum=base, ntiles=2) == -1 and b'colsum' in lib.bags_last_error()   # ceil(4/128) = 1 row tile
+    assert call(clear=base + 4, clear_bytes=16) == -1 and b'clear' in lib.bags_last_error()
+    assert call(clear=base, clear_bytes=8) == -1 and b'clear' in lib.bags_last_error()
+    assert call(wsb=16) == -1 and b'workspace' in lib.bags_last_error()
+    # the materialised route keeps the rules it shares with the fused one
+    assert call(logits=base, colsum=base, ntiles=0) == -1 and b'colsum' in lib.bags_last_error()
+    assert call(logits=base, clear=base + 4, clear_bytes=16) == -1 and b'clear' in lib.bags_last_error()
+
+
 def test_cast_bf16_rejects_misaligned_pointers():
     """bags_cast_bf16 reads float4 from src and writes 8-byte groups to dst: a misaligned pointer is a bad argument,
     reported before any launch."""

@@ -21,6 +21,7 @@ DTYPE_BF16 = 1
 WEIGHTS_U8 = 0
 WEIGHTS_F32 = 1
 MAX_BINS = 8
+MASK_TILE = 64          # BAGS_MASK_TILE: pixels per tile of bags_mask_fwd's rsum scratch
 
 _lib = None
 _lock = threading.Lock()
@@ -46,6 +47,9 @@ SIGNATURES = {
     'bags_box_fwd': (_i, [_vp, _ll, _i, _vp, _ll, _vp, _vp, _vp, _vp, C.c_float, C.c_float, _i, _i, _i, _vp, _vp, _vp,
                           _vp, _vp, _sz, _vp]),
     'bags_box_bwd': (_i, [_vp, _vp, _vp, _ll, _i, _vp, _ll, _vp, _vp, _i, _i, _i, _vp, _ll, _vp, _vp, _ll, _vp]),
+    'bags_mask_fwd': (_i, [_vp, _i, _vp, _ll, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _vp, _sz,
+                           _vp]),
+    'bags_mask_bwd': (_i, [_vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),
     'bags_reweight': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     'bags_bwd_scratch_bytes': (_sz, [_i, _ll, _i]),
     'bags_bwd': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _ll, _vp, _sz, _i, _i,

@@ -13,7 +13,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, 'csrc')
 OUT = os.path.join(_HERE, 'libbags_b200.so')
 SOURCES = [os.path.join(CSRC, 'bags_api.cu')]
-HEADERS = [os.path.join(CSRC, f) for f in ('bags_ptx.cuh', 'bags_wgmma.cuh', 'bags_gemm.cuh', 'bags_kernels.cuh', 'bags_fused_fwd.cuh', 'bags_allreduce.cuh', 'bags_nms.cuh', 'bags_box.cuh')] + [
+HEADERS = [os.path.join(CSRC, f) for f in ('bags_ptx.cuh', 'bags_wgmma.cuh', 'bags_gemm.cuh', 'bags_kernels.cuh', 'bags_fused_fwd.cuh', 'bags_allreduce.cuh', 'bags_nms.cuh', 'bags_box.cuh', 'bags_mask.cuh')] + [
     os.path.join(os.path.dirname(_HERE), 'include', 'bags_b200.h')]
 
 NVCC_FLAGS = [

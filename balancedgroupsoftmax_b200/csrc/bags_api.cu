@@ -20,6 +20,7 @@
 #include "bags_allreduce.cuh"
 #include "bags_nms.cuh"
 #include "bags_box.cuh"
+#include "bags_mask.cuh"
 
 using namespace bags;
 
@@ -786,6 +787,111 @@ extern "C" int bags_box_bwd(const float* g, const float* gout, const void* x, lo
   const dim3 grid(static_cast<unsigned>(class_units + roi_units));
   if (dtype == BAGS_DTYPE_BF16) bags_box_bwd_kernel<true><<<grid, kBoxBwdThreads, 0, stream>>>(p);
   else                          bags_box_bwd_kernel<false><<<grid, kBoxBwdThreads, 0, stream>>>(p);
+  BAGS_CUDA(cudaGetLastError());
+  return BAGS_OK;
+}
+
+// ----------------------------------------------------------------------------
+// class-specific mask logits + mask_cross_entropy (fcn_mask_head.py:82,102,114-123, cross_entropy_loss.py:54-61)
+// ----------------------------------------------------------------------------
+static int check_mask_shape(const char* who, int dtype, long long ldw, int P, int Cin, int HW, int classes) {
+  BAGS_REQUIRE(P >= 0 && Cin >= 1 && HW >= 1, "%s: bad shape P=%d Cin=%d HW=%d", who, P, Cin, HW);
+  BAGS_REQUIRE(dtype == BAGS_DTYPE_F32 || dtype == BAGS_DTYPE_BF16, "%s: bad dtype %d", who, dtype);
+  BAGS_REQUIRE(classes >= 1 && classes <= kBoxMaxClasses, "%s: classes=%d outside [1,%d]", who, classes, kBoxMaxClasses);
+  BAGS_REQUIRE(ldw >= Cin, "%s: ldw=%lld must be >= Cin=%d", who, ldw, Cin);
+  const long long tiles = (HW + kMaskTile - 1) / kMaskTile;
+  BAGS_REQUIRE(tiles * P < (1LL << 30), "%s: P=%d HW=%d is too large", who, P, HW);
+  return BAGS_OK;
+}
+
+static long long mask_rsum_floats(int P, int Cin, int HW) {
+  const long long tiles = (HW + kMaskTile - 1) / kMaskTile;
+  return static_cast<long long>(P) * tiles * (Cin + 2LL);
+}
+
+// four pixels per thread when every (RoI, channel) row starts on a 4-element boundary
+static bool mask_vec4(const void* y, int dtype, int HW) {
+  return (HW % 4) == 0 && aligned(y, dtype == BAGS_DTYPE_BF16 ? 8 : 16);
+}
+
+extern "C" int bags_mask_fwd(const void* y, int dtype, const float* w, long long ldw, const float* bias,
+                             const int64_t* labels, const float* targets, int P, int Cin, int HW, int classes,
+                             float* loss, float* g, float* rsum, size_t rsum_floats, int32_t* index, void* workspace,
+                             size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = check_mask_shape("bags_mask_fwd", dtype, ldw, P, Cin, HW, classes)) return rc;
+  BAGS_REQUIRE(loss && index && workspace && (P == 0 || (y && w && labels && targets && g && rsum)),
+               "bags_mask_fwd: NULL argument");
+  BAGS_REQUIRE(static_cast<long long>(rsum_floats) >= mask_rsum_floats(P, Cin, HW),
+               "bags_mask_fwd: rsum too small (%zu < %lld floats)", rsum_floats, mask_rsum_floats(P, Cin, HW));
+  BAGS_REQUIRE(workspace_bytes >= bags_workspace_bytes(), "bags_mask_fwd: workspace too small (%zu < %zu)",
+               workspace_bytes, bags_workspace_bytes());
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  // the class index, also for P == 0 (all offsets zero)
+  bags_mask_sort_kernel<<<1, kBoxThreads, 0, stream>>>(reinterpret_cast<const long long*>(labels), P, classes, index);
+  BAGS_CUDA(cudaGetLastError());
+  if (P == 0) {
+    BAGS_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), stream));
+    return BAGS_OK;
+  }
+  MaskFwdParams p{};
+  p.y = y; p.w = w; p.ldw = ldw; p.bias = bias;
+  p.labels = reinterpret_cast<const long long*>(labels);
+  p.targets = targets;
+  p.P = P; p.Cin = Cin; p.HW = HW; p.classes = classes;
+  p.tiles = (HW + kMaskTile - 1) / kMaskTile;
+  p.n = static_cast<float>(static_cast<double>(P) * HW);
+  p.loss = loss; p.g = g; p.rsum = rsum;
+  p.counter = reinterpret_cast<unsigned int*>(workspace) + kMaskCounterWord;
+  // one CTA per (RoI, pixel tile): the grid depends only on the shape, so the loss's summation order does too
+  const dim3 grid(static_cast<unsigned>(P * p.tiles));
+  const bool v4 = mask_vec4(y, dtype, HW);
+  if (dtype == BAGS_DTYPE_BF16) {
+    if (v4) bags_mask_fwd_kernel<true, 4><<<grid, kMaskThreads, 0, stream>>>(p);
+    else    bags_mask_fwd_kernel<true, 1><<<grid, kMaskThreads, 0, stream>>>(p);
+  } else {
+    if (v4) bags_mask_fwd_kernel<false, 4><<<grid, kMaskThreads, 0, stream>>>(p);
+    else    bags_mask_fwd_kernel<false, 1><<<grid, kMaskThreads, 0, stream>>>(p);
+  }
+  BAGS_CUDA(cudaGetLastError());
+  return BAGS_OK;
+}
+
+extern "C" int bags_mask_bwd(const float* g, const float* rsum, const float* gout, int dtype, const float* w,
+                             long long ldw, const int64_t* labels, const int32_t* index, int P, int Cin, int HW,
+                             int classes, float* dW, long long lddw, float* db, void* dY, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = check_mask_shape("bags_mask_bwd", dtype, ldw, P, Cin, HW, classes)) return rc;
+  BAGS_REQUIRE(index && ((dW == nullptr && db == nullptr) || P == 0 || rsum) &&
+               (dY == nullptr || P == 0 || (g && w && labels)),
+               "bags_mask_bwd: NULL argument");
+  if (dW != nullptr) BAGS_REQUIRE(lddw >= Cin, "bags_mask_bwd: lddw=%lld must be >= Cin=%d", lddw, Cin);
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  MaskBwdParams p{};
+  p.g = g; p.rsum = rsum; p.gout = gout; p.w = w; p.ldw = ldw;
+  p.labels = reinterpret_cast<const long long*>(labels);
+  p.index = index;
+  p.P = P; p.Cin = Cin; p.HW = HW; p.classes = classes;
+  p.tiles = (HW + kMaskTile - 1) / kMaskTile;
+  p.dW = dW; p.lddw = lddw; p.db = db; p.dY = dY;
+  p.chunks = (Cin + 1 + 31) / 32;
+  // work list: class units (32 columns of dW and db per class) first, then (RoI, pixel tile) units (dY)
+  const long long class_units = (dW != nullptr || db != nullptr) ? 1LL * classes * p.chunks : 0;
+  const long long roi_units = (dY != nullptr) ? 1LL * P * p.tiles : 0;
+  BAGS_REQUIRE(class_units + roi_units < (1LL << 31), "bags_mask_bwd: P=%d Cin=%d HW=%d is too large", P, Cin, HW);
+  p.class_units = static_cast<int>(class_units);
+  if (class_units + roi_units == 0) return BAGS_OK;
+  const dim3 grid(static_cast<unsigned>(class_units + roi_units));
+  const bool v4 = dY != nullptr && mask_vec4(dY, dtype, HW);
+  if (dtype == BAGS_DTYPE_BF16) {
+    if (v4) bags_mask_bwd_kernel<true, 4><<<grid, kMaskThreads, 0, stream>>>(p);
+    else    bags_mask_bwd_kernel<true, 1><<<grid, kMaskThreads, 0, stream>>>(p);
+  } else {
+    if (v4) bags_mask_bwd_kernel<false, 4><<<grid, kMaskThreads, 0, stream>>>(p);
+    else    bags_mask_bwd_kernel<false, 1><<<grid, kMaskThreads, 0, stream>>>(p);
+  }
   BAGS_CUDA(cudaGetLastError());
   return BAGS_OK;
 }

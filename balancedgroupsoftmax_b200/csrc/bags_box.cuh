@@ -63,22 +63,35 @@ __device__ __forceinline__ float4 box_load4(const void* base, long long off) {
 
 __device__ __forceinline__ bool box_positive(long long l, int classes) { return l > 0 && l < classes; }
 
-// The class index: offsets[c] = #positives of classes < c (offsets[classes] = all positives) and, after the offsets,
-// the positive RoIs ordered by class and, inside a class, by ascending RoI id.  Run by one CTA of kBoxThreads.
-__device__ __forceinline__ void box_class_sort(const BoxFwdParams& p, int* s_cursor, short* s_lab, int* s_scan) {
+// The label rules of the class index: a box loss reads the RoIs with 0 < l < classes, a mask loss every 0 <= l <
+// classes (class-agnostic mask heads pass label 0 to their one channel).
+struct BoxPositive {
+  __device__ __forceinline__ bool operator()(long long l, int classes) const { return box_positive(l, classes); }
+};
+struct MaskLabelValid {
+  __device__ __forceinline__ bool operator()(long long l, int classes) const { return l >= 0 && l < classes; }
+};
+
+// The class index of the RoIs whose label passes ``Valid``: offsets[c] = #such RoIs of classes < c (offsets[classes]
+// = all of them) and, after the offsets, those RoIs ordered by class and, inside a class, by ascending RoI id.  Run by
+// one CTA of kBoxThreads.
+template <class Valid>
+__device__ __forceinline__ void box_class_sort(const long long* labels, int N, int classes, int* index, int* s_cursor,
+                                               short* s_lab, int* s_scan) {
+  const Valid valid;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  int* offsets = p.index;
-  int* rois = p.index + p.classes + 1;
-  for (int c = tid; c < p.classes; c += kBoxThreads) s_cursor[c] = 0;
+  int* offsets = index;
+  int* rois = index + classes + 1;
+  for (int c = tid; c < classes; c += kBoxThreads) s_cursor[c] = 0;
   __syncthreads();
-  for (int n = tid; n < p.N; n += kBoxThreads) {
-    const long long l = __ldg(p.labels + n);
-    if (box_positive(l, p.classes)) atomicAdd(s_cursor + l, 1);
+  for (int n = tid; n < N; n += kBoxThreads) {
+    const long long l = __ldg(labels + n);
+    if (valid(l, classes)) atomicAdd(s_cursor + l, 1);
   }
   __syncthreads();
   // exclusive scan: thread t owns the contiguous class run [t * per, (t + 1) * per)
-  const int per = (p.classes + kBoxThreads - 1) / kBoxThreads;
-  const int lo = min(tid * per, p.classes), hi = min(lo + per, p.classes);
+  const int per = (classes + kBoxThreads - 1) / kBoxThreads;
+  const int lo = min(tid * per, classes), hi = min(lo + per, classes);
   int own = 0;
   for (int c = lo; c < hi; ++c) own += s_cursor[c];
   int incl = own;
@@ -98,15 +111,15 @@ __device__ __forceinline__ void box_class_sort(const BoxFwdParams& p, int* s_cur
     s_cursor[c] = run;
     run += cnt;
   }
-  if (tid == kBoxThreads - 1) offsets[p.classes] = run;
+  if (tid == kBoxThreads - 1) offsets[classes] = run;
   __syncthreads();
   // stable placement: one warp walks the RoIs in order, 32 at a time; lanes with the same class take consecutive
   // slots in lane order
-  for (int base = 0; base < p.N; base += kBoxSortBatch) {
-    const int m = min(kBoxSortBatch, p.N - base);
+  for (int base = 0; base < N; base += kBoxSortBatch) {
+    const int m = min(kBoxSortBatch, N - base);
     for (int i = tid; i < m; i += kBoxThreads) {
-      const long long l = __ldg(p.labels + base + i);
-      s_lab[i] = box_positive(l, p.classes) ? static_cast<short>(l) : static_cast<short>(-1);
+      const long long l = __ldg(labels + base + i);
+      s_lab[i] = valid(l, classes) ? static_cast<short>(l) : static_cast<short>(-1);
     }
     __syncthreads();
     if (warp == 0) {
@@ -139,7 +152,7 @@ bags_box_fwd_kernel(const BoxFwdParams p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   float mine = 0.f;   // lane 0: this warp's rows, in ascending order
   if (blockIdx.x == gridDim.x - 1) {
-    box_class_sort(p, s_cursor, s_lab, s_scan);
+    box_class_sort<BoxPositive>(p.labels, p.N, p.classes, p.index, s_cursor, s_lab, s_scan);
   } else {
     const int stride = (gridDim.x - 1) * (kBoxThreads / 32);
     const float inv_avg = 1.f / p.avg;

@@ -12,6 +12,9 @@ replaced by one fused CUDA call (ops.GroupSoftmaxFunction); the per-bin modules
 only contribute their ``loss_weight``.  ``SmoothL1Loss`` (<= 128x4 values per
 image) stays plain PyTorch, as scopes it.
 
+With ``use_mask=True`` ``CrossEntropyLoss`` is the reference's ``mask_cross_entropy`` on materialised mask logits;
+the mask heads (mask_head.py) fuse it into conv_logits instead (ops.MaskBCEFunction).
+
 ``FocalLoss`` keeps the contract of mmdet/models/losses/focal_loss.py:46-88,
 quirks included; on plain logits it restates the reference's op in torch, and
 ``ReweightBBoxHead`` fuses it into fc_cls (ops.SigmoidFocalFunction).
@@ -41,6 +44,16 @@ def _reduce(loss, weight, reduction, avg_factor):
     return loss
 
 
+def mask_cross_entropy(pred, target, label, reduction='mean', avg_factor=None):
+    """The mask loss of FCNMaskHead on materialised logits ``pred`` [P, classes, H, W]: each RoI p is scored on its
+    own channel label[p] only, with a BCE-with-logits against ``target`` [P, H, W] averaged over all P * H * W pixels;
+    returned as a [1] tensor.  Only reduction 'mean' without avg_factor exists, as in mmdet.  Heads with
+    ``MaskPredHandle`` compute the same loss fused into conv_logits instead (ops.MaskBCEFunction)."""
+    assert reduction == 'mean' and avg_factor is None, 'the mask loss supports reduction="mean" without avg_factor only'
+    own_channel = pred[torch.arange(pred.shape[0], device=pred.device), label]
+    return F.binary_cross_entropy_with_logits(own_channel, target, reduction='mean').reshape(1)
+
+
 class CrossEntropyLoss(nn.Module):
 
     def __init__(self, use_sigmoid=False, use_mask=False, reduction='mean', loss_weight=1.0):
@@ -55,7 +68,8 @@ class CrossEntropyLoss(nn.Module):
         assert reduction_override in (None, 'none', 'mean', 'sum')
         reduction = reduction_override if reduction_override else self.reduction
         if self.use_mask:
-            raise NotImplementedError('mask cross-entropy is outside the BAGS head path')
+            return self.loss_weight * mask_cross_entropy(cls_score, label, weight, reduction=reduction,
+                                                         avg_factor=avg_factor, **kwargs)
         if weight is not None:
             weight = weight.float()
         if self.use_sigmoid:

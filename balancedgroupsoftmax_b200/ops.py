@@ -219,6 +219,63 @@ def fused_eligible(dt: DeviceTables) -> bool:
     return bool(nat.lib().bags_fused_eligible(dt.slices_host, dt.G, dt.num_logits))
 
 
+def mask_fwd(y, w, bias, labels, targets):
+    """bags_mask_fwd: the class-specific channel of conv_logits (a 1x1 conv) fused with mask_cross_entropy -- BCE with
+    logits, 'mean' over P * H * W (FCNMaskHead.loss).  Returns (loss [1], g [P, H, W], rsum, index int32
+    [classes + 1 + P]); ``g``, ``rsum`` and ``index`` feed ``mask_bwd``.  ``y``: bf16 or fp32 [P, Cin, H, W] (made
+    contiguous); ``w``: the fp32 [classes, Cin] weight (never cast to bf16); ``labels``: int64 [P], a row with a label
+    outside [0, classes) contributes 0 but counts in the mean; ``targets``: [P, H, W]."""
+    _require_cuda(y, w, bias, labels, targets)
+    y = y.contiguous()
+    w = _row_major(w.reshape(w.shape[0], -1))
+    if w.dtype != torch.float32:
+        raise nat.BagsNativeError('mask_fwd: the conv_logits weight must be float32 (got %s)' % w.dtype)
+    P, Cin, H, W_ = y.shape
+    classes = w.shape[0]
+    if bias is not None:
+        assert bias.dtype == torch.float32 and bias.numel() == classes, 'mask_fwd: bias must be fp32 [classes]'
+        bias = bias.contiguous()
+    labels = labels.contiguous()
+    assert w.shape[1] == Cin and labels.dtype == torch.int64 and labels.numel() == P
+    targets = targets.to(torch.float32).contiguous()
+    assert targets.shape == (P, H, W_)
+    dev = y.device
+    tiles = (H * W_ + nat.MASK_TILE - 1) // nat.MASK_TILE
+    loss = torch.empty((1,), dtype=torch.float32, device=dev)
+    g = torch.empty((P, H, W_), dtype=torch.float32, device=dev)
+    rsum = torch.empty((P * tiles * (Cin + 2),), dtype=torch.float32, device=dev)
+    index = torch.empty((classes + 1 + P,), dtype=torch.int32, device=dev)
+    ws = _workspace(dev)
+    nat.check(nat.lib().bags_mask_fwd(
+        y.data_ptr(), _dtype_code(y.dtype), w.data_ptr(), w.stride(0), nat.ptr(bias), labels.data_ptr(),
+        targets.data_ptr(), P, Cin, H * W_, classes, loss.data_ptr(), g.data_ptr(), rsum.data_ptr(), rsum.numel(),
+        index.data_ptr(), ws.data_ptr(), ws.numel(), _stream_ptr(dev)), 'bags_mask_fwd')
+    return loss, g, rsum, index
+
+
+def mask_bwd(g, rsum, gout, w, labels, index, y_shape, y_dtype, need_dw: bool = True, need_db: bool = True,
+             need_dy: bool = True):
+    """bags_mask_bwd: (dW fp32 [classes, Cin] | None, db fp32 [classes] | None, dY [P, Cin, H, W] in ``y_dtype`` |
+    None) from the ``g``, ``rsum`` and ``index`` of ``mask_fwd``; ``gout``: dL/dloss as a device fp32 [1] tensor, or
+    None for 1."""
+    _require_cuda(g, rsum, gout, w, labels, index)
+    w = _row_major(w.reshape(w.shape[0], -1))
+    P, Cin, H, W_ = y_shape
+    classes = w.shape[0]
+    dev = g.device
+    if gout is not None:
+        gout = _gout(gout)
+        assert gout.numel() == 1
+    dW = torch.empty((classes, Cin), dtype=torch.float32, device=dev) if need_dw else None
+    db = torch.empty((classes,), dtype=torch.float32, device=dev) if need_db else None
+    dY = torch.empty((P, Cin, H, W_), dtype=y_dtype, device=dev) if need_dy else None
+    nat.check(nat.lib().bags_mask_bwd(
+        g.data_ptr(), rsum.data_ptr(), nat.ptr(gout), _dtype_code(y_dtype), w.data_ptr(), w.stride(0),
+        labels.contiguous().data_ptr(), index.data_ptr(), P, Cin, H * W_, classes, nat.ptr(dW), Cin, nat.ptr(db),
+        nat.ptr(dY), _stream_ptr(dev)), 'bags_mask_bwd')
+    return dW, db, dY
+
+
 def _fused_outputs(x, w, bias, G: int, want_acc: bool, want_dz: bool, want_colsum: bool,
                    clear: Optional[torch.Tensor], acc_out: Optional[torch.Tensor] = None):
     """Operands and outputs shared by bags_fwd, bags_ce_fwd and bags_focal_fwd: row-major x and w of one dtype, the
@@ -872,6 +929,43 @@ class SmoothL1BoxFunction(torch.autograd.Function):
                              need_db=ctx.needs_input_grad[2] and ctx.has_bias, need_dx=ctx.needs_input_grad[0])
         dX, dW, db = _grads_in_param_dtypes(ctx, dX, dW, db)
         return dX, dW, db, None, None, None, None, None
+
+
+class MaskBCEFunction(torch.autograd.Function):
+    """loss[1] = mask_cross_entropy of the class-specific 1x1 conv_logits, the conv included (FCNMaskHead.loss on
+    conv_logits(y) with loss_weight 1) -- only the channel of each RoI's label:
+
+    forward : bags_mask_fwd (fp32 products from the fp32 weight, the loss, its gradient g, the per-tile sums of g y for
+              dW and the class index; no host sync)
+    backward: bags_mask_bwd (dW fully written -- zero rows for absent classes --, db, dY), only what autograd needs.
+
+    ``weight`` may be the conv's [classes, Cin, 1, 1] parameter; its gradient comes back in that shape."""
+
+    @staticmethod
+    def forward(ctx, y, weight, bias, labels, targets):
+        _require_cuda(y, weight, bias, labels, targets)
+        yc = y if y.dtype in (torch.bfloat16, torch.float32) else y.float()
+        wc = weight if weight.dtype == torch.float32 else weight.float()
+        b32 = None if bias is None else (bias if bias.dtype == torch.float32 else bias.float())
+        labels = labels.contiguous()
+        loss, g, rsum, index = mask_fwd(yc, wc, b32, labels, targets)
+        _save_param_dtypes(ctx, y, weight, bias)
+        ctx.y_shape, ctx.y_cdtype, ctx.w_shape = tuple(yc.shape), yc.dtype, weight.shape
+        if any(ctx.needs_input_grad[:3]):
+            ctx.save_for_backward(g, rsum, index, wc.reshape(wc.shape[0], -1), labels)
+        return loss
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_loss):
+        g, rsum, index, wc, labels = ctx.saved_tensors
+        dW, db, dY = mask_bwd(g, rsum, grad_loss, wc, labels, index, ctx.y_shape, ctx.y_cdtype,
+                              need_dw=ctx.needs_input_grad[1], need_db=ctx.needs_input_grad[2] and ctx.has_bias,
+                              need_dy=ctx.needs_input_grad[0])
+        dY, dW, db = _grads_in_param_dtypes(ctx, dY, dW, db)
+        if dW is not None:
+            dW = dW.reshape(ctx.w_shape)
+        return dY, dW, db, None, None
 
 
 class GroupCEFunction(torch.autograd.Function):

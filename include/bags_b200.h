@@ -24,6 +24,8 @@
  *     focal_loss.py:29-88, sigmoid_focal_loss_cuda.cu:23-96
  *   fc_reg + gather + SmoothL1Loss (class-specific)       bags_box_fwd / bags_box_bwd
  *     bbox_head.py:118-128, smooth_l1_loss.py
+ *   conv_logits + mask_cross_entropy (class-specific)  bags_mask_fwd / bags_mask_bwd
+ *     fcn_mask_head.py:82,102,114-123, cross_entropy_loss.py:54-61
  *   autograd backward of the above (dW, db, dX)           bags_bwd
  *     triggered at mmdet/core/utils/dist_utils.py:53
  *   GSBBoxHeadWith0._merge_score                          bags_merge_scores
@@ -202,6 +204,38 @@ int bags_box_fwd(const void* x, long long ldx, int dtype, const float* w, long l
 int bags_box_bwd(const float* g, const float* gout, const void* x, long long ldx, int dtype, const float* w, long long ldw,
                  const int64_t* labels, const int32_t* index, int N, int K, int classes, float* dW, long long lddw,
                  float* db, void* dX, long long lddx, void* stream);
+
+/* Class-specific mask logits fused with their BCE loss -- replaces, for the training loss, conv_logits' 1x1 conv into
+ * [P, classes, H, W] (fcn_mask_head.py:82,102), the channel gather pred[arange(P), labels] of mask_cross_entropy and
+ * its BCE-with-logits 'mean' (FCNMaskHead.loss, fcn_mask_head.py:114-123; cross_entropy_loss.py:54-61).  A row p is
+ * valid when 0 <= l = labels[p] < classes (class-agnostic heads pass label 0 to one channel); only channel l of it is
+ * computed, with fp32 products and accumulation from the fp32 W, over the HW = H * W pixels q:
+ *   z[p,q]  = bias[l] + sum_c W[l,c] y[p,c,q]
+ *   loss[0] = sum_{p valid, q} (max(z,0) - z t[p,q] + log1p(exp(-|z|))) / (P HW)   (fixed order: bit-identical runs)
+ *   g[p,q]  = (sigmoid(z) - t[p,q]) / (P HW); 0 on an invalid row, which still counts in P HW
+ * y: contiguous [P, Cin, HW] bf16 or fp32 (dtype); W: [classes, Cin] fp32 (ldw >= Cin); bias: [classes] fp32 or NULL;
+ * labels: int64 [P]; targets, g: contiguous fp32 [P, HW].  1 <= classes <= 8192.  P == 0: loss = 0.
+ * rsum: fp32 scratch of at least P * ceil(HW / BAGS_MASK_TILE) * (Cin + 2) floats, written for bags_mask_bwd: each
+ * (RoI, pixel tile)'s sum_q g y per channel and sum_q g, then the tile losses.  index: int32 [classes + 1 + P], the
+ * valid RoIs sorted by class (as bags_box_fwd's).  workspace: as bags_fwd (its counter is left at zero).
+ * Two launches, no host sync; y is read from memory once. */
+#define BAGS_MASK_TILE 64
+int bags_mask_fwd(const void* y, int dtype, const float* w, long long ldw, const float* bias, const int64_t* labels,
+                  const float* targets, int P, int Cin, int HW, int classes, float* loss, float* g, float* rsum,
+                  size_t rsum_floats, int32_t* index, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Backward of bags_mask_fwd (the gather's scatter and conv_logits' dW / db / dX), given its g, rsum, index and
+ * gout = dL/dloss[0] (device fp32 [1]; NULL => 1):
+ *   dW[l, c]   = gout sum_{p of class l} sum_q g[p,q] y[p,c,q]              fp32 [classes, Cin] (lddw), FULLY
+ *                                                                          overwritten: absent classes are zero
+ *   db[l]      = gout sum_{p of class l} sum_q g[p,q]                       fp32 [classes]
+ *   dY[p,c,q]  = gout g[p,q] W[l,c]                                         dtype [P, Cin, HW]; 0 on invalid rows
+ * The class sums run in an order fixed by the labels alone (the class's RoIs ascending, per-tile partials dealt to 8
+ * warps, the warps added in order).  Each output is optional (NULL to skip).  One launch; no atomics, so every output
+ * is bit-identical across runs and CUDA-graph replays. */
+int bags_mask_bwd(const float* g, const float* rsum, const float* gout, int dtype, const float* w, long long ldw,
+                  const int64_t* labels, const int32_t* index, int P, int Cin, int HW, int classes, float* dW,
+                  long long lddw, float* db, void* dY, void* stream);
 
 /* ---- reweight head variant (GSBBoxHeadWith0Reweight, mmdet/models/bbox_heads/gs_bbox_head_with0_reweight.py:57-109):
  * per-(bin, RoI) fp32 weights instead of 0/1 masks, consumed by bags_fwd / bags_group_ce as BAGS_WEIGHTS_F32. ----

@@ -133,14 +133,35 @@ def delta2bbox(rois, deltas, means=(0, 0, 0, 0), stds=(1, 1, 1, 1), max_shape=No
 # --------------------------------------------------------------------------- lazy projections
 class _LazyHandle(object):
     """A projection a training ``forward`` records instead of launching, so that ``loss`` can fuse it with its loss.
-    Subclasses give ``shape``, ``device`` and ``tensor()`` (the materialised, autograd-connected output); indexing, any
-    other attribute and any torch function handed a handle see ``tensor()``, so every other consumer keeps working."""
+    Subclasses give ``shape`` and ``_project()`` (the projection of ``input``, looked up on the head when it runs).
+    ``tensor()`` is the materialised, autograd-connected output, computed once; indexing, any other attribute and any
+    torch function handed a handle see it, so every other consumer keeps working.  Every real attribute is set in
+    ``__init__``: reading one the handle does not have materialises the projection."""
+
+    def __init__(self, head, input: torch.Tensor):
+        self._head = head
+        self.input = input
+        self._out = None
+
+    @property
+    def pending(self) -> bool:
+        """True while the projection has not run, so that a fused loss can still skip it."""
+        return self._out is None
+
+    @property
+    def device(self):
+        return self.input.device
 
     def size(self, dim=None):
         return self.shape if dim is None else self.shape[dim]
 
     def dim(self):
-        return 2
+        return len(self.shape)
+
+    def tensor(self) -> torch.Tensor:
+        if self._out is None:
+            self._out = self._project()
+        return self._out
 
     def __getattr__(self, name):  # argmax, float, detach, ... -> materialise
         if name.startswith('_'):
@@ -174,23 +195,16 @@ class ClsScoreHandle(_LazyHandle):
     wgmma kernel, autograd-connected, so every other consumer keeps working.
     """
 
-    def __init__(self, head: 'GSBBoxHeadWith0', x_cls: torch.Tensor):
-        self._head = head
-        self.x_cls = x_cls
-        self._logits = None
+    # the names callers read before ``input`` / ``pending``; read-only, so they never fall through to __getattr__
+    x_cls = property(lambda self: self.input)
+    _logits = property(lambda self: self._out)
 
     @property
     def shape(self):
-        return torch.Size((self.x_cls.shape[0], self._head.fc_cls.out_features))
+        return torch.Size((self.input.shape[0], self._head.fc_cls.out_features))
 
-    @property
-    def device(self):
-        return self.x_cls.device
-
-    def tensor(self) -> torch.Tensor:
-        if self._logits is None:
-            self._logits = self._head._fc_cls_logits(self.x_cls)
-        return self._logits
+    def _project(self):
+        return self._head._fc_cls_logits(self.input)
 
 
 class BoxPredHandle(_LazyHandle):
@@ -201,27 +215,31 @@ class BoxPredHandle(_LazyHandle):
     tensor attribute access) materialises that projection through ``_fc_reg``, autograd-connected.
     """
 
-    def __init__(self, head: 'NativeFcClsHead', x_reg: torch.Tensor):
-        self._head = head
-        self.x_reg = x_reg
-        self._pred = None
+    x_reg = property(lambda self: self.input)      # earlier names, as in ClsScoreHandle
+    _pred = property(lambda self: self._out)
 
     @property
     def shape(self):
-        return torch.Size((self.x_reg.shape[0], self._head.fc_reg.out_features))
+        return torch.Size((self.input.shape[0], self._head.fc_reg.out_features))
 
-    @property
-    def device(self):
-        return self.x_reg.device
-
-    def tensor(self) -> torch.Tensor:
-        if self._pred is None:
-            self._pred = self._head._fc_reg(self.x_reg)
-        return self._pred
+    def _project(self):
+        return self._head._fc_reg(self.input)
 
 
-def _as_tensor(cls_score):
-    return cls_score.tensor() if isinstance(cls_score, ClsScoreHandle) else cls_score
+def _as_tensor(x):
+    """A handle's materialised output; anything else as it is."""
+    return x.tensor() if isinstance(x, _LazyHandle) else x
+
+
+def _pending_input(x) -> Optional[torch.Tensor]:
+    """The recorded input of a handle whose projection has not run -- a fused loss can then compute from it and skip
+    the projection; None for anything else."""
+    return x.input if isinstance(x, _LazyHandle) and x.pending else None
+
+
+def _weighted(loss, loss_weight):
+    """loss * loss_weight, without the multiply (one more kernel launch) when the weight is 1."""
+    return loss if loss_weight == 1.0 else loss * loss_weight
 
 
 class FcClsFunction(torch.autograd.Function):
@@ -238,24 +256,22 @@ class FcClsFunction(torch.autograd.Function):
         b32 = None if bias is None else bias.detach().float().contiguous()
         out = ops.linear_fwd(xc, wc, b32)
         ctx.save_for_backward(xc, wc)
-        ctx.meta = (x.dtype, weight.dtype, None if bias is None else bias.dtype)
+        ops._save_param_dtypes(ctx, x, weight, bias)
         return out
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
         xc, wc = ctx.saved_tensors
-        xd, wd, bd = ctx.meta
         N, Cc = grad_out.shape
         ldd = ops.pad_cols(Cc)
         dz = torch.zeros((N, ldd), dtype=xc.dtype, device=xc.device)
         dz[:, :Cc] = grad_out
         colsum = grad_out.float().sum(0, keepdim=True)
         dW, db, dX = ops.fused_bwd(dz, xc, wc, None, ops._single_slice_tables(Cc, xc.device), colsum,
-                                   need_dw=ctx.needs_input_grad[1], need_db=ctx.needs_input_grad[2] and bd is not None,
+                                   need_dw=ctx.needs_input_grad[1], need_db=ctx.needs_input_grad[2] and ctx.has_bias,
                                    need_dx=ctx.needs_input_grad[0])
-        return (None if dX is None else dX.to(xd), None if dW is None else dW.to(wd),
-                None if db is None else db.to(bd), None)
+        return ops._grads_in_param_dtypes(ctx, dX, dW, db) + (None,)
 
 
 # --------------------------------------------------------------------------- base heads
@@ -538,12 +554,17 @@ class NativeFcClsHead(SharedFCBBoxHead):
         self.fuse_bbox_loss = bool(_cfg_get(cfg, 'fuse_bbox_loss', False))
 
     @staticmethod
-    def _cuda_index(device) -> int:
+    def _per_device(cache: Dict[int, object], device, make):
+        """``cache``'s entry for a CUDA device, keyed by its index and made by ``make(device)`` on the first call."""
         device = torch.device(device)
         if device.type != 'cuda':
             raise ops.nat.BagsNativeError(
                 'the BAGS head hot path runs on an H100 GPU only (tensor on %s); there is no CPU fallback' % device)
-        return device.index if device.index is not None else torch.cuda.current_device()
+        idx = device.index if device.index is not None else torch.cuda.current_device()
+        entry = cache.get(idx)
+        if entry is None:
+            entry = cache[idx] = make(device)
+        return entry
 
     def _active_dtype(self):
         return self.compute_dtype if self.training else self.eval_compute_dtype
@@ -585,15 +606,13 @@ class NativeFcClsHead(SharedFCBBoxHead):
     def _bbox_loss(self, bbox_pred, labels, bbox_targets, bbox_weights, reduction_override):
         """An unmaterialised ``BoxPredHandle`` with a 'mean' SmoothL1 takes the fused route (avg_factor =
         bbox_targets.size(0) from the shape); anything else the reference's op sequence on the materialised deltas."""
-        if isinstance(bbox_pred, BoxPredHandle):
-            if bbox_pred._pred is None and self._fused_bbox_loss_ok(reduction_override):
-                lb = self.loss_bbox
-                loss = ops.SmoothL1BoxFunction.apply(bbox_pred.x_reg, self.fc_reg.weight, self.fc_reg.bias, labels,
-                                                     bbox_targets, bbox_weights, float(lb.beta),
-                                                     float(bbox_targets.size(0)))[0]
-                return loss if lb.loss_weight == 1.0 else loss * lb.loss_weight
-            bbox_pred = bbox_pred.tensor()
-        return super()._bbox_loss(bbox_pred, labels, bbox_targets, bbox_weights, reduction_override)
+        x_reg = _pending_input(bbox_pred)
+        if x_reg is not None and self._fused_bbox_loss_ok(reduction_override):
+            lb = self.loss_bbox
+            loss = ops.SmoothL1BoxFunction.apply(x_reg, self.fc_reg.weight, self.fc_reg.bias, labels, bbox_targets,
+                                                 bbox_weights, float(lb.beta), float(bbox_targets.size(0)))[0]
+            return _weighted(loss, lb.loss_weight)
+        return super()._bbox_loss(_as_tensor(bbox_pred), labels, bbox_targets, bbox_weights, reduction_override)
 
     @auto_fp16()
     def forward(self, x):
@@ -697,12 +716,7 @@ class GSBBoxHeadWith0(NativeFcClsHead):
 
     # ---- device-side tables -------------------------------------------------------------
     def device_tables(self, device) -> ops.DeviceTables:
-        idx = self._cuda_index(device)
-        dt = self._device_tables.get(idx)
-        if dt is None:
-            dt = ops.DeviceTables.from_tables(self.tables, torch.device(device))
-            self._device_tables[idx] = dt
-        return dt
+        return self._per_device(self._device_tables, device, lambda d: ops.DeviceTables.from_tables(self.tables, d))
 
     # ---- label remap / sampling ---------------------------------------------------------
     def _next_seed(self) -> int:
@@ -751,47 +765,38 @@ class GSBBoxHeadWith0(NativeFcClsHead):
         if cls_score is not None:
             assert reduction_override in (None, 'none', 'mean', 'sum')
             dt = self.device_tables(labels.device)
+            x_cls = _pending_input(cls_score)
+            loss_vec = None      # stays None on the 'none' / 'sum' fallback, whose loss modules apply their loss_weight
             if (self.graph_cache and type(self)._remap_labels is GSBBoxHeadWith0._remap_labels and self.sampler == 'device'
-                    and reduction_override in (None, 'mean') and isinstance(cls_score, ClsScoreHandle)
-                    and cls_score._logits is None and torch.is_grad_enabled()):
+                    and reduction_override in (None, 'mean') and x_cls is not None and torch.is_grad_enabled()):
                 # opt-in (gs_config['graph_cache']): recurring RoI counts replay two CUDA graphs (sampler + fused forward;
                 # preparation + merged backward) instead of paying the host work of every call; new counts run eagerly first
                 if self._graph_loss is None:
                     from .api import GraphCachedHeadLoss
                     self._graph_loss = GraphCachedHeadLoss(dt, self.others_sample_ratio, compute_dtype=self.compute_dtype,
                                                            seed=self._next_seed())
-                loss_vec = self._graph_loss(cls_score.x_cls, self.fc_cls.weight, self.fc_cls.bias, labels)
+                loss_vec = self._graph_loss(x_cls, self.fc_cls.weight, self.fc_cls.bias, labels)
                 self.last_sample = None
-                for i in range(dt.G):
-                    lw = self.loss_bins[i].loss_weight
-                    losses['loss_cls_bin{}'.format(i)] = loss_vec[i] if lw == 1.0 else loss_vec[i] * lw
-                if bbox_pred is not None:
-                    losses['loss_bbox'] = self._bbox_loss(bbox_pred, labels, bbox_targets, bbox_weights, reduction_override)
-                return losses
-            wmask, avg = self._remap_labels(labels)
-            self.last_sample = (wmask, avg)
-            if reduction_override in ('none', 'sum'):
-                # per-element / summed losses (only OHEM asks for these): materialised fallback through the
-                # per-bin loss modules, the reference's own op sequence
-                z = cls_score.tensor() if isinstance(cls_score, ClsScoreHandle) else cls_score
-                preds = self._slice_preds(z)
-                for i in range(dt.G):
-                    t = dt.label2bin[i].long()[labels]
-                    losses['loss_cls_bin{}'.format(i)] = self.loss_bins[i](
-                        preds[i], t, wmask[i].float(), avg_factor=None if reduction_override == 'sum' else avg[i],
-                        reduction_override=reduction_override)
             else:
-                if isinstance(cls_score, ClsScoreHandle) and cls_score._logits is None:
-                    loss_vec = ops.GroupSoftmaxFunction.apply(
-                        cls_score.x_cls, self.fc_cls.weight, self.fc_cls.bias, labels, dt, wmask, avg,
-                        self.compute_dtype, None)
+                wmask, avg = self._remap_labels(labels)
+                self.last_sample = (wmask, avg)
+                if reduction_override in ('none', 'sum'):
+                    # per-element / summed losses (only OHEM asks for these): materialised fallback through the
+                    # per-bin loss modules, the reference's own op sequence
+                    preds = self._slice_preds(_as_tensor(cls_score))
+                    for i in range(dt.G):
+                        t = dt.label2bin[i].long()[labels]
+                        losses['loss_cls_bin{}'.format(i)] = self.loss_bins[i](
+                            preds[i], t, wmask[i].float(), avg_factor=None if reduction_override == 'sum' else avg[i],
+                            reduction_override=reduction_override)
+                elif x_cls is not None:
+                    loss_vec = ops.GroupSoftmaxFunction.apply(x_cls, self.fc_cls.weight, self.fc_cls.bias, labels, dt,
+                                                              wmask, avg, self.compute_dtype, None)
                 else:
-                    z = cls_score.tensor() if isinstance(cls_score, ClsScoreHandle) else cls_score
-                    loss_vec = ops.GroupCEFunction.apply(z, labels, dt, wmask, avg)
+                    loss_vec = ops.GroupCEFunction.apply(_as_tensor(cls_score), labels, dt, wmask, avg)
+            if loss_vec is not None:
                 for i in range(dt.G):
-                    li = loss_vec[i]
-                    lw = self.loss_bins[i].loss_weight
-                    losses['loss_cls_bin{}'.format(i)] = li if lw == 1.0 else li * lw
+                    losses['loss_cls_bin{}'.format(i)] = _weighted(loss_vec[i], self.loss_bins[i].loss_weight)
         if bbox_pred is not None:
             losses['loss_bbox'] = self._bbox_loss(bbox_pred, labels, bbox_targets, bbox_weights,
                                                   reduction_override)
@@ -801,9 +806,7 @@ class GSBBoxHeadWith0(NativeFcClsHead):
     @force_fp32(apply_to=('cls_score'))
     def _merge_score(self, cls_score):
         """[N,1236] logits -> [N,1231] scores (gs_bbox_head_with0.py:239-273), one kernel."""
-        if isinstance(cls_score, ClsScoreHandle):
-            cls_score = cls_score.tensor()
-        z = cls_score.detach()
+        z = _as_tensor(cls_score).detach()
         if z.dtype != torch.float32:
             z = z.float()
         return ops.merge_scores(z, self.device_tables(z.device))
@@ -811,8 +814,7 @@ class GSBBoxHeadWith0(NativeFcClsHead):
     @force_fp32(apply_to=('cls_score', 'bbox_pred'))
     def get_det_bboxes(self, rois, cls_score, bbox_pred, img_shape, scale_factor, rescale=False, cfg=None):
         if isinstance(cls_score, list):
-            cls_score = [c.tensor() if isinstance(c, ClsScoreHandle) else c for c in cls_score]
-            cls_score = sum(cls_score) / float(len(cls_score))
+            cls_score = sum(_as_tensor(c) for c in cls_score) / float(len(cls_score))
         scores = self._merge_score(cls_score)
         bboxes = self._decode(rois, bbox_pred, img_shape, scale_factor, rescale)
         if cfg is None:
@@ -857,11 +859,8 @@ class GSBBoxHeadWith0Reweight(GSBBoxHeadWith0):
     def _remap_labels(self, labels):
         """(wfloat [G,N] fp32, avg [G] fp32): the base class's sampled masks times the per-class weights."""
         wmask, _ = super()._remap_labels(labels)
-        dev = labels.device
-        idx = dev.index if dev.index is not None else torch.cuda.current_device()
-        if idx not in self._cls_weight_dev:
-            self._cls_weight_dev[idx] = self._cls_weight_table.to(dev)
-        return ops.reweight(labels, self.device_tables(dev), wmask, self._cls_weight_dev[idx])
+        table = self._per_device(self._cls_weight_dev, labels.device, self._cls_weight_table.to)
+        return ops.reweight(labels, self.device_tables(labels.device), wmask, table)
 
 
 class ReweightBBoxHead(NativeFcClsHead):
@@ -898,13 +897,9 @@ class ReweightBBoxHead(NativeFcClsHead):
 
     def _reweight(self, labels):
         """cls_weight[labels] (reweight_bbox_head.py:29-33), gathered on the labels' device."""
-        idx = self._cuda_index(labels.device) if labels.is_cuda else None
-        if idx is None:
+        if not labels.is_cuda:
             return self.cls_weight[labels]
-        w = self._cls_weight_dev.get(idx)
-        if w is None:
-            w = self._cls_weight_dev[idx] = self.cls_weight.to(labels.device)
-        return w[labels]
+        return self._per_device(self._cls_weight_dev, labels.device, self.cls_weight.to)[labels]
 
     def _fused_loss_ok(self) -> Optional[str]:
         """'ce' for a softmax CrossEntropyLoss, 'focal' for a sigmoid FocalLoss, both with reduction 'mean' (recognised
@@ -927,22 +922,21 @@ class ReweightBBoxHead(NativeFcClsHead):
             assert reduction_override in (None, 'none', 'mean', 'sum')
             weight = self._reweight(labels)
             kind = self._fused_loss_ok()
-            if (reduction_override in (None, 'mean') and kind is not None and isinstance(cls_score, ClsScoreHandle)
-                    and cls_score._logits is None):
+            x_cls = _pending_input(cls_score)
+            if reduction_override in (None, 'mean') and kind is not None and x_cls is not None:
                 acc = torch.empty((1,), dtype=torch.float32, device=labels.device)
                 if kind == 'focal':
                     # FocalLoss.forward: the one-hot targets' quirk, and avg_factor = N * 1231 whatever the caller passes
                     lc, N = self.loss_cls, labels.numel()
                     loss = ops.SigmoidFocalFunction.apply(
-                        cls_score.x_cls, self.fc_cls.weight, self.fc_cls.bias, focal_targets(labels, N), weight,
+                        x_cls, self.fc_cls.weight, self.fc_cls.bias, focal_targets(labels, N), weight,
                         max(float(N * FOCAL_ONE_HOT_CLASSES), 1.), float(lc.gamma), float(lc.alpha), self.compute_dtype,
                         labels, acc)[0]
                 else:
                     avg = (label_weights > 0).sum(dtype=torch.float32).clamp_min(1.0).reshape(1)
-                    loss = ops.SoftmaxCEFunction.apply(cls_score.x_cls, self.fc_cls.weight, self.fc_cls.bias, labels,
-                                                       weight, avg, self.compute_dtype, acc)[0]
-                lw = self.loss_cls.loss_weight
-                losses['loss_cls'] = loss if lw == 1.0 else loss * lw
+                    loss = ops.SoftmaxCEFunction.apply(x_cls, self.fc_cls.weight, self.fc_cls.bias, labels, weight, avg,
+                                                       self.compute_dtype, acc)[0]
+                losses['loss_cls'] = _weighted(loss, self.loss_cls.loss_weight)
                 losses['acc'] = acc
             else:
                 losses['loss_cls'] = self._cls_loss(cls_score, labels, weight, label_weights, reduction_override)

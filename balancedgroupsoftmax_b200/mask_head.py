@@ -22,7 +22,7 @@ from torch.nn.modules.utils import _pair
 
 from . import ops
 from .fp16 import auto_fp16, force_fp32
-from .head import _LazyHandle, _mmdet_core
+from .head import _LazyHandle, _as_tensor, _mmdet_core, _pending_input, _weighted
 from .losses import CrossEntropyLoss  # noqa: F401  (registers it)
 from .registry import HEADS, build_loss, register
 
@@ -80,26 +80,15 @@ class MaskPredHandle(_LazyHandle):
     any tensor attribute access, indexing or torch function) materialises them through ``conv_logits``,
     autograd-connected."""
 
-    def __init__(self, head: 'FCNMaskHead', y: torch.Tensor):
-        self._head = head
-        self.y = y
-        self._pred = None
+    y = property(lambda self: self.input)          # earlier names, as in ClsScoreHandle
+    _pred = property(lambda self: self._out)
 
     @property
     def shape(self):
-        return torch.Size((self.y.shape[0], self._head.conv_logits.out_channels) + tuple(self.y.shape[2:]))
+        return torch.Size((self.input.shape[0], self._head.conv_logits.out_channels) + tuple(self.input.shape[2:]))
 
-    @property
-    def device(self):
-        return self.y.device
-
-    def dim(self):
-        return len(self.shape)
-
-    def tensor(self) -> torch.Tensor:
-        if self._pred is None:
-            self._pred = self._head.conv_logits(self.y)
-        return self._pred
+    def _project(self):
+        return self._head.conv_logits(self.input)
 
 
 def _cfg_get(cfg, key):
@@ -274,14 +263,11 @@ class FCNMaskHead(nn.Module):
         the materialised logits."""
         if self.class_agnostic:
             labels = torch.zeros_like(labels)
-        if isinstance(mask_pred, MaskPredHandle):
-            if mask_pred._pred is None and self._fused_loss_ok():
-                lw = self.loss_mask.loss_weight
-                loss_mask = ops.MaskBCEFunction.apply(mask_pred.y, self.conv_logits.weight, self.conv_logits.bias,
-                                                      labels, mask_targets)
-                return dict(loss_mask=loss_mask if lw == 1.0 else loss_mask * lw)
-            mask_pred = mask_pred.tensor()
-        return dict(loss_mask=self.loss_mask(mask_pred, mask_targets, labels))
+        y = _pending_input(mask_pred)
+        if y is not None and self._fused_loss_ok():
+            loss_mask = ops.MaskBCEFunction.apply(y, self.conv_logits.weight, self.conv_logits.bias, labels, mask_targets)
+            return dict(loss_mask=_weighted(loss_mask, self.loss_mask.loss_weight))
+        return dict(loss_mask=self.loss_mask(_as_tensor(mask_pred), mask_targets, labels))
 
     def get_seg_masks(self, mask_pred, det_bboxes, det_labels, rcnn_test_cfg, ori_shape, scale_factor, rescale):
         """fcn_mask_head.py:125-181: masks from the label's channel (channel 0 when class-agnostic)."""

@@ -688,7 +688,7 @@ class LinearActFunction(torch.autograd.Function):
         b32 = None if bias is None else bias.detach().float().contiguous()
         y = linear_act(xc, wc, b32, bool(relu), out_dtype=out_dtype)
         ctx.relu = bool(relu)
-        ctx.meta = (x.dtype, weight.dtype, None if bias is None else bias.dtype)
+        _save_param_dtypes(ctx, x, weight, bias)
         if any(ctx.needs_input_grad[:3]):
             ctx.save_for_backward(xc, wc, y if relu else None)
         return y
@@ -697,13 +697,11 @@ class LinearActFunction(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_out):
         xc, wc, y = ctx.saved_tensors
-        xd, wd, bd = ctx.meta
         g = act_bwd(grad_out.detach(), y, xc.dtype)
         dt1 = _single_slice_tables(wc.shape[0], xc.device)
         dW, db, dX = fused_bwd(g, xc, wc, None, dt1, None, need_dw=ctx.needs_input_grad[1],
-                               need_db=ctx.needs_input_grad[2] and bd is not None, need_dx=ctx.needs_input_grad[0])
-        return (None if dX is None else dX.to(xd), None if dW is None else dW.to(wd),
-                None if db is None else db.to(bd), None, None, None)
+                               need_db=ctx.needs_input_grad[2] and ctx.has_bias, need_dx=ctx.needs_input_grad[0])
+        return _grads_in_param_dtypes(ctx, dX, dW, db) + (None, None, None)
 
 
 # --------------------------------------------------------------------------- autograd
@@ -900,6 +898,15 @@ class SigmoidFocalFunction(torch.autograd.Function):
         return _fused_loss_bwd(ctx, grad_loss) + (None,) * 8
 
 
+def _fp32_master_operands(x, weight, bias):
+    """(xc, wc, b32) of the kernels that multiply in fp32 from the fp32 master weight (box and mask losses): x stays
+    bf16 or fp32, anything else becomes fp32; the weight and the bias are fp32."""
+    xc = x if x.dtype in (torch.bfloat16, torch.float32) else x.float()
+    wc = weight if weight.dtype == torch.float32 else weight.float()
+    b32 = None if bias is None else (bias if bias.dtype == torch.float32 else bias.float())
+    return xc, wc, b32
+
+
 class SmoothL1BoxFunction(torch.autograd.Function):
     """loss[1] = SmoothL1 'mean' of the class-specific box deltas of the positive RoIs, fc_reg included
     (BBoxHead._bbox_loss on fc_reg(x) with loss_weight 1) -- only the four columns each positive RoI's loss reads:
@@ -911,9 +918,7 @@ class SmoothL1BoxFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, weight, bias, labels, targets, weights, beta, avg):
         _require_cuda(x, weight, bias, labels, targets, weights)
-        xc = x if x.dtype in (torch.bfloat16, torch.float32) else x.float()
-        wc = weight if weight.dtype == torch.float32 else weight.float()
-        b32 = None if bias is None else (bias if bias.dtype == torch.float32 else bias.float())
+        xc, wc, b32 = _fp32_master_operands(x, weight, bias)
         labels = labels.contiguous()
         loss, g, index, _ = box_fwd(xc, wc, b32, labels, targets, weights, beta, avg)
         _save_param_dtypes(ctx, x, weight, bias)
@@ -944,9 +949,7 @@ class MaskBCEFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, y, weight, bias, labels, targets):
         _require_cuda(y, weight, bias, labels, targets)
-        yc = y if y.dtype in (torch.bfloat16, torch.float32) else y.float()
-        wc = weight if weight.dtype == torch.float32 else weight.float()
-        b32 = None if bias is None else (bias if bias.dtype == torch.float32 else bias.float())
+        yc, wc, b32 = _fp32_master_operands(y, weight, bias)
         labels = labels.contiguous()
         loss, g, rsum, index = mask_fwd(yc, wc, b32, labels, targets)
         _save_param_dtypes(ctx, y, weight, bias)

@@ -190,6 +190,7 @@ def head_params(inp, kind):
 def run_mask_loss(head, inp, kind, device='cpu', dtype=torch.float32):
     """loss_mask of ``head`` on the fixture inputs and its gradients w.r.t. conv_logits.weight (FIX_ROWS of its
     [classes, Cin] view), conv_logits.bias and conv_logits' input y."""
+    from balancedgroupsoftmax_b200.mask_head import MaskPredHandle
     head.load_state_dict(head_params(inp, kind), strict=True)
     head.to(device, dtype).train()
     head.zero_grad()
@@ -205,9 +206,9 @@ def run_mask_loss(head, inp, kind, device='cpu', dtype=torch.float32):
             mask_pred = head(feats, inp['res_feat'].to(device, dtype), return_feat=False)
         else:
             mask_pred = head(feats)
-        if 'y' not in seen and hasattr(mask_pred, 'y'):     # a lazy handle: conv_logits has not run
-            seen['y'] = mask_pred.y
-            mask_pred.y.retain_grad()
+        if 'y' not in seen and isinstance(mask_pred, MaskPredHandle):     # a lazy handle: conv_logits has not run
+            seen['y'] = mask_pred.input
+            mask_pred.input.retain_grad()
         loss = head.loss(mask_pred, inp['targets'].to(device, dtype), inp['labels'].to(device))['loss_mask']
         loss.sum().backward()
     finally:

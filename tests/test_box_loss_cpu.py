@@ -138,14 +138,14 @@ def test_box_pred_handle_materialises_like_the_projection():
     want = head.fc_reg(x_reg)
     h = BoxPredHandle(head, x_reg)
     assert h.shape == (5, 4 * 1231) and h.size(1) == 4 * 1231 and h.dim() == 2 and h.device == x_reg.device
-    assert h._pred is None
+    assert h.pending and h._pred is None and h.input is x_reg and h.x_reg is x_reg
     torch.testing.assert_close(h[1:3], want[1:3])
-    assert h._pred is not None and h.tensor() is h._pred and h.tensor().requires_grad
+    assert not h.pending and h.tensor() is h._pred and h.tensor().requires_grad
     torch.testing.assert_close(torch.cat([BoxPredHandle(head, x_reg), want]), torch.cat([want, want]))
     torch.testing.assert_close(BoxPredHandle(head, x_reg).float(), want)
     # the classifier's handle keeps its own behaviour
     c = ClsScoreHandle(head, x_reg)
-    assert c.shape == (5, 1231) and c._logits is None
+    assert c.shape == (5, 1231) and c.pending and c._logits is None and c.x_cls is x_reg
     with pytest.raises(AttributeError):
         c._missing
 

@@ -264,7 +264,7 @@ def test_focal_head_fused_matches_materialised_per_element(monkeypatch, gamma, a
     calls = _count_fused_calls(monkeypatch)
     handle = ClsScoreHandle(head, x)
     out_f = head.loss(handle, None, labels, lw, None, None)
-    assert len(calls) == 1 and handle._logits is None
+    assert len(calls) == 1 and handle.pending
     head.zero_grad(set_to_none=True)
     out_f['loss_cls'].backward()
     dW_f, db_f = W.grad.double(), b.grad.double()
@@ -314,7 +314,7 @@ def test_bfocal_head_step_makes_no_host_sync(monkeypatch):
         losses['loss_cls'].backward()
     finally:
         torch.cuda.set_sync_debug_mode(0)
-    assert isinstance(cls_score, ClsScoreHandle) and cls_score._logits is None and len(calls) == 1
+    assert isinstance(cls_score, ClsScoreHandle) and cls_score.pending and len(calls) == 1
     assert head.fc_cls.weight.grad is not None
 
 

@@ -153,9 +153,9 @@ def test_head_training_matches_reference_fixture(fixture, compute_dtype):
     head = _head(inp, compute_dtype).train()
     feats = inp['feats'].cuda().requires_grad_(True)
     cls_score, bbox_pred = head(feats)
-    assert isinstance(cls_score, ClsScoreHandle) and cls_score._logits is None
+    assert isinstance(cls_score, ClsScoreHandle) and cls_score.pending
     losses = head.loss(cls_score, bbox_pred, *_targets(inp))
-    assert cls_score._logits is None                          # the fused kernel ran: no logits in memory
+    assert cls_score.pending                                  # the fused kernel ran: no logits in memory
     assert sorted(losses) == ['acc', 'loss_bbox', 'loss_cls'] and losses['acc'].shape == (1,)
     (losses['loss_cls'] + losses['loss_bbox']).backward()
     torch.cuda.synchronize()

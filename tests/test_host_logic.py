@@ -344,8 +344,8 @@ def test_cls_score_handle_works_with_torch_functions():
     x = torch.randn(5, 4)
     h = ClsScoreHandle(FakeHead(), x)
     z = FakeHead()._fc_cls_logits(x)
-    assert tuple(h.shape) == (5, 6) and h.size(1) == 6 and h.dim() == 2
-    assert torch.equal(torch.cat([h, z], 0), torch.cat([z, z], 0))
+    assert tuple(h.shape) == (5, 6) and h.size(1) == 6 and h.dim() == 2 and h.pending
+    assert torch.equal(torch.cat([h, z], 0), torch.cat([z, z], 0)) and not h.pending
     assert torch.allclose(torch.softmax(h, 1), torch.softmax(z, 1))
     assert torch.equal(h.argmax(1), z.argmax(1)) and torch.equal(h[:, 1:3], z[:, 1:3])
     assert torch.equal(torch.stack((h, h)).sum(0), 2 * z)

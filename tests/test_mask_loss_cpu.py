@@ -187,9 +187,9 @@ def test_mask_pred_handle_materialises_like_the_conv():
     want = head.conv_logits(y)
     h = MH.MaskPredHandle(head, y)
     assert h.shape == (3, 11, 14, 14) and h.size(1) == 11 and h.dim() == 4 and h.device == y.device
-    assert h._pred is None
+    assert h.pending and h._pred is None and h.input is y and h.y is y
     torch.testing.assert_close(h[1:3], want[1:3])
-    assert h._pred is not None and h.tensor() is h._pred and h.tensor().requires_grad
+    assert not h.pending and h.tensor() is h._pred and h.tensor().requires_grad
     torch.testing.assert_close(torch.cat([MH.MaskPredHandle(head, y), want]), torch.cat([want, want]))
     torch.testing.assert_close(MH.MaskPredHandle(head, y).float(), want)
 

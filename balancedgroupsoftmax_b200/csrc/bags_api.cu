@@ -21,6 +21,7 @@
 #include "bags_nms.cuh"
 #include "bags_box.cuh"
 #include "bags_mask.cuh"
+#include "bags_segm.cuh"
 
 using namespace bags;
 
@@ -1234,6 +1235,38 @@ extern "C" int bags_class_nms_dense(const float* boxes, int box_cols, const int3
   const size_t smem = static_cast<size_t>((seg + 1) & ~1) * sizeof(float4) + static_cast<size_t>(seg) * words * sizeof(uint32_t);
   BAGS_CUDA(cudaFuncSetAttribute(class_nms_dense_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   class_nms_dense_kernel<<<num_classes_fg, kNmsThreads, smem, stream>>>(boxes, box_cols, order, counts, n, iou_thr, keep, overflow);
+  BAGS_CUDA(cudaGetLastError());
+  return BAGS_OK;
+}
+
+// ----------------------------------------------------------------------------
+// test-time masks as COCO RLE (see bags_segm.cuh)
+// ----------------------------------------------------------------------------
+extern "C" int bags_segm_rle(const float* probs, int n, int mask_h, int mask_w, const int32_t* boxes_host,
+                             int32_t* boxes, int img_h, int img_w, double thr, int64_t* lengths, char* out,
+                             void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  BAGS_REQUIRE(n >= 0, "bags_segm_rle: n = %d < 0", n);
+  BAGS_REQUIRE(mask_h >= 2 && mask_w >= 2, "bags_segm_rle: mask size %d x %d: at least 2 x 2 (OpenCV resizes one-row "
+               "and one-column maps by other arithmetic)", mask_h, mask_w);
+  BAGS_REQUIRE(img_h >= 1 && img_w >= 1 && static_cast<long long>(img_h) * img_w <= 0x7fffffffLL,
+               "bags_segm_rle: canvas %d x %d must be positive and hold at most 2^31 - 1 pixels", img_h, img_w);
+  if (n == 0) return BAGS_OK;
+  BAGS_REQUIRE(probs && boxes_host && boxes && lengths, "bags_segm_rle: NULL argument");
+  for (int d = 0; d < n; ++d) {
+    const int32_t* b = boxes_host + 4 * static_cast<size_t>(d);
+    BAGS_REQUIRE(b[2] >= 1 && b[3] >= 1, "bags_segm_rle: detection %d has an empty box (w = %d, h = %d)", d, b[2], b[3]);
+    BAGS_REQUIRE(b[0] >= 0 && b[1] >= 0 && b[2] <= img_w - b[0] && b[3] <= img_h - b[1],
+                 "bags_segm_rle: detection %d's box (left %d, top %d, w %d, h %d) leaves the %d x %d canvas", d, b[0],
+                 b[1], b[2], b[3], img_h, img_w);
+  }
+  BAGS_REQUIRE((reinterpret_cast<uintptr_t>(boxes) & 15) == 0, "bags_segm_rle: boxes must be 16-byte aligned");
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  // pageable source: staged by the driver before the call returns, no wait on the device
+  BAGS_CUDA(cudaMemcpyAsync(boxes, boxes_host, 16 * static_cast<size_t>(n), cudaMemcpyHostToDevice, stream));
+  bags_segm_rle_kernel<<<n, kSegmThreads, 0, stream>>>(probs, mask_h, mask_w, reinterpret_cast<const int4*>(boxes),
+                                                       img_h, img_w, thr, reinterpret_cast<long long*>(lengths), out);
   BAGS_CUDA(cudaGetLastError());
   return BAGS_OK;
 }

@@ -15,6 +15,8 @@ Everything else -- an eval-mode ``forward``, a materialised handle, another ``lo
 """
 from __future__ import annotations
 
+import os
+
 import numpy as np
 import torch
 import torch.nn as nn
@@ -141,14 +143,49 @@ def mask_target(pos_proposals_list, pos_assigned_gt_inds_list, gt_masks_list, cf
                       zip(pos_proposals_list, pos_assigned_gt_inds_list, gt_masks_list)])
 
 
+def _paste_canvas(ori_shape, scale_factor, rescale):
+    """(img_h, img_w, scale_factor) of the image the masks are pasted into (fcn_mask_head.py:164-170)."""
+    if rescale:
+        img_h, img_w = ori_shape[:2]
+    else:
+        img_h = np.round(ori_shape[0] * scale_factor).astype(np.int32)
+        img_w = np.round(ori_shape[1] * scale_factor).astype(np.int32)
+        scale_factor = 1.0
+    return img_h, img_w, scale_factor
+
+
+def _to_host(*tensors):
+    """numpy copies of several device tensors through one device-to-host copy (one host sync)."""
+    flat = [t.contiguous().reshape(-1).view(torch.uint8) for t in tensors]
+    packed = torch.cat(flat).cpu().numpy()
+    out, at = [], 0
+    for t, f in zip(tensors, flat):
+        dtype = torch.empty((), dtype=t.dtype).numpy().dtype
+        out.append(packed[at:at + f.numel()].view(dtype).reshape(tuple(t.shape)))
+        at += f.numel()
+    return out
+
+
 def seg_masks(mask_pred, det_bboxes, det_labels, rcnn_test_cfg, ori_shape, scale_factor, rescale, num_classes,
-              channel_of_label):
+              label_channel):
     """COCO-RLE masks per class from the test-time mask logits (fcn_mask_head.py:125-239).  ``mask_pred``: [n, C, h, w]
     logits (a tensor, squashed by a sigmoid) or probabilities (an ndarray, multi-scale testing); det_labels are
-    0-based foreground labels, so class k's masks go to list k.  ``channel_of_label(label)`` picks the probability map
-    of a 1-based label.  Each detection's map is resized to its box (the box divided by ``scale_factor`` and truncated
-    to int32, at least one pixel), thresholded at ``rcnn_test_cfg.mask_thr_binary`` and pasted into an empty image of
-    the original size (``rescale``) or of the scaled size."""
+    0-based foreground labels, so class k's masks go to list k.  Each detection's probability map is the channel of its
+    1-based label (``label_channel``) or channel 0.  It is resized to its box (the box divided by ``scale_factor`` and
+    truncated to int32, at least one pixel), thresholded at ``rcnn_test_cfg.mask_thr_binary`` and pasted into an empty
+    image of the original size (``rescale``) or of the scaled size.
+
+    With detections on the GPU this runs natively (``ops.seg_masks_rle``; BAGS_SEGM_NATIVE=0 turns it off): same
+    masks, no pycocotools, three host syncs whatever n is.  A box that leaves the image takes the host loop, whose numpy
+    slicing decides what such a paste gives."""
+    on_gpu = isinstance(mask_pred, np.ndarray) or (isinstance(mask_pred, torch.Tensor) and mask_pred.is_cuda)
+    if (os.environ.get('BAGS_SEGM_NATIVE', '1') != '0' and on_gpu and isinstance(det_bboxes, torch.Tensor)
+            and det_bboxes.is_cuda):
+        boxes, labels = _to_host(det_bboxes[:, :4], det_labels)                # host sync 1
+        per_class = _seg_masks_native(mask_pred, det_labels, boxes, labels + 1, rcnn_test_cfg, ori_shape,
+                                      scale_factor, rescale, num_classes, label_channel)
+        if per_class is not None:
+            return per_class
     if isinstance(mask_pred, torch.Tensor):
         mask_pred = mask_pred.sigmoid().cpu().numpy()
     assert isinstance(mask_pred, np.ndarray)
@@ -156,20 +193,46 @@ def seg_masks(mask_pred, det_bboxes, det_labels, rcnn_test_cfg, ori_shape, scale
     per_class = [[] for _ in range(num_classes - 1)]
     boxes = det_bboxes.cpu().numpy()[:, :4]
     labels = det_labels.cpu().numpy() + 1
-    if rescale:
-        img_h, img_w = ori_shape[:2]
-    else:
-        img_h = np.round(ori_shape[0] * scale_factor).astype(np.int32)
-        img_w = np.round(ori_shape[1] * scale_factor).astype(np.int32)
-        scale_factor = 1.0
+    img_h, img_w, scale_factor = _paste_canvas(ori_shape, scale_factor, rescale)
     thr = _cfg_get(rcnn_test_cfg, 'mask_thr_binary')
     for k in range(boxes.shape[0]):
         left, top, right, bottom = (boxes[k, :] / scale_factor).astype(np.int32)
         width, height = max(right - left + 1, 1), max(bottom - top + 1, 1)
-        resized = _imresize_linear(probs[k, channel_of_label(labels[k]), :, :], (width, height))
+        resized = _imresize_linear(probs[k, labels[k] if label_channel else 0, :, :], (width, height))
         canvas = np.zeros((img_h, img_w), dtype=np.uint8)
         canvas[top:top + height, left:left + width] = (resized > thr).astype(np.uint8)
         per_class[labels[k] - 1].append(_encode_rle(canvas))
+    return per_class
+
+
+def _seg_masks_native(mask_pred, det_labels, boxes, labels, rcnn_test_cfg, ori_shape, scale_factor, rescale,
+                      num_classes, label_channel):
+    """seg_masks on the GPU, given the detections' boxes and 1-based labels on the host; None when a box leaves the
+    image or the maps have a single row or column (cv2 resizes those by other arithmetic)."""
+    if min(mask_pred.shape[-2:]) < 2:
+        return None
+    img_h, img_w, scale_factor = _paste_canvas(ori_shape, scale_factor, rescale)
+    img_h, img_w = int(img_h), int(img_w)
+    left, top, right, bottom = (boxes / scale_factor).astype(np.int32).T     # the host loop's expression, per row
+    width, height = np.maximum(right - left + 1, 1), np.maximum(bottom - top + 1, 1)
+    if ((left < 0) | (top < 0) | (left.astype(np.int64) + width > img_w) | (top.astype(np.int64) + height > img_h)).any():
+        return None
+    n = boxes.shape[0]
+    dev = det_labels.device
+    if isinstance(mask_pred, torch.Tensor):
+        # the sigmoid is elementwise: these are bitwise the host loop's probabilities, in the logits' dtype first
+        channel = det_labels + 1 if label_channel else torch.zeros_like(det_labels)
+        probs = mask_pred[torch.arange(n, device=dev), channel].sigmoid().float()
+    else:
+        channel = labels if label_channel else np.zeros_like(labels)
+        probs = torch.from_numpy(mask_pred[np.arange(n), channel].astype(np.float32)).to(dev, non_blocking=True)
+    # ``resized > thr`` compares in numpy's promoted type: float32 for a Python float, float64 for np.float64
+    thr = _cfg_get(rcnn_test_cfg, 'mask_thr_binary')
+    thr = float(np.asarray(thr).astype(np.result_type(np.float32, thr)))
+    counts = ops.seg_masks_rle(probs, np.stack([left, top, width, height], 1), img_h, img_w, thr)   # host syncs 2, 3
+    per_class = [[] for _ in range(num_classes - 1)]
+    for label, rle in zip(labels.tolist(), counts):
+        per_class[label - 1].append({'size': [img_h, img_w], 'counts': rle})
     return per_class
 
 
@@ -272,14 +335,14 @@ class FCNMaskHead(nn.Module):
     def get_seg_masks(self, mask_pred, det_bboxes, det_labels, rcnn_test_cfg, ori_shape, scale_factor, rescale):
         """fcn_mask_head.py:125-181: masks from the label's channel (channel 0 when class-agnostic)."""
         return seg_masks(mask_pred, det_bboxes, det_labels, rcnn_test_cfg, ori_shape, scale_factor, rescale,
-                         self.num_classes, (lambda label: 0) if self.class_agnostic else (lambda label: label))
+                         self.num_classes, not self.class_agnostic)
 
     def get_seg_masks_without(self, mask_pred, det_bboxes, det_labels, rcnn_test_cfg, ori_shape, scale_factor,
                               rescale):
         """fcn_mask_head.py:183-239: masks from channel 0 whatever the label (HTC's test path calls this variant,
         htc.py:419)."""
         return seg_masks(mask_pred, det_bboxes, det_labels, rcnn_test_cfg, ori_shape, scale_factor, rescale,
-                         self.num_classes, lambda label: 0)
+                         self.num_classes, False)
 
 
 class HTCMaskHead(FCNMaskHead):

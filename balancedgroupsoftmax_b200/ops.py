@@ -574,6 +574,35 @@ def multiclass_nms(multi_bboxes: torch.Tensor, multi_scores: torch.Tensor, score
     return dets, cls
 
 
+def seg_masks_rle(probs: torch.Tensor, boxes: np.ndarray, img_h: int, img_w: int, thr: float) -> list:
+    """COCO compressed RLE strings (the ``counts`` of pycocotools.mask.encode) of n test-time masks, each the map
+    ``probs[d]`` (fp32 [n, h, w] on the GPU) resized to its box as cv2.INTER_LINEAR does, thresholded with ``> thr``
+    and pasted at (left, top) into an empty ``img_h x img_w`` image (fcn_mask_head.py:160-179).  ``boxes``: int32
+    [n, 4] (left, top, w, h), each inside the image.  The comparison is in float64 against ``thr`` as given, so pass
+    ``float(np.float32(thr))`` for numpy's float32 comparison.  Two launches of bags_segm_rle and two host syncs:
+    the string lengths, then the strings."""
+    _require_cuda(probs)
+    n = int(boxes.shape[0])
+    if n == 0:
+        return []
+    dev = probs.device
+    probs = probs.float().contiguous()
+    if probs.dim() != 3 or probs.shape[0] != n:
+        raise nat.BagsNativeError('seg_masks_rle: probs must be [n, h, w] with n = %d boxes' % n)
+    boxes = np.ascontiguousarray(boxes, dtype=np.int32)
+    boxes_dev = torch.empty((n, 4), dtype=torch.int32, device=dev)
+    lengths = torch.empty((n,), dtype=torch.int64, device=dev)
+    args = (probs.data_ptr(), n, probs.shape[1], probs.shape[2], boxes.ctypes.data, boxes_dev.data_ptr(), int(img_h),
+            int(img_w), float(thr), lengths.data_ptr())
+    nat.check(nat.lib().bags_segm_rle(*args, None, _stream_ptr(dev)), 'bags_segm_rle')
+    lens = lengths.cpu().numpy()                                     # host sync: the sizes
+    ends = np.cumsum(lens)
+    out = torch.empty((max(int(ends[-1]), 1),), dtype=torch.uint8, device=dev)
+    nat.check(nat.lib().bags_segm_rle(*args, out.data_ptr(), _stream_ptr(dev)), 'bags_segm_rle')
+    data = out[:int(ends[-1])].cpu().numpy().tobytes()               # host sync: the strings
+    return [data[e - l:e] for e, l in zip(ends.tolist(), lens.tolist())]
+
+
 def gemm_probe(a, a_mn: bool, b, b_mn: bool, M: int, N: int, K: int, block_n: int = 256, splits: int = 1,
                epi: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Test hook for one wgmma GEMM (see bags_gemm_probe)."""

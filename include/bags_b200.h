@@ -30,6 +30,8 @@
  *     triggered at mmdet/core/utils/dist_utils.py:53
  *   GSBBoxHeadWith0._merge_score                          bags_merge_scores
  *     gs_bbox_head_with0.py:239-273
+ *   FCNMaskHead.get_seg_masks: resize, paste, RLE     bags_segm_rle
+ *     fcn_mask_head.py:125-239
  *   allreduce_grads / _allreduce_coalesced                bags_grad_allreduce
  *     mmdet/core/utils/dist_utils.py:9-41
  *
@@ -307,6 +309,22 @@ int bags_grad_allreduce(void* const* peer_bufs_host, void* mc_buf, long long fla
  *   class has more than 1024 candidates (its tail is dropped). */
 int bags_class_nms_dense(const float* boxes, int box_cols, const int32_t* order, const int32_t* counts,
                          int num_classes_fg, int n, float iou_thr, uint8_t* keep, int32_t* overflow, void* stream);
+
+/* Test-time masks as COCO compressed RLE -- replaces the per-detection loop of FCNMaskHead.get_seg_masks /
+ * get_seg_masks_without (fcn_mask_head.py:125-239: cv2 INTER_LINEAR resize to the box, "> thr", paste into an empty
+ * img_h x img_w image, pycocotools.mask.encode) without materialising the image:
+ *   probs     device fp32 [n, mask_h, mask_w], mask_h, mask_w >= 2: each detection's probability map (its channel)
+ *   boxes_host int32 [n, 4] (left, top, w, h): w, h >= 1 and the box inside the canvas (checked here; the caller
+ *             handles boxes that leave it); copied stream-ordered into boxes (int32 [n, 4], 16-byte aligned)
+ *   thr       a pixel is set when (double) resized > thr (pass float32(thr) for a float32 comparison)
+ *   lengths   device int64 [n]
+ *   out       NULL: the sizing pass, which writes each detection's string length to lengths[d].  Otherwise the write
+ *             pass, given the lengths of the sizing pass: it writes detection d's string (pycocotools' rleToString of
+ *             the column-major run lengths, not NUL-terminated) at out + lengths[0] + ... + lengths[d-1].
+ * The resize reproduces OpenCV's float32 INTER_LINEAR bitwise (dsize == ssize copies).  One launch per pass, no host
+ * sync; the caller reads the lengths back between the passes. */
+int bags_segm_rle(const float* probs, int n, int mask_h, int mask_w, const int32_t* boxes_host, int32_t* boxes,
+                  int img_h, int img_w, double thr, int64_t* lengths, char* out, void* stream);
 
 /* test hook: launch `blocks` x `threads` threads that wait `micros` microseconds and exit */
 int bags_debug_spin(int blocks, int threads, int micros, void* stream);

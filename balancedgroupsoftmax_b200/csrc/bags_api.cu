@@ -584,6 +584,15 @@ static int fused_fwd(const char* who, FusedLoss loss, const void* x, long long l
     BAGS_REQUIRE(colsum_tiles == (N + 127) / 128 || (N == 0 && colsum_tiles >= 1),
                  "%s: colsum must hold ceil(N/128) = %d row tiles of C floats (got %d)", who, (N + 127) / 128,
                  colsum_tiles);
+  if (N > 0) {
+    // the operands' TMA maps: rows of K elements at a row stride of ldx / ldw elements
+    const int elt = dtype == BAGS_DTYPE_BF16 ? 2 : 4;
+    BAGS_REQUIRE(ldx >= p.K && ldw >= p.K, "%s: ldx=%lld and ldw=%lld must be >= K=%d", who, ldx, ldw, p.K);
+    BAGS_REQUIRE(aligned(x, 16) && aligned(w, 16), "%s: x and W must be 16-byte aligned", who);
+    BAGS_REQUIRE((ldx * elt) % 16 == 0 && (ldw * elt) % 16 == 0,
+                 "%s: the row strides of x and W (%lld, %lld bytes) must be multiples of 16 bytes", who, ldx * elt,
+                 ldw * elt);
+  }
   if (int rc = check_clear(who, clear, clear_bytes)) return rc;
   if (int rc = make_group_table(p.gt, slices_host, G, C)) return rc;
   DeviceInfo di;

@@ -630,8 +630,12 @@ __device__ __forceinline__ void fused_fwd_body(const CUtensorMap& tmap_x, const 
           const float zt = s_zt[g * BLOCK_M + row_l];
           if (cf != 0.f) atomicAdd(&s_loss[g], cf * (lse_v - zt));
           // top-1 accuracy (a comparison, not an argmax: a tie with the row max counts as correct); the count rides
-          // the spare last slot of the per-CTA loss partials
-          if (p.acc != nullptr && g == 0 && row < p.N && zt == M) atomicAdd(&s_loss[kMaxG - 1], 1.f);
+          // the spare last slot of the per-CTA loss partials.  A label outside [0, classes) is scored against column
+          // 0 but never counts as correct (mmdet's accuracy compares the argmax with the label itself).  Only
+          // bags_ce_fwd asks for the accuracy, and it runs the WF instantiation: the byte-mask one has no label check.
+          if (p.acc != nullptr && g == 0 && row < p.N && zt == M &&
+              (!WF || (__ldg(p.labels + row) >= 0 && __ldg(p.labels + row) < p.classes)))
+            atomicAdd(&s_loss[kMaxG - 1], 1.f);
         }
         if (p.lse != nullptr && row < p.N && s_gs[g] >= n0 && s_gs[g] < n0 + BLOCK_N)
           p.lse[static_cast<long long>(row) * G + g] = lse_v;

@@ -127,7 +127,10 @@ int bags_fused_eligible(const int32_t* slices_host, int G, int C);
  * The fused kernel is launched with programmatic dependent launch: when the preceding kernel in the stream is
  * bags_sample_others / bags_mask_avg, its GEMM mainloop overlaps them and only the epilogue waits.  It is also a
  * cooperative launch of at most one 4-CTA group per 4 SMs that loops over the row tiles (no limit on N); where that
- * grid cannot be resident at once, bags_fwd returns BAGS_ERR_CUDA. */
+ * grid cannot be resident at once, bags_fwd returns BAGS_ERR_CUDA.
+ * Operands of the fused kernel (bags_fwd with logits == NULL, bags_ce_fwd, bags_focal_fwd), when N > 0: x [N, K] and
+ * W [C, K] 16-byte aligned, ldx >= K and ldw >= K, and both row strides multiples of 16 bytes (ldx, ldw % 8 == 0 for
+ * bf16, % 4 == 0 for fp32); checked before anything touches the device. */
 int bags_fwd(const void* x, long long ldx, const void* w, long long ldw, const float* bias,
              const int64_t* labels, const int32_t* label2bin, const int32_t* slices_host,
              const void* weights, int weights_dtype, const float* avg, int N, int K, int C, int G, int classes,
@@ -139,7 +142,8 @@ int bags_fwd(const void* x, long long ldx, const void* w, long long ldw, const f
  * BBoxHead.loss, bbox_head.py:97-129), logits kept on chip -- the fused kernel of bags_fwd with the single bin (0, C):
  *   loss[0] = sum_n w[n] * (logsumexp(z[n,:]) - z[n, labels[n]]) / avg[0]      (weights NULL => w = 1, avg NULL => N)
  *   acc[0]  = 100 * #{n : z[n, labels[n]] == max_c z[n, c]} / N                (optional, NULL to skip; mmdet accuracy,
- *             topk = 1.  A tie with the row maximum counts as correct.  N <= 2^24 when requested: the count is exact)
+ *             topk = 1.  A tie with the row maximum counts as correct; a label outside [0, C) never counts as correct.
+ *             N <= 2^24 when requested: the count is exact)
  * weights: fp32 [N] per-RoI weights (cls_weight[labels] for ReweightBBoxHead).
  * dz, colsum, clear, workspace: as bags_fwd (ldd % 8 == 0, colsum [ceil(N/128), C]); dW, db and dX then come from
  * bags_bwd with the single slice (0, C) and gout = dL/dloss[0].

@@ -83,9 +83,11 @@ def test_fwd_invalid_arguments_return_error_codes():
     assert lib.bags_fused_eligible(tiles, 2, 8) == 1
 
     def call(slices=tiles, l2b=base, wdt=nat.WEIGHTS_U8, N=4, K=8, dtype=nat.DTYPE_BF16, bias=None, logits=None,
-             dz=None, ldd=0, colsum=None, ntiles=0, wsb=ws, clear=None, clear_bytes=0):
-        return lib.bags_fwd(base, K, base, K, bias, base, l2b, slices, None, wdt, None, N, K, 8, 2, 4, dtype, logits,
-                            8 if logits else 0, base, None, dz, ldd, colsum, ntiles, base, wsb, clear, clear_bytes, None)
+             dz=None, ldd=0, colsum=None, ntiles=0, wsb=ws, clear=None, clear_bytes=0, x=base, ldx=None, w=base,
+             ldw=None):
+        return lib.bags_fwd(x, K if ldx is None else ldx, w, K if ldw is None else ldw, bias, base, l2b, slices, None,
+                            wdt, None, N, K, 8, 2, 4, dtype, logits, 8 if logits else 0, base, None, dz, ldd, colsum,
+                            ntiles, base, wsb, clear, clear_bytes, None)
 
     gap = nat.int32_array([0, 2, 4, 4])     # columns 2 and 3 lie in no bin
     assert lib.bags_fused_eligible(gap, 2, 8) == 0
@@ -101,9 +103,32 @@ def test_fwd_invalid_arguments_return_error_codes():
     assert call(clear=base + 4, clear_bytes=16) == -1 and b'clear' in lib.bags_last_error()
     assert call(clear=base, clear_bytes=8) == -1 and b'clear' in lib.bags_last_error()
     assert call(wsb=16) == -1 and b'workspace' in lib.bags_last_error()
+    check_fused_operand_rules(lib, 'bags_fwd', call, base)
     # the materialised route keeps the rules it shares with the fused one
     assert call(logits=base, colsum=base, ntiles=0) == -1 and b'colsum' in lib.bags_last_error()
     assert call(logits=base, clear=base + 4, clear_bytes=16) == -1 and b'clear' in lib.bags_last_error()
+
+
+def check_fused_operand_rules(lib, who, call, base):
+    """The fused route's operand rules in both operand dtypes, reported with the entry point's name before anything
+    touches a device: ldx >= K and ldw >= K, x and W 16-byte aligned, row strides whole multiples of 16 bytes.
+    ``call(dtype=, K=, x=, ldx=, w=, ldw=)`` is the entry point with otherwise valid arguments (x = W = ``base``, 16-byte
+    aligned, ldx = ldw = K by default).  Shared with test_reweight_head_cpu.py and test_focal_cpu.py."""
+    for dtype, a in ((nat.DTYPE_BF16, 8), (nat.DTYPE_F32, 4)):   # a: elements per 16 bytes
+        K = 2 * a
+        for kw in (dict(ldx=K - a), dict(ldw=K - a), dict(ldx=K - a, ldw=K - a)):
+            assert call(dtype=dtype, K=K, **kw) == -1, (dtype, kw)
+            msg = lib.bags_last_error()
+            assert who.encode() in msg and b'>= K' in msg, msg
+        for kw in (dict(ldx=K + 1), dict(ldw=K + 2), dict(ldx=K + a // 2)):   # >= K, rows not whole 16-byte pieces
+            assert call(dtype=dtype, K=K, **kw) == -1, (dtype, kw)
+            msg = lib.bags_last_error()
+            assert who.encode() in msg and b'multiples of 16 bytes' in msg, msg
+        for name in ('x', 'w'):
+            for off in (4, 8):
+                assert call(dtype=dtype, K=K, **{name: base + off}) == -1, (dtype, name, off)
+                msg = lib.bags_last_error()
+                assert who.encode() in msg and b'16-byte aligned' in msg, msg
 
 
 def test_cast_bf16_rejects_misaligned_pointers():

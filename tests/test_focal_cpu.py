@@ -23,6 +23,7 @@ import torch
 import torch.nn.functional as F
 
 import focal_oracle as FO
+from test_abi import check_fused_operand_rules
 from balancedgroupsoftmax_b200 import _native as nat
 from balancedgroupsoftmax_b200 import losses as L
 from oracle import ref_shim
@@ -200,10 +201,13 @@ def test_focal_fwd_invalid_arguments_return_error_codes():
     p = C.addressof(buf)
     ws = lib.bags_workspace_bytes()
 
+    base = (p + 15) // 16 * 16
+
     def call(N=4, K=8, C_=1231, targets=p, labels=None, loss=p, acc=None, dz=None, ldd=0, dtype=nat.DTYPE_BF16,
-             wsb=ws, norm=4 * 1231.0, x=p, colsum=None, tiles=0):
-        return lib.bags_focal_fwd(x, K, p, K, None, targets, labels, None, norm, 2.0, 0.25, N, K, C_, dtype, loss,
-                                  acc, dz, ldd, colsum, tiles, p, wsb, None, 0, None)
+             wsb=ws, norm=4 * 1231.0, x=base, colsum=None, tiles=0, ldx=None, w=base, ldw=None):
+        return lib.bags_focal_fwd(x, K if ldx is None else ldx, w, K if ldw is None else ldw, None, targets, labels,
+                                  None, norm, 2.0, 0.25, N, K, C_, dtype, loss, acc, dz, ldd, colsum, tiles, p, wsb,
+                                  None, 0, None)
 
     for c in (0, 1281):
         assert call(C_=c) == -1 and b'bad shape' in lib.bags_last_error(), c
@@ -220,6 +224,7 @@ def test_focal_fwd_invalid_arguments_return_error_codes():
     for bad in (0.0, -1.0, float('inf'), float('nan')):
         assert call(norm=bad) == -1 and b'norm' in lib.bags_last_error(), bad
     assert call(colsum=p, tiles=2) == -1 and b'colsum' in lib.bags_last_error()
+    check_fused_operand_rules(lib, 'bags_focal_fwd', call, base)
 
 
 # --------------------------------------------------------------------------- registers

@@ -18,6 +18,7 @@ import torch
 import torch.nn.functional as F
 
 import reweight_oracle as R
+from test_abi import check_fused_operand_rules
 from balancedgroupsoftmax_b200 import _native as nat
 from balancedgroupsoftmax_b200 import losses as L
 from balancedgroupsoftmax_b200 import tables as T
@@ -33,9 +34,12 @@ def test_ce_fwd_invalid_arguments_return_error_codes():
     p = C.addressof(buf)
     ws = lib.bags_workspace_bytes()
 
-    def call(N=4, K=8, C_=1231, loss=p, acc=None, dz=None, ldd=0, dtype=nat.DTYPE_BF16, wsb=ws):
-        return lib.bags_ce_fwd(p, K, p, K, None, p, None, None, N, K, C_, dtype, loss, acc, dz, ldd, None, 0, p, wsb,
-                               None, 0, None)
+    base = (p + 15) // 16 * 16
+
+    def call(N=4, K=8, C_=1231, loss=p, acc=None, dz=None, ldd=0, dtype=nat.DTYPE_BF16, wsb=ws, x=base, ldx=None, w=base,
+             ldw=None):
+        return lib.bags_ce_fwd(x, K if ldx is None else ldx, w, K if ldw is None else ldw, None, p, None, None, N, K, C_,
+                               dtype, loss, acc, dz, ldd, None, 0, p, wsb, None, 0, None)
 
     for c in (0, 1281):
         assert call(C_=c) == -1 and b'bad shape' in lib.bags_last_error(), c
@@ -45,6 +49,7 @@ def test_ce_fwd_invalid_arguments_return_error_codes():
     assert call(dz=p, ldd=1224) == -1 and b'ldd' in lib.bags_last_error()      # < C
     assert call(dtype=7) == -1 and b'dtype' in lib.bags_last_error()
     assert call(wsb=16) == -1 and b'workspace' in lib.bags_last_error()
+    check_fused_operand_rules(lib, 'bags_ce_fwd', call, base)
 
 
 def test_fused_eligibility_keeps_its_multiple_of_4_rule():

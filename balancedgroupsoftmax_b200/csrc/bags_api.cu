@@ -202,34 +202,27 @@ static cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_
 }
 
 // ----------------------------------------------------------------------------
-// GEMM launcher
+// forward GEMM launcher: out[M, N] = A[M, K] B[N, K]^T, both operands K-major
 // ----------------------------------------------------------------------------
 struct GemmArgs {
-  const void* a; long long lda; bool a_mn;
-  const void* b; long long ldb; bool b_mn;
+  const void* a; long long lda;
+  const void* b; long long ldb;
   int M, N, K;
   int dtype;
   int splits;
-  GemmParams p;  // epilogue fields pre-filled (out, ldo, bias, gscale, ...)
+  GemmParams p;  // epilogue fields pre-filled (out, ldo, bias, relu)
 };
 
-template <int BLOCK_N, bool A_MN, bool B_MN, int EPI, bool TF32, int STAGES>
-static int launch_gemm(const GemmArgs& ga, const DeviceInfo& di, cudaStream_t stream, bool pdl = false) {
-  using Cfg = GemmCfg<BLOCK_N, A_MN, B_MN, EPI, TF32, STAGES>;
-  auto kernel = bags_gemm_kernel<BLOCK_N, A_MN, B_MN, EPI, TF32, STAGES>;
+template <int BLOCK_N, int EPI, bool TF32, int STAGES>
+static int launch_gemm(const GemmArgs& ga, const DeviceInfo& di, cudaStream_t stream) {
+  using Cfg = GemmCfg<BLOCK_N, false, false, EPI, TF32, STAGES>;
+  auto kernel = bags_gemm_kernel<BLOCK_N, EPI, TF32, STAGES>;
   CUtensorMap ta, tb;
   int rc;
-  // A (an MN-major fp32 operand is read without TMA: the tensor map is still encoded, which validates alignment)
-  if (A_MN) rc = make_tmap(&ta, ga.a, ga.dtype, ga.M, ga.K, ga.lda, Cfg::SLAB, Cfg::BLOCK_K);
-  else      rc = make_tmap(&ta, ga.a, ga.dtype, ga.K, ga.M, ga.lda, Cfg::BLOCK_K, Cfg::BLOCK_M);
-  if (rc) return rc;
-  if (B_MN) rc = make_tmap(&tb, ga.b, ga.dtype, ga.N, ga.K, ga.ldb, Cfg::SLAB, Cfg::BLOCK_K);
-  else      rc = make_tmap(&tb, ga.b, ga.dtype, ga.K, ga.N, ga.ldb, Cfg::BLOCK_K, BLOCK_N);
-  if (rc) return rc;
+  if ((rc = make_tmap(&ta, ga.a, ga.dtype, ga.K, ga.M, ga.lda, Cfg::BLOCK_K, Cfg::BLOCK_M))) return rc;
+  if ((rc = make_tmap(&tb, ga.b, ga.dtype, ga.K, ga.N, ga.ldb, Cfg::BLOCK_K, BLOCK_N))) return rc;
 
   GemmParams p = ga.p;
-  p.a_ptr = static_cast<const float*>(ga.a); p.lda = ga.lda; p.a_rows = ga.M; p.a_k = ga.K;
-  p.b_ptr = static_cast<const float*>(ga.b); p.ldb = ga.ldb; p.b_rows = ga.N; p.b_k = ga.K;
   p.M = ga.M; p.N = ga.N; p.K = ga.K;
   p.num_m_tiles = (ga.M + Cfg::BLOCK_M - 1) / Cfg::BLOCK_M;
   p.num_n_tiles = (ga.N + BLOCK_N - 1) / BLOCK_N;
@@ -243,15 +236,8 @@ static int launch_gemm(const GemmArgs& ga, const DeviceInfo& di, cudaStream_t st
   const int grid = units < di.num_sms ? units : di.num_sms;
 
   BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, pdl, false, ta, tb, p));
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(Cfg::NUM_THREADS), Cfg::SMEM_BYTES, stream, false, false, ta, tb, p));
   return BAGS_OK;
-}
-
-static int pick_splits(int tiles, int kblocks, int num_sms) {
-  int s = num_sms / (tiles > 0 ? tiles : 1);
-  if (s < 1) s = 1;
-  if (s > kblocks) s = kblocks;
-  return s;
 }
 
 // ----------------------------------------------------------------------------
@@ -283,14 +269,14 @@ extern "C" int bags_linear_act_fwd(const void* x, long long ldx, const void* w, 
     BAGS_REQUIRE((reinterpret_cast<uintptr_t>(out) & 15) == 0, "bags_linear_act_fwd: out must be 16-byte aligned");
   }
   GemmArgs ga{};
-  ga.a = x; ga.lda = ldx; ga.a_mn = false;
-  ga.b = w; ga.ldb = ldw; ga.b_mn = false;
+  ga.a = x; ga.lda = ldx;
+  ga.b = w; ga.ldb = ldw;
   ga.M = N; ga.N = C; ga.K = K; ga.dtype = dtype; ga.splits = 1;
   ga.p.out = out; ga.p.ldo = ldo; ga.p.bias = bias; ga.p.relu = relu ? 1 : 0;
   if (dtype == BAGS_DTYPE_BF16)
-    return out_dtype == BAGS_DTYPE_BF16 ? launch_gemm<256, false, false, EPI_STORE_BF16, false, 4>(ga, di, stream)
-                                        : launch_gemm<256, false, false, EPI_STORE_F32, false, 4>(ga, di, stream);
-  return launch_gemm<256, false, false, EPI_STORE_F32, true, 4>(ga, di, stream);
+    return out_dtype == BAGS_DTYPE_BF16 ? launch_gemm<256, EPI_STORE_BF16, false, 4>(ga, di, stream)
+                                        : launch_gemm<256, EPI_STORE_F32, false, 4>(ga, di, stream);
+  return launch_gemm<256, EPI_STORE_F32, true, 4>(ga, di, stream);
 }
 
 // Split-K factor worth using for a forward layer (1 = the single-pass kernel): few output tiles and a long contraction --
@@ -324,12 +310,12 @@ extern "C" int bags_linear_act_fwd_splitk(const void* x, long long ldx, const vo
   if (int rc = device_info(di)) return rc;
   BAGS_CUDA(cudaMemsetAsync(ws, 0, sizeof(float) * static_cast<size_t>(N) * static_cast<size_t>(ldws), stream));
   GemmArgs ga{};
-  ga.a = x; ga.lda = ldx; ga.a_mn = false;
-  ga.b = w; ga.ldb = ldw; ga.b_mn = false;
+  ga.a = x; ga.lda = ldx;
+  ga.b = w; ga.ldb = ldw;
   ga.M = N; ga.N = C; ga.K = K; ga.dtype = dtype; ga.splits = splits;
   ga.p.out = ws; ga.p.ldo = ldws;
-  int rc = (dtype == BAGS_DTYPE_BF16) ? launch_gemm<256, false, false, EPI_RED_F32, false, 4>(ga, di, stream)
-                                      : launch_gemm<256, false, false, EPI_RED_F32, true, 4>(ga, di, stream);
+  int rc = (dtype == BAGS_DTYPE_BF16) ? launch_gemm<256, EPI_RED_F32, false, 4>(ga, di, stream)
+                                      : launch_gemm<256, EPI_RED_F32, true, 4>(ga, di, stream);
   if (rc) return rc;
   const long long quads = static_cast<long long>(N) * ((C + 3) / 4);
   long long grid = (quads + 255) / 256;
@@ -933,32 +919,6 @@ scale_colsum_kernel(const float* __restrict__ colsum, int tiles, float* __restri
 }
 
 
-template <bool TF32>
-static int launch_bwd_merged(const void* dz, long long ldd, const void* x, long long ldx, const void* w, const void* wb,
-                             long long ldw, const BwdMergedParams& bp, const DeviceInfo& di, cudaStream_t stream) {
-  using CW = BwdDwCfg<TF32>;
-  using CX = BwdDxCfg<TF32>;
-  const int dtype = TF32 ? BAGS_DTYPE_F32 : BAGS_DTYPE_BF16;
-  const int C = bp.dw.M, K = bp.dw.N, N = bp.dw.K;
-  CUtensorMap t_dzT, t_xT, t_dz, t_w, t_wp;
-  int rc;
-  if ((rc = make_tmap(&t_dzT, dz, dtype, C, N, ldd, CW::SLAB, CW::BLOCK_K))) return rc;   // dW: A = dz^T
-  if ((rc = make_tmap(&t_xT, x, dtype, K, N, ldx, CW::SLAB, CW::BLOCK_K))) return rc;     // dW: B = x^T
-  if ((rc = make_tmap(&t_dz, dz, dtype, C, N, ldd, CX::BLOCK_K, CX::BLOCK_M))) return rc;  // dX: A = dz
-  if ((rc = make_tmap(&t_w, w, dtype, K, C, ldw, CX::SLAB, CX::BLOCK_K))) return rc;      // dX: B = W^T
-  if ((rc = make_tmap(&t_wp, wb, dtype, K, C, ldw, CX::SLAB, CX::BLOCK_K))) return rc;    // dX: B = W'^T
-  CUtensorMap t_dx = t_dz;   // (unused unless bp.dx_tma)
-  if (bp.dx_tma && (rc = make_tmap(&t_dx, bp.dx.out, dtype, K, N, bp.dx.ldo, 64, 64))) return rc;   // dX store boxes
-  auto kernel = bags_bwd_merged_kernel<TF32>;
-  constexpr int smem = bwd_merged_smem_bytes<TF32>();
-  BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  const int units = bp.dw_units + bp.dx_units;
-  const int grid = units < di.num_sms ? units : di.num_sms;
-  BAGS_CUDA(launch(kernel, dim3(grid), dim3(CW::NUM_THREADS), smem, stream, true, false, t_dzT, t_xT, t_dz, t_w, t_wp,
-                   t_dx, bp));
-  return BAGS_OK;
-}
-
 // Split-K factor of the merged backward's dW units.  The kernel deals its work list (dW units split-major, then the
 // dX units) round-robin to min(units, SMs) CTAs, and a CTA runs its units back to back, so the backward ends with the
 // CTA that holds the most work.  The cost of a split factor is exactly that: the largest sum over one CTA's units of
@@ -1003,6 +963,66 @@ extern "C" size_t bags_bwd_scratch_bytes(int C, long long ldw, int dtype) {
   return wprime_bytes(C, ldw, dtype) + static_cast<size_t>(kColsumTiles) * C * sizeof(float);
 }
 
+// One launch of bags_bwd_merged_kernel over the problems asked for through p.dw.out and p.dx.out:
+//   dW[C, K] += rowscale(c) * dz^T x   split-K reduce-add, `splits` partials (< 1: merged_dw_splits)
+//   dX[N, K]  = dz wb                  wb = W' (the preparation kernel's scaled copy) or W
+// The caller fills the epilogue fields of p.dw (out, ldo, gscale, groups, colsum) and p.dx (out, ldo), and gout, G,
+// uniform_ok, inputs_ready and wprime_prepared; this fills the shapes, tilings and operands.  Only the tensor maps of
+// the problems present are encoded (the others stay zero), so x is not read without dW, nor w and wb without dX.
+template <bool TF32>
+static int launch_bwd_merged(const void* dz, long long ldd, const void* x, long long ldx, const void* w, const void* wb,
+                             long long ldw, int N, int K, int C, int splits, BwdMergedParams p, const DeviceInfo& di,
+                             cudaStream_t stream) {
+  using CW = BwdDwCfg<TF32>;
+  using CX = BwdDxCfg<TF32>;
+  const int dtype = TF32 ? BAGS_DTYPE_F32 : BAGS_DTYPE_BF16;
+  CUtensorMap t_dzT{}, t_xT{}, t_dz{}, t_w{}, t_wp{}, t_dx{};
+  int rc;
+  GemmParams& px = p.dx;
+  if (px.out != nullptr) {
+    px.M = N; px.N = K; px.K = C;
+    px.num_m_tiles = (N + CX::BLOCK_M - 1) / CX::BLOCK_M;
+    px.num_n_tiles = (K + CX::BLOCK_N_ - 1) / CX::BLOCK_N_;
+    px.kblocks_total = (C + CX::BLOCK_K - 1) / CX::BLOCK_K;
+    px.num_splits = 1;
+    px.b_ptr = static_cast<const float*>(wb); px.ldb = ldw; px.b_rows = K; px.b_k = C;
+    p.w = static_cast<const float*>(w);
+    p.dx_units = px.num_m_tiles * px.num_n_tiles;
+    // TMA-stored bf16 dX: a store box writes whole 16-byte pieces at the right edge, so K must end on one
+    p.dx_tma = (!TF32 && (K % 8) == 0 && (px.ldo % 8) == 0) ? 1 : 0;
+    if ((rc = make_tmap(&t_dz, dz, dtype, C, N, ldd, CX::BLOCK_K, CX::BLOCK_M))) return rc;   // A = dz
+    if ((rc = make_tmap(&t_w, w, dtype, K, C, ldw, CX::SLAB, CX::BLOCK_K))) return rc;       // B = W^T
+    if ((rc = make_tmap(&t_wp, wb, dtype, K, C, ldw, CX::SLAB, CX::BLOCK_K))) return rc;     // B = W'^T
+    if (p.dx_tma && (rc = make_tmap(&t_dx, px.out, dtype, K, N, px.ldo, 64, 64))) return rc;  // dX store boxes
+  }
+  GemmParams& pw = p.dw;
+  if (pw.out != nullptr) {
+    pw.M = C; pw.N = K; pw.K = N;
+    pw.num_m_tiles = (C + CW::BLOCK_M - 1) / CW::BLOCK_M;
+    pw.num_n_tiles = (K + CW::BLOCK_N_ - 1) / CW::BLOCK_N_;
+    pw.kblocks_total = (N + CW::BLOCK_K - 1) / CW::BLOCK_K;
+    const int dw_tiles = pw.num_m_tiles * pw.num_n_tiles;
+    if (splits < 1) splits = merged_dw_splits(dw_tiles, pw.kblocks_total, p.dx_units, px.kblocks_total, di.num_sms);
+    if (splits > pw.kblocks_total) splits = pw.kblocks_total;
+    pw.num_splits = splits;
+    pw.a_ptr = static_cast<const float*>(dz); pw.lda = ldd; pw.a_rows = C; pw.a_k = N;
+    pw.b_ptr = static_cast<const float*>(x); pw.ldb = ldx; pw.b_rows = K; pw.b_k = N;
+    p.dw_units = dw_tiles * splits;
+    if ((rc = make_tmap(&t_dzT, dz, dtype, C, N, ldd, CW::SLAB, CW::BLOCK_K))) return rc;   // A = dz^T
+    if ((rc = make_tmap(&t_xT, x, dtype, K, N, ldx, CW::SLAB, CW::BLOCK_K))) return rc;     // B = x^T
+  }
+  p.timing = g_timing ? g_timing + 1024 * 8 : nullptr;   // rows [1024, 1024 + 2 grid)
+  const int units = p.dw_units + p.dx_units;
+  if (units == 0) return BAGS_OK;
+  auto kernel = bags_bwd_merged_kernel<TF32>;
+  constexpr int smem = bwd_merged_smem_bytes<TF32>();
+  BAGS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  const int grid = units < di.num_sms ? units : di.num_sms;
+  BAGS_CUDA(launch(kernel, dim3(grid), dim3(CW::NUM_THREADS), smem, stream, true, false, t_dzT, t_xT, t_dz, t_w, t_wp,
+                   t_dx, p));
+  return BAGS_OK;
+}
+
 extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long ldx, const void* w,
                         long long ldw, const float* gout, const int32_t* slices_host,
                         const float* colsum, int colsum_tiles, float* dW, long long lddw, float* db, void* dX,
@@ -1015,40 +1035,46 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
   BAGS_REQUIRE(N >= 0 && K >= 1 && C >= 1, "bags_bwd: bad shape");
   GroupTable gt;
   if (int rc = make_group_table(gt, slices_host, G, C)) return rc;
-  DeviceInfo di;
-  if (int rc = device_info(di)) return rc;
   const bool bf = dtype == BAGS_DTYPE_BF16;
   const int vecw = bf ? 8 : 4;
 
   const bool want_scale = (dX != nullptr && N > 0 && gout != nullptr);
   const bool want_colpart = (db != nullptr && colsum == nullptr && N > 0);
-  if (db != nullptr && colsum == nullptr && N == 0) {   // no rows: zero bias gradient
-    BAGS_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * C, stream));
-    db = nullptr;
-  }
   if (want_scale || want_colpart) {
     BAGS_REQUIRE(wscratch != nullptr && wscratch_bytes >= bags_bwd_scratch_bytes(C, ldw, dtype),
                  "bags_bwd: wscratch must provide bags_bwd_scratch_bytes() = %zu bytes (got %zu)",
                  bags_bwd_scratch_bytes(C, ldw, dtype), wscratch_bytes);
     BAGS_REQUIRE((reinterpret_cast<uintptr_t>(wscratch) & 255) == 0, "bags_bwd: wscratch must be 256-byte aligned");
   }
-  float* colpart = (wscratch == nullptr) ? nullptr
-                   : reinterpret_cast<float*>(reinterpret_cast<char*>(wscratch) + wprime_bytes(C, ldw, dtype));
-  if (dW != nullptr)
-    BAGS_REQUIRE((x != nullptr || N == 0) && lddw >= K && (lddw % 4) == 0 && (K % 4) == 0 &&
-                     (reinterpret_cast<uintptr_t>(dW) & 15) == 0,
+  if (dW != nullptr) {
+    BAGS_REQUIRE(x != nullptr || N == 0, "bags_bwd: x is NULL but dW requested");
+    BAGS_REQUIRE(lddw >= K && (lddw % 4) == 0 && (K % 4) == 0 && (reinterpret_cast<uintptr_t>(dW) & 15) == 0,
                  "bags_bwd: dW must be 16-byte aligned with K and lddw multiples of 4");
+  }
+  if (dX != nullptr && N > 0) {
+    BAGS_REQUIRE(w != nullptr, "bags_bwd: w is NULL but dX requested");
+    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(dX) & 15) == 0, "bags_bwd: dX not 16-byte aligned");
+  }
   if (want_scale)
-    BAGS_REQUIRE(w != nullptr && (K % vecw) == 0 && (ldw % vecw) == 0 && (reinterpret_cast<uintptr_t>(w) & 15) == 0,
+    BAGS_REQUIRE((K % vecw) == 0 && (ldw % vecw) == 0 && (reinterpret_cast<uintptr_t>(w) & 15) == 0,
                  "bags_bwd: w must be 16-byte aligned with K and ldw multiples of %d", vecw);
   if (want_colpart)
     BAGS_REQUIRE(((ldd * (bf ? 2 : 4)) % 16) == 0 && (reinterpret_cast<uintptr_t>(dz) & 15) == 0,
                  "bags_bwd: dz rows must be 16-byte aligned");
+  BAGS_REQUIRE(db == nullptr || colsum == nullptr || colsum_tiles >= 1,
+               "bags_bwd: db requested from colsum with colsum_tiles = %d < 1", colsum_tiles);
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
 
-  // ---- preparation (one small kernel): zero dW, W' = gout-scaled W, bias-gradient partial column sums; then both
-  // contractions in one merged launch, or the one requested as a plain split-K dW (red.add) / dX GEMM ----
-  // both contractions requested: one merged persistent launch after the preparation kernel (see bags_bwd_merged_kernel)
-  const bool merged = dW != nullptr && dX != nullptr && N > 0 && env_int("BAGS_BWD_MERGED", 1);
+  if (db != nullptr && colsum == nullptr && N == 0) {   // no rows: zero bias gradient
+    BAGS_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * C, stream));
+    db = nullptr;
+  }
+  float* colpart = (wscratch == nullptr) ? nullptr
+                   : reinterpret_cast<float*>(reinterpret_cast<char*>(wscratch) + wprime_bytes(C, ldw, dtype));
+
+  // ---- preparation (one small kernel): zero dW, W' = gout-scaled W, bias-gradient partial column sums; then the
+  // requested contractions in one merged launch (see bags_bwd_merged_kernel) ----
   // a dz column outside every bin is scaled by 0 when gout is given: the merged kernel's uniform-gout shortcut (dz W,
   // output scaled by gout[0]) would scale it by gout[0], so it is taken only when the bins tile [0, C)
   const bool no_gaps = bins_tile(slices_host, G, C);
@@ -1061,7 +1087,7 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
     pp.z_ctas = (dW != nullptr && !prezeroed) ? di.num_sms : 0;
     pp.s_ctas = want_scale ? di.num_sms : 0;
     pp.c_ctas = want_colpart ? ((C + 63) / 64) * kColsumTiles : 0;
-    pp.skip_scale_if_uniform = (merged && no_gaps) ? 1 : 0;   // the merged kernel reads W itself (see bp.uniform_ok)
+    pp.skip_scale_if_uniform = no_gaps ? 1 : 0;   // the merged kernel reads W itself (see bp.uniform_ok)
     pp.timing = g_timing ? g_timing + 2048 * 8 : nullptr;       // rows [2048, 4096)
     const int grid = pp.z_ctas + pp.s_ctas + pp.c_ctas;
     if (grid > 0) {
@@ -1071,91 +1097,32 @@ extern "C" int bags_bwd(const void* dz, long long ldd, const void* x, long long 
   }
   const float* cs_in = (colsum != nullptr) ? colsum : colpart;
   const int cs_tiles = (colsum != nullptr) ? colsum_tiles : kColsumTiles;
-  if (db != nullptr) BAGS_REQUIRE(cs_in != nullptr && cs_tiles >= 1, "bags_bwd: db requested but no column sums available");
+  if (db != nullptr && !(dW != nullptr && N > 0)) {   // (with dW units, their epilogue writes db)
+    scale_colsum_kernel<<<(C + 255) / 256, 256, 0, stream>>>(cs_in, cs_tiles, db, C, gt, gout);
+    BAGS_CUDA(cudaGetLastError());
+  }
+  if (N == 0 || (dW == nullptr && dX == nullptr)) return BAGS_OK;
 
-  if (merged) {
-    BAGS_REQUIRE(w != nullptr && x != nullptr, "bags_bwd: w / x is NULL but dW and dX requested");
-    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(dX) & 15) == 0, "bags_bwd: dX not 16-byte aligned");
-    const int bk = bf ? 64 : 32;
-    BwdMergedParams bp{};
+  BwdMergedParams bp{};
+  if (dW != nullptr) {
     GemmParams& pw = bp.dw;
-    pw.M = C; pw.N = K; pw.K = N;
-    pw.num_m_tiles = (C + 127) / 128; pw.num_n_tiles = (K + 255) / 256; pw.kblocks_total = (N + bk - 1) / bk;
-    GemmParams& px = bp.dx;
-    px.M = N; px.N = K; px.K = C;
-    px.num_m_tiles = (N + 127) / 128; px.num_n_tiles = (K + 255) / 256; px.kblocks_total = (C + bk - 1) / bk;
-    px.num_splits = 1;
-    const int dw_tiles = pw.num_m_tiles * pw.num_n_tiles, dx_units = px.num_m_tiles * px.num_n_tiles;
-    int splits = merged_dw_splits(dw_tiles, pw.kblocks_total, dx_units, px.kblocks_total, di.num_sms);
-    splits = env_int("BAGS_DW_SPLITS", splits);
-    if (splits < 1) splits = 1;
-    if (splits > pw.kblocks_total) splits = pw.kblocks_total;
-    pw.num_splits = splits;
     pw.out = dW; pw.ldo = lddw;
     pw.gscale = gout; pw.G = (gout != nullptr) ? gt.G : 0;
     for (int g = 0; g < kMaxGroups; ++g) { pw.gstart[g] = gt.start[g]; pw.glen[g] = gt.len[g]; }
     pw.colsum_in = (db != nullptr) ? cs_in : nullptr;
     pw.colsum_tiles = cs_tiles;
     pw.colsum_out = db;
-    pw.a_ptr = static_cast<const float*>(dz); pw.lda = ldd; pw.a_rows = C; pw.a_k = N;
-    pw.b_ptr = static_cast<const float*>(x); pw.ldb = ldx; pw.b_rows = K; pw.b_k = N;
-    const void* wb = want_scale ? wscratch : w;
-    px.out = dX; px.ldo = lddx;
-    px.b_ptr = static_cast<const float*>(wb); px.ldb = ldw; px.b_rows = K; px.b_k = C;
-    bp.dw_units = pw.num_m_tiles * pw.num_n_tiles * splits;
-    bp.dx_units = px.num_m_tiles * px.num_n_tiles;
-    bp.w = static_cast<const float*>(w);
-    bp.gout = gout;
-    bp.G = gt.G;
-    bp.uniform_ok = no_gaps ? 1 : 0;
-    bp.inputs_ready = prep_launched ? 1 : 0;
-    bp.wprime_prepared = want_scale ? 1 : 0;
-    // TMA-stored bf16 dX: a store box writes whole 16-byte pieces at the right edge, so K must end on one
-    bp.dx_tma = (bf && (K % 8) == 0 && (lddx % 8) == 0) ? 1 : 0;
-    bp.timing = g_timing ? g_timing + 1024 * 8 : nullptr;   // rows [1024, 1024 + 2 grid)
-    return bf ? launch_bwd_merged<false>(dz, ldd, x, ldx, w, wb, ldw, bp, di, stream)
-              : launch_bwd_merged<true>(dz, ldd, x, ldx, w, wb, ldw, bp, di, stream);
   }
-
-  if (dW != nullptr && N > 0) {
-    GemmArgs ga{};
-    ga.a = dz; ga.lda = ldd; ga.a_mn = true;   // A = dz^T : [C, N_roi], stored [N_roi, C]
-    ga.b = x;  ga.ldb = ldx; ga.b_mn = true;   // B = x^T  : [K, N_roi], stored [N_roi, K]
-    ga.M = C; ga.N = K; ga.K = N; ga.dtype = dtype;
-    const int tiles = ((C + 127) / 128) * ((K + 255) / 256);
-    const int kblocks = (N + (bf ? 63 : 31)) / (bf ? 64 : 32);
-    ga.splits = env_int("BAGS_DW_SPLITS", pick_splits(tiles, kblocks, di.num_sms));
-    ga.p.out = dW; ga.p.ldo = lddw; ga.p.bias = nullptr;
-    ga.p.gscale = gout; ga.p.G = (gout != nullptr) ? gt.G : 0;
-    for (int g = 0; g < kMaxGroups; ++g) { ga.p.gstart[g] = gt.start[g]; ga.p.glen[g] = gt.len[g]; }
-    ga.p.colsum_in = (db != nullptr) ? cs_in : nullptr;
-    ga.p.colsum_tiles = cs_tiles;
-    ga.p.colsum_out = (db != nullptr) ? db : nullptr;
-    ga.p.pdl_wait_epilogue = 1;   // dW zeroing + column-sum partials come from bwd_prep; the mainloop overlaps it
-    ga.p.pdl_wait_producer = prep_launched ? 0 : 1;   // no preparation kernel in between: dz comes from the preceding kernel
-    int rc = bf ? launch_gemm<256, true, true, EPI_RED_F32, false, 4>(ga, di, stream, true)
-                : launch_gemm<256, true, true, EPI_RED_F32, true, 4>(ga, di, stream, true);
-    if (rc) return rc;
-  } else if (db != nullptr) {
-    scale_colsum_kernel<<<(C + 255) / 256, 256, 0, stream>>>(cs_in, cs_tiles, db, C, gt, gout);
-    BAGS_CUDA(cudaGetLastError());
-  }
-
-  if (dX != nullptr && N > 0) {
-    BAGS_REQUIRE(w != nullptr, "bags_bwd: w is NULL but dX requested");
-    BAGS_REQUIRE((reinterpret_cast<uintptr_t>(dX) & 15) == 0, "bags_bwd: dX not 16-byte aligned");
-    GemmArgs ga{};
-    ga.a = dz; ga.lda = ldd; ga.a_mn = false;                 // A = dz : [N_roi, C]
-    ga.b = want_scale ? wscratch : w; ga.ldb = ldw; ga.b_mn = true;   // B = W'^T: [K, C], stored [C, K]
-    ga.M = N; ga.N = K; ga.K = C; ga.dtype = dtype; ga.splits = 1;
-    ga.p.out = dX; ga.p.ldo = lddx; ga.p.bias = nullptr; ga.p.gscale = nullptr; ga.p.G = 0;
-    ga.p.colsum_in = nullptr; ga.p.colsum_out = nullptr;
-    ga.p.pdl_wait_producer = 1;   // W' is produced by bwd_prep (two kernels back; the chain of waits covers it)
-    int rc = bf ? launch_gemm<256, false, true, EPI_STORE_BF16, false, 4>(ga, di, stream, true)
-                : launch_gemm<256, false, true, EPI_STORE_F32, true, 4>(ga, di, stream, true);
-    if (rc) return rc;
-  }
-  return BAGS_OK;
+  bp.dx.out = dX; bp.dx.ldo = lddx;
+  bp.gout = (dX != nullptr) ? gout : nullptr;
+  bp.G = gt.G;
+  bp.uniform_ok = no_gaps ? 1 : 0;
+  bp.inputs_ready = prep_launched ? 1 : 0;
+  bp.wprime_prepared = want_scale ? 1 : 0;
+  const void* wb = want_scale ? wscratch : w;
+  const int splits = env_int("BAGS_DW_SPLITS", 0);   // a forced dW split count; unset: merged_dw_splits
+  return bf ? launch_bwd_merged<false>(dz, ldd, x, ldx, w, wb, ldw, N, K, C, splits, bp, di, stream)
+            : launch_bwd_merged<true>(dz, ldd, x, ldx, w, wb, ldw, N, K, C, splits, bp, di, stream);
 }
 
 // ----------------------------------------------------------------------------
@@ -1346,26 +1313,35 @@ extern "C" int bags_gemm_probe(const void* a, long long lda, int a_mn, const voi
                                int block_n, int splits, int epi, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   BAGS_REQUIRE(a && b && out, "bags_gemm_probe: NULL argument");
-  DeviceInfo di;
-  if (int rc = device_info(di)) return rc;
-  GemmArgs ga{};
-  ga.a = a; ga.lda = lda; ga.a_mn = a_mn != 0;
-  ga.b = b; ga.ldb = ldb; ga.b_mn = b_mn != 0;
-  ga.M = M; ga.N = N; ga.K = K; ga.dtype = dtype; ga.splits = splits;
-  ga.p.out = out; ga.p.ldo = ldo; ga.p.bias = nullptr; ga.p.gscale = nullptr; ga.p.G = 0;
-  ga.p.colsum_in = nullptr; ga.p.colsum_out = nullptr;
   const bool bf = dtype == BAGS_DTYPE_BF16;
   BAGS_REQUIRE(bf || dtype == BAGS_DTYPE_F32, "bags_gemm_probe: bad dtype");
-  // the instantiations the product uses
-  if (!a_mn && !b_mn && epi == 0 && block_n == 256)
-    return bf ? launch_gemm<256, false, false, EPI_STORE_F32, false, 4>(ga, di, stream)
-              : launch_gemm<256, false, false, EPI_STORE_F32, true, 4>(ga, di, stream);
-  if (!a_mn && b_mn && block_n == 256 && ((bf && epi == 1) || (!bf && epi == 0)))
-    return bf ? launch_gemm<256, false, true, EPI_STORE_BF16, false, 4>(ga, di, stream)
-              : launch_gemm<256, false, true, EPI_STORE_F32, true, 4>(ga, di, stream);
-  if (a_mn && b_mn && block_n == 256 && epi == 2)
-    return bf ? launch_gemm<256, true, true, EPI_RED_F32, false, 4>(ga, di, stream)
-              : launch_gemm<256, true, true, EPI_RED_F32, true, 4>(ga, di, stream);
-  return fail(BAGS_ERR_INVALID, "bags_gemm_probe: configuration a_mn=%d b_mn=%d block_n=%d epi=%d dtype=%d not instantiated",
-              a_mn, b_mn, block_n, epi, dtype);
+  // the kernels the product runs: kk the forward GEMM, kmn the merged backward's dX units alone (a = dz [M, K],
+  // b = W [K, N]), mnmn its split-K dW units alone (a = dz [K, M], b = x [K, N])
+  const bool kk = !a_mn && !b_mn && epi == 0, kmn = !a_mn && b_mn && epi == (bf ? 1 : 0);
+  const bool mnmn = a_mn && b_mn && epi == 2;
+  BAGS_REQUIRE(block_n == 256 && (kk || kmn || mnmn),
+               "bags_gemm_probe: configuration a_mn=%d b_mn=%d block_n=%d epi=%d dtype=%d not instantiated", a_mn, b_mn,
+               block_n, epi, dtype);
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  if (kk) {
+    GemmArgs ga{};
+    ga.a = a; ga.lda = lda;
+    ga.b = b; ga.ldb = ldb;
+    ga.M = M; ga.N = N; ga.K = K; ga.dtype = dtype; ga.splits = 1;
+    ga.p.out = out; ga.p.ldo = ldo;
+    return bf ? launch_gemm<256, EPI_STORE_F32, false, 4>(ga, di, stream)
+              : launch_gemm<256, EPI_STORE_F32, true, 4>(ga, di, stream);
+  }
+  // in bags_bwd's terms: kmn has M RoIs, N features and K logits; mnmn has K RoIs, N features and M logits
+  BwdMergedParams bp{};
+  if (kmn) {
+    bp.dx.out = out; bp.dx.ldo = ldo;
+    return bf ? launch_bwd_merged<false>(a, lda, nullptr, 0, b, b, ldb, M, N, K, 0, bp, di, stream)
+              : launch_bwd_merged<true>(a, lda, nullptr, 0, b, b, ldb, M, N, K, 0, bp, di, stream);
+  }
+  bp.dw.out = out; bp.dw.ldo = ldo;
+  if (splits < 1) splits = 1;
+  return bf ? launch_bwd_merged<false>(a, lda, b, ldb, nullptr, nullptr, 0, K, N, M, splits, bp, di, stream)
+            : launch_bwd_merged<true>(a, lda, b, ldb, nullptr, nullptr, 0, K, N, M, splits, bp, di, stream);
 }

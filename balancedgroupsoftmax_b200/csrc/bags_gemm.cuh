@@ -7,9 +7,9 @@
 // index strided).  That covers the three contractions of the BAGS head without
 // any transposed copies in HBM:
 //
-//   forward  z  = X  W^T  : A = X   [N_roi,K]  K-major , B = W   [C,K]      K-major
-//   backward dX = dz W    : A = dz  [N_roi,C]  K-major , B = W   [C,K]      MN-major
-//   backward dW = dz^T X  : A = dz  [N_roi,C]  MN-major, B = X   [N_roi,K]  MN-major
+//   forward  z  = X  W^T  : A = X   [N_roi,K]  K-major , B = W   [C,K]      K-major   (bags_gemm_kernel)
+//   backward dX = dz W    : A = dz  [N_roi,C]  K-major , B = W   [C,K]      MN-major  (bags_bwd_merged_kernel)
+//   backward dW = dz^T X  : A = dz  [N_roi,C]  MN-major, B = X   [N_roi,K]  MN-major  (bags_bwd_merged_kernel)
 //
 // Pipeline (one CTA per SM, 384 threads = 3 warpgroups):
 //   warpgroup 0   : producer.  TMA (cp.async.bulk.tensor, 128B swizzle, mbarrier tx) for every bf16 operand and
@@ -51,8 +51,6 @@ struct GemmParams {
   const float* colsum_in;  // optional [colsum_tiles, M]: db_out[m] = rowscale(m) * sum_t colsum_in[t, m]
   int colsum_tiles;
   float* colsum_out;       // written by the (n_tile==0, split==0) unit
-  int pdl_wait_producer;   // griddepcontrol.wait before the first operand load (B comes from the previous kernel)
-  int pdl_wait_epilogue;   // griddepcontrol.wait before the first output access (output prepared by the previous kernel)
   // MN-major fp32 operands (loaded without TMA): base pointer, leading dimension (elements), extents
   const float* a_ptr; long long lda; int a_rows, a_k;
   const float* b_ptr; long long ldb; int b_rows, b_k;
@@ -309,39 +307,38 @@ __device__ __forceinline__ Pipe setup_pipe(uint8_t* smem_raw, int stages, int a_
   return pp;
 }
 
-template <int BLOCK_N, bool A_MN, bool B_MN, int EPI, bool TF32, int STAGES>
+// The forward GEMM: both operands K-major, so every load is a TMA load issued by producer thread 0.
+template <int BLOCK_N, int EPI, bool TF32, int STAGES>
 __global__ void __launch_bounds__(384, 1)
 bags_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const GemmParams p) {
-  using Cfg = GemmCfg<BLOCK_N, A_MN, B_MN, EPI, TF32, STAGES>;
+  using Cfg = GemmCfg<BLOCK_N, false, false, EPI, TF32, STAGES>;
   extern __shared__ uint8_t smem_raw[];
   const int wg = threadIdx.x >> 7;
   const int tid = threadIdx.x & 127;
   pdl_trigger();   // a dependent kernel may begin its own prologue
   if (threadIdx.x == 0) { tma_prefetch_desc(&tmap_a); tma_prefetch_desc(&tmap_b); }
-  Pipe pp = setup_pipe(smem_raw, STAGES, Cfg::A_BYTES, Cfg::STAGE_BYTES, Cfg::ANY_MANUAL);
+  Pipe pp = setup_pipe(smem_raw, STAGES, Cfg::A_BYTES, Cfg::STAGE_BYTES, false);
 
   const int units_per_split = p.num_m_tiles * p.num_n_tiles;
   const int num_units = units_per_split * p.num_splits;
   if (wg == 0) {
     // ===================== producer =====================
     setmaxnreg_dec<40>();
-    if (Cfg::ANY_MANUAL || tid == 0) {
-      if (p.pdl_wait_producer) pdl_wait();
+    if (tid == 0) {
       for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
         const int split = u / units_per_split;
         const int t = u - split * units_per_split;
         const int m_tile = t / p.num_n_tiles, n_tile = t - m_tile * p.num_n_tiles;
         int kb0, kb1;
         split_range(p, split, kb0, kb1);
-        produce_unit<Cfg, A_MN, B_MN>(&tmap_a, &tmap_b, p, p.b_ptr, m_tile * 128, n_tile * BLOCK_N, kb0, kb1, pp, tid);
+        produce_unit<Cfg, false, false>(&tmap_a, &tmap_b, p, nullptr, m_tile * 128, n_tile * BLOCK_N, kb0, kb1, pp, tid);
       }
     }
   } else {
     // ===================== consumers =====================
     setmaxnreg_inc<232>();
     const int cw = wg - 1, warp = tid >> 5, lane = tid & 31;
-    if (p.pdl_wait_epilogue) pdl_wait();
     float acc[128];
     for (int u = blockIdx.x; u < num_units; u += gridDim.x) {
       const int split = u / units_per_split;
@@ -349,20 +346,21 @@ bags_gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       const int m_tile = t / p.num_n_tiles, n_tile = t - m_tile * p.num_n_tiles;
       int kb0, kb1;
       split_range(p, split, kb0, kb1);
-      consume_unit<Cfg, A_MN, B_MN, TF32>(acc, cw, kb0, kb1, pp, lane);
+      consume_unit<Cfg, false, false, TF32>(acc, cw, kb0, kb1, pp, lane);
       epilogue_unit<BLOCK_N, EPI>(acc, p, m_tile, n_tile, split, cw, warp, lane, 1.0f);
     }
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Merged backward: both contractions of the BAGS head's backward in ONE persistent launch.
+// Merged backward: the contractions of the BAGS head's backward in ONE persistent launch.
 //
 //   dW units : dW[C,K]  += gout(bin(c)) * dz^T x       (A = dz MN-major, B = x MN-major, split-K, red.add)
 //   dX units : dX[N,K]   = dz W'                       (A = dz K-major,  B = W' MN-major, plain stores)
 //
 // The units form one work list (dW first: their split-K partials are the longer tail), dealt round-robin to the
-// CTAs, so the SMs that finish their dW share early take dX tiles instead of idling at a kernel boundary.  When the
+// CTAs, so the SMs that finish their dW share early take dX tiles instead of idling at a kernel boundary.  A request
+// for only dW or only dX leaves the other list empty (dx_units = 0 / dw_units = 0).  When the
 // bins tile [0, C) and all gout[g] are equal (the reference's setting) the dX units read W itself and scale their
 // output by gout[0]: the preparation kernel then skips the scaled copy W' (it makes the same device-side decision).
 // With gaps between the bins W' is always built, since its gap rows are 0 while W's are not.
@@ -383,7 +381,7 @@ struct BwdMergedParams {
   GemmParams dx;     // ... of the dX problem (b_ptr: W')
   int dw_units, dx_units;
   const float* w;    // W (B of the dX units when gout is uniform)
-  const float* gout; // [G] per-bin upstream gradients, or nullptr (dX reads b_ptr unscaled)
+  const float* gout; // [G] per-bin upstream gradients of the dX units, or nullptr (dX reads b_ptr unscaled)
   int G;
   int uniform_ok;    // the bins tile [0, C): a uniform gout may take the W shortcut
   int inputs_ready;     // a preparation kernel ran between the forward and this launch: dz and x are complete at launch

@@ -262,8 +262,9 @@ size_t bags_bwd_scratch_bytes(int C, long long ldw, int dtype);
  * colsum: optional [colsum_tiles, C] partial column sums of dz from the forward; NULL => recomputed from dz.
  * wscratch: 256-byte aligned, bags_bwd_scratch_bytes() bytes; required when (dX and gout) or (db without colsum).
  * flags: BAGS_BWD_DW_PREZEROED = dW is already zero on entry (stream-ordered), e.g. by bags_fwd's clear hook.
- * Launch structure: one small preparation kernel (zero dW, scaled W, column-sum partials) whose execution is
- * overlapped by the dW GEMM's mainloop (programmatic dependent launch), then the dX GEMM. */
+ * Launch structure: one small preparation kernel (zero dW, scaled W, column-sum partials), then one merged launch whose
+ * work list holds the requested contractions (split-K dW tiles, dX tiles, or both) and whose mainloop overlaps the
+ * preparation kernel (programmatic dependent launch).  db without dW takes one more small kernel. */
 #define BAGS_BWD_DW_PREZEROED 1
 int bags_bwd(const void* dz, long long ldd, const void* x, long long ldx, const void* w,
              long long ldw, const float* gout, const int32_t* slices_host, const float* colsum,
@@ -360,8 +361,13 @@ int bags_act_bwd(const void* dy, long long lddy, int dy_dtype, const void* y, lo
 int bags_cast_bf16(const float* src, long long lds, void* dst, long long ldd, int rows, int cols,
                    void* stream);
 
-/* Test hook: one wgmma GEMM, out[M,N] = A * B^T with either operand K-major ([rows,K]) or
- * MN-major ([K,rows]).  epi: 0 = fp32 store, 1 = bf16 store, 2 = fp32 reduce-add (split-K).  block_n = 256. */
+/* Test hook: out[M,N] = A * B^T on the wgmma kernel the product runs for that layout, each operand K-major ([rows,K])
+ * or MN-major ([K,rows]); block_n = 256:
+ *   both K-major, epi 0 (fp32 store):                        the forward GEMM
+ *   A K-major, B MN-major, epi 1 (bf16 store; bf16 operands)
+ *                       or epi 0 (fp32 store; fp32 operands): the merged backward with dX units only
+ *   both MN-major, epi 2 (fp32 reduce-add, `splits` split-K): the merged backward with dW units only
+ * Any other combination is BAGS_ERR_INVALID. */
 int bags_gemm_probe(const void* a, long long lda, int a_mn, const void* b, long long ldb, int b_mn,
                     void* out, long long ldo, int M, int N, int K, int dtype, int block_n,
                     int splits, int epi, void* stream);

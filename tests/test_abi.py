@@ -131,6 +131,23 @@ def check_fused_operand_rules(lib, who, call, base):
                 assert who.encode() in msg and b'16-byte aligned' in msg, msg
 
 
+def test_bwd_invalid_arguments_return_error_codes():
+    """bags_bwd's operand rules for each requested output, reported before anything touches a device."""
+    lib = nat.lib()
+    buf = (C.c_char * 256)()
+    base = (C.addressof(buf) + 15) // 16 * 16
+    slices = nat.int32_array([0, 4, 4, 4])
+
+    def call(x=base, w=base, dW=None, dX=None, colsum=None, ntiles=0, db=None):
+        return lib.bags_bwd(base, 8, x, 8, w, 8, None, slices, colsum, ntiles, dW, 8, db, dX, 8, None, 0, 4, 8, 8, 2,
+                            nat.DTYPE_BF16, 0, None)
+
+    assert call(w=None, dX=base) == -1 and b'w is NULL' in lib.bags_last_error()
+    assert call(x=None, dW=base) == -1 and b'x is NULL' in lib.bags_last_error()
+    assert call(dX=base + 4) == -1 and b'dX not 16-byte aligned' in lib.bags_last_error()
+    assert call(db=base, colsum=base, ntiles=0) == -1 and b'colsum_tiles' in lib.bags_last_error()
+
+
 def test_cast_bf16_rejects_misaligned_pointers():
     """bags_cast_bf16 reads float4 from src and writes 8-byte groups to dst: a misaligned pointer is a bad argument,
     reported before any launch."""

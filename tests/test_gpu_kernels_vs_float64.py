@@ -2,8 +2,8 @@
 
 Every reference here is plain torch in float64 on the device (cuBLAS DGEMM, torch.logsumexp), never this library.
 Arguments the Python wrappers do not expose (leading dimensions, colsum_tiles, BAGS_BWD_DW_PREZEROED, odd output
-strides, padded output buffers) go through ctypes; backward routes are forced with BAGS_BWD_MERGED / BAGS_DW_SPLITS
-and _native.reload_env().
+strides, padded output buffers) go through ctypes; the backward's dW split count is forced with BAGS_DW_SPLITS and
+_native.reload_env().
 
 Exact tier (most cases).  Operands are small integers, exact in bf16, fp32 and TF32; upstream gradients and scales
 are powers of two, 0 and -1 included; every partial sum is a multiple of 2^-2 whose magnitude stays below 2^12
@@ -135,8 +135,8 @@ def _check_bound(got, ref, tol, what):
 # ------------------------------------------------------------------------------------------------ GEMM (bags_gemm_probe)
 GEMM_KINDS = {   # A MN-major, B MN-major, epilogue for (bf16, fp32) operands -- the six instantiations the product uses
     'kk': (False, False, {BF: 0, F32: 0}),    # forward z = x W^T: fp32 store
-    'kmn': (False, True, {BF: 1, F32: 0}),    # dX = dz W: bf16 store (bf16 operands) / fp32 store
-    'mnmn': (True, True, {BF: 2, F32: 2}),    # dW = dz^T x: split-K reduce-add
+    'kmn': (False, True, {BF: 1, F32: 0}),    # dX = dz W (the merged backward's dX units): bf16 / fp32 store
+    'mnmn': (True, True, {BF: 2, F32: 2}),    # dW = dz^T x (its dW units): split-K reduce-add
 }
 # (M, N, K): every M in {1, 127, 128, 129, 300}, N in {1, 255, 256, 257, 1236} and K in {BLOCK_K - 8, BLOCK_K,
 # BLOCK_K + 8, 1000, 12544} at least once, around the 128 x 256 tile edges
@@ -386,8 +386,7 @@ BWD_ROUTES = [
     ('merged_colsum3_prezeroed', {}, True, True, True, 3, True),
     ('merged_splits1_colsum1', {'BAGS_DW_SPLITS': 1}, True, True, True, 1, False),
     ('merged_splits16_prezeroed', {'BAGS_DW_SPLITS': 16}, True, True, True, 0, True),
-    ('unmerged', {'BAGS_BWD_MERGED': 0}, True, True, True, 0, False),
-    ('unmerged_splits16_colsum1_prezeroed', {'BAGS_BWD_MERGED': 0, 'BAGS_DW_SPLITS': 16}, True, True, True, 1, True),
+    ('dw_db_splits16_colsum1_prezeroed', {'BAGS_DW_SPLITS': 16}, True, True, False, 1, True),
     ('dw_db', {}, True, True, False, 0, False),
     ('dw_db_splits1_colsum3_prezeroed', {'BAGS_DW_SPLITS': 1}, True, True, False, 3, True),
     ('dw', {}, True, False, False, 0, False),
@@ -440,7 +439,7 @@ def test_bwd_exact_all_routes(case):
         db = torch.full((C + 4,), SENT, dtype=F32, device=DEV)
         dX = torch.full((N + 2, K + 8), SENT, dtype=dtype, device=DEV)
         cs = colsums[tiles] if tiles else None
-        with _env(BAGS_BWD_MERGED=switches.get('BAGS_BWD_MERGED'), BAGS_DW_SPLITS=switches.get('BAGS_DW_SPLITS')):
+        with _env(BAGS_DW_SPLITS=switches.get('BAGS_DW_SPLITS')):
             nat.check(nat.lib().bags_bwd(
                 dz.data_ptr(), dz.stride(0), x.data_ptr(), x.stride(0), w.data_ptr(), w.stride(0), nat.ptr(gout_t),
                 slices_host, nat.ptr(cs), tiles, dW.data_ptr() if want_dw else None, dW.stride(0),
@@ -457,18 +456,17 @@ def test_bwd_exact_all_routes(case):
             _check_exact(dX, N, K, ref['dX'], '%s: dX' % name)
             outs['dX'] = dX[:N, :K]
         results[name] = outs
-    # the same bits on every route, up to the sign of a zero: with a uniform gout the merged kernel scales dz W by
-    # gout[0] (gout = -1 turns an exact 0 into -0), the other routes contract dz with the scaled copy -W (+0)
+    # the same bits on every route, signs of zeros included
     for out in ('dW', 'db', 'dX'):
-        runs = [(name, _bits(r[out] + 0.0)) for name, r in results.items() if out in r]
+        runs = [(name, _bits(r[out])) for name, r in results.items() if out in r]
         for name, t in runs[1:]:
             assert torch.equal(t, runs[0][1]), '%s: route %s differs in its bits from %s' % (out, name, runs[0][0])
 
 
 @pytest.mark.parametrize('dtype', DTYPES, ids=DT_IDS)
 def test_bwd_numeric(dtype):
-    """Random normal operands, synthetic table, non-uniform gout: merged and unmerged routes within the numeric bounds
-    (contractions over N for dW, over C for dX)."""
+    """Random normal operands, synthetic table, non-uniform gout: the full call and the split pair (dW + db, then dX)
+    within the numeric bounds (contractions over N for dW, over C for dX)."""
     ops = _ops()
     C, K, N = 1236, 264, 1000 + 77
     slices = _bwd_table('synthetic', C)
@@ -487,19 +485,22 @@ def test_bwd_numeric(dtype):
                           torch.zeros(1, dtype=torch.int32, device=DEV),
                           nat.int32_array([v for sl in slices for v in sl]), np.array(slices, dtype=np.int64))
     ttf = 2.0 ** -8 if dtype == F32 else 0.0
-    for merged in (1, 0):
-        with _env(BAGS_BWD_MERGED=merged):
+    for route in ('full', 'split'):
+        if route == 'full':
             dW, db, dX = ops.fused_bwd(dz, x, w, gout_t, dt, None)
-            torch.cuda.synchronize()
+        else:
+            dW, db, _ = ops.fused_bwd(dz, x, w, gout_t, dt, None, need_dx=False)
+            _, _, dX = ops.fused_bwd(dz, x, w, gout_t, dt, None, need_dw=False, need_db=False)
+        torch.cuda.synchronize()
         # dW: sum over N rows of the scaled dz; the splits of the reduce-add are at most 16
         S = (DZ.abs() * s.abs()).t() @ X.abs()
-        _check_bound(dW, (DZ * s).t() @ X, (ttf + (N + 16) * 2.0 ** -23) * S, 'dW merged=%d' % merged)
+        _check_bound(dW, (DZ * s).t() @ X, (ttf + (N + 16) * 2.0 ** -23) * S, 'dW %s' % route)
         cs = (DZ * s).sum(0)
-        _check_bound(db, cs, (N + 16) * 2.0 ** -23 * (DZ.abs() * s.abs()).sum(0), 'db merged=%d' % merged)
+        _check_bound(db, cs, (N + 16) * 2.0 ** -23 * (DZ.abs() * s.abs()).sum(0), 'db %s' % route)
         S = (DZ.abs() * s.abs()) @ Wm.abs()
         ref = (DZ * s) @ Wm
         tol = (ttf + (C + 1) * 2.0 ** -23) * S + (2.0 ** -8 * ref.abs() if dtype == BF else 0.0)
-        _check_bound(dX, ref, tol, 'dX merged=%d' % merged)
+        _check_bound(dX, ref, tol, 'dX %s' % route)
 
 
 # ------------------------------------------------------------------------------------------------ bags_group_ce

@@ -507,7 +507,8 @@ def test_graphed_step_config2_vs_oracle(env, need_dx):
 @pytest.mark.parametrize('N', [512, 4096])
 def test_split_backward_matches_oracle(env, N, mode, gname):
     """The two launches of the in-step exchange schedule (dW + db first, then dX while the gradients travel): each half
-    alone runs as a plain GEMM (with the preparation kernel where it has work) and must give the oracle's gradients."""
+    alone runs the merged kernel with the other unit list empty (after the preparation kernel where it has work) and
+    must give the oracle's gradients."""
     ops, t, dt, l2b, ps = env
     x, W, b, labels, remapped = _problem(N, seed=55 + N)
     gout = GOUTS[gname]

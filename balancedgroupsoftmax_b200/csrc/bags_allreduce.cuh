@@ -5,7 +5,7 @@
 // copy back) by ONE kernel working directly on the ranks' gradient buckets, which live in symmetric
 // (peer-mapped) memory:
 //
-//   barrier (all ranks' local dW / db are complete)            flag words in the peers' buffers, sys-scope CAS
+//   barrier (all ranks' local dW / db are complete)            epoch flag words in the peers' buffers, sys scope
 //   two-shot exchange: rank r owns vectors [r*chunk, (r+1)*chunk)
 //       NVLS   : multimem.ld_reduce.add.v4.f32 on the multicast address (the switch sums the N copies)
 //                -> * scale -> multimem.st.v4.f32 (the switch broadcasts to the N copies)
@@ -16,9 +16,9 @@
 // 5.07 MB per head: 2 * (N-1)/N * 5.07 MB cross each GPU's links plus two flag round trips.
 //
 // Flags (inside every rank's bucket allocation, zeroed once by the caller):
-//   slot[b][r]  written by rank r's block b with an EPOCH number (st.release.sys, fire and forget), polled locally by
-//               this rank's block b (ld.acquire.sys until it reaches the expected epoch);
-//               or, protocol "cas": toggled 0 -> 1 by the sender (CAS on the target) and 1 -> 0 by the receiver;
+//   slot[b][r]  written by rank r's block b with an EPOCH number (fire and forget: st.relaxed.sys at the first barrier,
+//               st.release.sys at the second), polled locally by this rank's block b (ld.relaxed.sys until it
+//               reaches the expected epoch, then one ld.acquire.sys);
 //   epoch[b]    this rank's block b's own count of barriers so far (all ranks run the same launches, so they agree);
 //   status      set to 1 when a wait timed out (bounded in time; the kernel then traps -- see rank_barrier).
 // Epochs only grow, so nothing is reset and CUDA-graph replays need no host work; a sender may be one barrier ahead
@@ -34,7 +34,7 @@ constexpr int kMaxRanks = 16;
 // Small blocks with few registers: an exchange block fits on an SM next to a GEMM CTA of this library (48-55 K
 // registers), so an exchange launched on a side stream really overlaps the next step's kernels.
 constexpr int kArMaxBlocks = 320;
-constexpr int kArThreads = 256;   // upper bound; the launch may use fewer (BAGS_AR_THREADS)
+constexpr int kArThreads = 256;
 
 struct AllReduceParams {
   float* peer[kMaxRanks];   // this process's mapping of every rank's bucket (peer[rank] is the local one)
@@ -48,11 +48,6 @@ struct AllReduceParams {
                             //    loudly -- NCCL would hang); 0 (construction-time self test only): set the status word,
                             //    skip the exchange and let the host fall back to NCCL
   long long* timing;        // debug timeline [grid][8] (%globaltimer) or nullptr
-  int mode;                 // protocol switches (epoch flags only): bit 0 = the FIRST barrier's flag store is relaxed --
-                            //   the data it publishes was written by the preceding kernel and is in L2, the point of
-                            //   coherence peers read through, so no system-scope release fence is needed; bit 1 = poll
-                            //   with relaxed loads and acquire once at the end; bit 2 = let the next kernel launch
-                            //   (griddepcontrol.launch_dependents) only after the data phase instead of at the start
 };
 
 __device__ __forceinline__ void st_release_sys_u32(uint32_t* p, uint32_t v) {
@@ -68,15 +63,8 @@ __device__ __forceinline__ uint32_t ld_acquire_sys_u32(const uint32_t* p) {
   asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-__device__ __forceinline__ uint32_t cas_release_sys(uint32_t* p, uint32_t cmp, uint32_t val) {
-  uint32_t old;
-  asm volatile("atom.global.release.sys.cas.b32 %0, [%1], %2, %3;" : "=r"(old) : "l"(p), "r"(cmp), "r"(val) : "memory");
-  return old;
-}
-__device__ __forceinline__ uint32_t cas_acquire_sys(uint32_t* p, uint32_t cmp, uint32_t val) {
-  uint32_t old;
-  asm volatile("atom.global.acquire.sys.cas.b32 %0, [%1], %2, %3;" : "=r"(old) : "l"(p), "r"(cmp), "r"(val) : "memory");
-  return old;
+__device__ __forceinline__ void st_relaxed_sys_u32(uint32_t* p, uint32_t v) {
+  asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ float4 ld_relaxed_sys_f4(const float* p) {
   float4 v;
@@ -110,12 +98,9 @@ __device__ __forceinline__ void multimem_st_f4(float* mc, const float4 v) {
 __device__ __forceinline__ uint32_t* ar_flags(const AllReduceParams& p, int rank) {
   return reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(p.peer[rank]) + p.flag_off);
 }
-// EPOCH = true : slots carry monotonically growing epoch numbers (release store, local acquire-load polling).
-// EPOCH = false: slots toggle 0 -> 1 -> 0 (put = CAS 0->1 on the target, wait = CAS 1->0 on the own copy).
-__device__ __forceinline__ void st_relaxed_sys_u32(uint32_t* p, uint32_t v) {
-  asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-template <bool EPOCH>
+// The FIRST barrier's flag store is relaxed: the data it publishes was written by the preceding kernel and is in L2,
+// the point of coherence peers read through, so no system-scope release is needed.  The second one releases this
+// block's peer stores.  Polling is relaxed, with one acquire load once the epoch has arrived.
 __device__ __forceinline__ bool rank_barrier(const AllReduceParams& p, uint32_t epoch, int* s_fail, bool first = false) {
   __syncthreads();
   if (threadIdx.x < static_cast<unsigned>(p.world)) {
@@ -132,31 +117,14 @@ __device__ __forceinline__ bool rank_barrier(const AllReduceParams& p, uint32_t 
       if (t0 == 0) { t0 = now; return false; }
       return now - t0 > p.timeout_ns;
     };
-    if (EPOCH) {
-      if (first && (p.mode & 1)) st_relaxed_sys_u32(theirs, epoch);
-      else                       st_release_sys_u32(theirs, epoch);
-      if (p.mode & 2) {
-        while (static_cast<int32_t>(ld_relaxed_sys_u32(mine) - epoch) < 0) {
-          if (expired()) { ok = false; break; }
-        }
-        if (ok) (void)ld_acquire_sys_u32(mine);
-      } else {
-        while (static_cast<int32_t>(ld_acquire_sys_u32(mine) - epoch) < 0) {
-          __nanosleep(20);
-          if (expired()) { ok = false; break; }
-        }
-      }
-    } else {
-      while (cas_release_sys(theirs, 0u, 1u) != 0u) {
-        if (expired()) { ok = false; break; }
-      }
-      spins = 0; t0 = 0;
-      while (ok && cas_acquire_sys(mine, 1u, 0u) != 1u) {
-        __nanosleep(20);
-        if (expired()) { ok = false; break; }
-      }
+    if (first) st_relaxed_sys_u32(theirs, epoch);
+    else       st_release_sys_u32(theirs, epoch);
+    while (static_cast<int32_t>(ld_relaxed_sys_u32(mine) - epoch) < 0) {
+      if (expired()) { ok = false; break; }
     }
-    if (!ok) {
+    if (ok) {
+      (void)ld_acquire_sys_u32(mine);
+    } else {
       *s_fail = 1;
       atomicExch(ar_flags(p, p.rank) + kArMaxBlocks * p.world + kArMaxBlocks, 1u);
       if (p.trap_on_timeout) {
@@ -172,11 +140,11 @@ __device__ __forceinline__ bool rank_barrier(const AllReduceParams& p, uint32_t 
   return *s_fail == 0;
 }
 
-template <bool MULTIMEM, bool EPOCH>
+template <bool MULTIMEM>
 __global__ void __launch_bounds__(kArThreads, 6)
 bags_grad_allreduce_kernel(const AllReduceParams p) {
   if (threadIdx.x == 0) stamp(p.timing, 0);
-  if (!(p.mode & 4)) pdl_trigger();   // the next kernel of the stream (next step's sampler / forward) may start launching
+  pdl_trigger();   // the next kernel of the stream (next step's sampler / forward) may start launching
   pdl_wait();      // the local gradients come from the preceding backward kernel
   if (threadIdx.x == 0) stamp(p.timing, 1);
   __shared__ int s_fail;
@@ -185,7 +153,7 @@ bags_grad_allreduce_kernel(const AllReduceParams p) {
   // soft-failed exchange (self test) leaves the epochs of all ranks consistent
   uint32_t* my_epoch = ar_flags(p, p.rank) + kArMaxBlocks * p.world + blockIdx.x;
   const uint32_t epoch = *my_epoch;
-  if (!rank_barrier<EPOCH>(p, epoch + 1u, &s_fail, true)) {
+  if (!rank_barrier(p, epoch + 1u, &s_fail, true)) {
     if (threadIdx.x == 0) *my_epoch = epoch + 2u;
     return;
   }
@@ -228,8 +196,7 @@ bags_grad_allreduce_kernel(const AllReduceParams p) {
     }
   }
   if (threadIdx.x == 0) stamp(p.timing, 3);
-  if (p.mode & 4) pdl_trigger();
-  rank_barrier<EPOCH>(p, epoch + 2u, &s_fail);
+  rank_barrier(p, epoch + 2u, &s_fail);
   if (threadIdx.x == 0) { *my_epoch = epoch + 2u; stamp(p.timing, 4); }
 }
 

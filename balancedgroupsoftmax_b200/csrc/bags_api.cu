@@ -1168,26 +1168,20 @@ extern "C" int bags_grad_allreduce(void* const* peer_bufs_host, void* mc_buf, lo
   if (max_blocks < 0) max_blocks = 0;
   p.timeout_ns = 1000000LL * env_int("BAGS_AR_TIMEOUT_MS", p.trap_on_timeout ? 30000 : 3000);
   p.timing = g_timing ? g_timing + 4096 * 8 : nullptr;   // rows [4096, ..): after the forward's and the backward's
-  p.mode = env_int("BAGS_AR_MODE", 3);   // relaxed first-barrier store + relaxed polling: -3..4 us per exchange
   if (count == 0) return BAGS_OK;
-  // enough threads to keep one vector per thread and unroll slot in flight, at most kArMaxBlocks blocks;
-  // every rank must launch the same grid: it depends only on (count, world, max_blocks) and the environment
-  int threads = env_int("BAGS_AR_THREADS", 256);
-  if (threads != 128 && threads != 256) threads = 256;
-  if (max_blocks > kArMaxBlocks) max_blocks = kArMaxBlocks;
+  // enough blocks to keep one vector per thread and unroll slot in flight, at most kArMaxBlocks;
+  // every rank must launch the same grid: it depends only on (count, world, max_blocks) and the transport
   const long long per_rank = (count / 4 + world - 1) / world;
-  long long blocks = (per_rank + static_cast<long long>(threads) * 4 - 1) / (static_cast<long long>(threads) * 4);
+  long long blocks = (per_rank + kArThreads * 4LL - 1) / (kArThreads * 4LL);
   if (blocks < 1) blocks = 1;
   const bool mm = p.mc != nullptr && !env_int("BAGS_AR_NO_MULTIMEM", 0);
   // Default grid: one block per SM on the multimem path (the exchange runs inside the step, where a small grid leaves
   // the switch bandwidth unused); the plain peer path keeps one vector per thread in flight.
-  if (max_blocks <= 0) max_blocks = env_int("BAGS_AR_MAX_BLOCKS", mm ? di.num_sms : kArMaxBlocks);
-  if (max_blocks <= 0 || max_blocks > kArMaxBlocks) max_blocks = kArMaxBlocks;
+  if (max_blocks <= 0) max_blocks = mm ? di.num_sms : kArMaxBlocks;
+  if (max_blocks > kArMaxBlocks) max_blocks = kArMaxBlocks;
   if (blocks > max_blocks) blocks = max_blocks;
-  const bool epoch = env_int("BAGS_AR_EPOCH", 1) != 0;
-  const dim3 grid(static_cast<unsigned>(blocks)), block(static_cast<unsigned>(threads));
-  auto kernel = mm ? (epoch ? bags_grad_allreduce_kernel<true, true> : bags_grad_allreduce_kernel<true, false>)
-                  : (epoch ? bags_grad_allreduce_kernel<false, true> : bags_grad_allreduce_kernel<false, false>);
+  const dim3 grid(static_cast<unsigned>(blocks)), block(kArThreads);
+  auto kernel = mm ? bags_grad_allreduce_kernel<true> : bags_grad_allreduce_kernel<false>;
   BAGS_CUDA(launch(kernel, grid, block, 0, stream, true, false, p));
   return BAGS_OK;
 }

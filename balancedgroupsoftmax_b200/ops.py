@@ -772,18 +772,33 @@ def _fused_loss_saved(ctx, xc, wc, dz, dW) -> None:
         ctx.save_for_backward(xc, wc, dz)
 
 
-def _fused_loss_bwd(ctx, grad_loss, dt: Optional[DeviceTables] = None, colsum: Optional[torch.Tensor] = None):
+def _fused_loss_bwd(ctx, grad_loss, dt: Optional[DeviceTables] = None, colsum: Optional[torch.Tensor] = None,
+                    bucket=None):
     """(dX, dW, db) in the parameters' dtypes from the dz~ a fused-loss forward saved: one bags_bwd over the bin table
     ``dt`` (None: the single slice (0, C)), with the forward's column-sum partials ``colsum`` when it took them; dX only
-    when x needs a gradient, dW zeroed by the forward kernel when ``ctx.dW`` is set."""
+    when x needs a gradient, dW zeroed by the forward kernel when ``ctx.dW`` is set.
+
+    With a gradient ``bucket`` (``views = (dW, db)``, ``exchange_overlapped()``) and a weight gradient wanted, dW + db
+    go straight into the bucket views in a first bags_bwd, the exchange starts as soon as they are complete, and dX is
+    a second bags_bwd that runs while the gradients travel; the exchange is joined before returning."""
     xc, wc, dz = ctx.saved_tensors
-    need_dx, need_dw, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+    need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+    need_db = ctx.needs_input_grad[2] and ctx.has_bias
+    split = bucket is not None and need_dw
     dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
     if dt is None:
         dt = _single_slice_tables(wc.shape[0], xc.device)
-    dW, db, dX = fused_bwd(dz, xc, wc, _gout(grad_loss), dt, colsum, need_dw=need_dw,
-                           need_db=(need_db and ctx.has_bias), need_dx=need_dx,
-                           dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None)
+    gout = _gout(grad_loss)
+    if split and dW0 is None:
+        dW0 = bucket.views[0].zero_()
+    dW, db, dX = fused_bwd(dz, xc, wc, gout, dt, colsum, need_dw=need_dw, need_db=need_db,
+                           need_dx=need_dx and not split, dW=dW0 if need_dw else None, dw_prezeroed=dW0 is not None,
+                           db=bucket.views[1] if (split and need_db and len(bucket.views) > 1) else None)
+    if split:
+        join = bucket.exchange_overlapped()
+        if need_dx:
+            _, _, dX = fused_bwd(dz, xc, wc, gout, dt, None, need_dw=False, need_db=False, need_dx=True)
+        join()
     return _grads_in_param_dtypes(ctx, dX, dW, db)
 
 
@@ -854,28 +869,7 @@ class GroupSoftmaxFunction(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_loss):
-        bucket = ctx.grad_bucket
-        if bucket is None or not ctx.needs_input_grad[1]:
-            return _fused_loss_bwd(ctx, grad_loss, ctx.dt, ctx.colsum) + (None,) * 7
-        xc, wc, dz = ctx.saved_tensors
-        need_dx, need_db = ctx.needs_input_grad[0], ctx.needs_input_grad[2]
-        gout = _gout(grad_loss)
-        dW0, ctx.dW = ctx.dW, None                      # (a second backward through a retained graph zeroes again)
-        # dW + db first, straight into the exchange bucket; the exchange starts when they are complete and runs
-        # while the dX contraction does
-        if dW0 is None:
-            bucket.views[0].zero_()
-        db_view = bucket.views[1] if (need_db and ctx.has_bias and len(bucket.views) > 1) else None
-        dW, db, _ = fused_bwd(dz, xc, wc, gout, ctx.dt, ctx.colsum, need_dw=True,
-                              need_db=(need_db and ctx.has_bias), need_dx=False, dW=bucket.views[0], db=db_view,
-                              dw_prezeroed=True)
-        join = bucket.exchange_overlapped()
-        dX = None
-        if need_dx:
-            _, _, dX = fused_bwd(dz, xc, wc, gout, ctx.dt, None, need_dw=False, need_db=False, need_dx=True)
-        join()
-        dX, dW, db = _grads_in_param_dtypes(ctx, dX, dW, db)
-        return dX, dW, db, None, None, None, None, None, None, None
+        return _fused_loss_bwd(ctx, grad_loss, ctx.dt, ctx.colsum, ctx.grad_bucket) + (None,) * 7
 
 
 class SoftmaxCEFunction(torch.autograd.Function):

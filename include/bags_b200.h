@@ -286,8 +286,8 @@ int bags_merge_scores(const float* logits, long long ldz, const int32_t* slices_
  *   mc_buf         : multicast (NVLS) mapping of the same bucket, or NULL -> plain peer loads / stores
  *   count          : fp32 elements at the start of the bucket to reduce in place (multiple of 4)
  *   flag_off_bytes : offset, inside the same allocation, of bags_grad_allreduce_flag_bytes(world) bytes of flag
- *                    words that the caller zeroes ONCE (before the first exchange, on every rank); every call
- *                    leaves them zero
+ *                    words that the caller zeroes ONCE (before the first exchange, on every rank); the calls
+ *                    keep them consistent from then on (epoch counters: no reset, also across CUDA-graph replays)
  *   scale          : applied to the sum (1/world = the reference's mean)
  *   max_blocks     : grid size limit (0 = the library's default for the transport; every rank the same value);
  *                    a NEGATIVE value selects the soft-failure mode of a construction-time self test (see below)

@@ -208,10 +208,13 @@ bags_mask_bwd_kernel(const MaskBwdParams p) {
       float total = 0.f;
 #pragma unroll
       for (int w = 0; w < kMaskThreads / 32; ++w) total += s_part[w][lane];
+      // + 0 makes a zero sum +0 also for a negative gout (go * +0 alone is -0), as the float64 gradient of a class
+      // without RoIs is; every nonzero product is unchanged
+      const float out = fmaf(go, total, 0.f);
       if (c < p.Cin) {
-        if (p.dW != nullptr) p.dW[l * p.lddw + c] = go * total;
+        if (p.dW != nullptr) p.dW[l * p.lddw + c] = out;
       } else if (p.db != nullptr) {
-        p.db[l] = go * total;
+        p.db[l] = out;
       }
     }
     return;

@@ -39,6 +39,7 @@ class_nms_dense_kernel(const float* __restrict__ boxes, int box_cols, const int*
   const int s = blockIdx.x;
   int cnt = counts[s];
   cnt = cnt < n ? cnt : n;
+  cnt = cnt > 0 ? cnt : 0;   // a negative count would start the zeroing loop below before this class's keep row
   if (cnt > kNmsMaxSeg) { if (threadIdx.x == 0) *overflow = 1; cnt = kNmsMaxSeg; }
   const int* ord = order + static_cast<long long>(s) * n;
   uint8_t* kp = keep + static_cast<long long>(s) * n;

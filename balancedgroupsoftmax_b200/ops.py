@@ -536,8 +536,11 @@ def multiclass_nms(multi_bboxes: torch.Tensor, multi_scores: torch.Tensor, score
         ->  bags_class_nms_dense: one CTA per class gathers its candidates' boxes and suppresses (IoU with "+1" widths,
             mmdet/ops/nms/src/nms_kernel.cu:13-21,60)  ->  top-``max_num`` by score of the survivors (bbox_nms.py:55-61)
 
-    Returns (dets [k,5], labels [k] 0-based): class-major / score-descending order when nothing is cut, score order
-    when ``max_num`` cuts -- as the reference; ``max_num = -1`` drops the lowest-scored detection, as the reference does."""
+    Returns (dets [k,5], labels [k] 0-based) in the reference's order: when nothing is cut, class-major and ascending
+    RoI index inside a class (the NMS op returns its kept indices sorted, nms_kernel.cu:127-130); score order when
+    ``max_num`` cuts.  ``max_num = -1`` drops the lowest-scored detection, as the reference does.  A candidate is a
+    score ``> score_thr`` compared in the scores' own dtype (bbox_nms.py:36), so a NaN score is never one.  Equal scores
+    of a class are visited lower RoI index first (the reference's unstable sort leaves that order open)."""
     _require_cuda(multi_bboxes, multi_scores)
     n, num_classes = multi_scores.shape
     dev = multi_scores.device
@@ -545,10 +548,15 @@ def multiclass_nms(multi_bboxes: torch.Tensor, multi_scores: torch.Tensor, score
     if n == 0 or S <= 0:
         return multi_bboxes.new_zeros((0, 5)), multi_bboxes.new_zeros((0,), dtype=torch.long)
     boxes = multi_bboxes.float().contiguous()
+    if boxes.data_ptr() % 16:                                        # a view at an odd offset: the kernel reads float4
+        boxes = boxes.clone()
     if boxes.shape[1] not in (4, 4 * num_classes):
         raise nat.BagsNativeError('multi_bboxes must be [n, 4] or [n, 4 * num_classes]')
-    vals, order = multi_scores[:, 1:].float().t().contiguous().sort(dim=1, descending=True, stable=True)   # [S, n]
-    counts = (vals > score_thr).sum(dim=1, dtype=torch.int32)
+    cand = (multi_scores[:, 1:] > score_thr).t()                     # in the scores' dtype; NaN is never a candidate
+    counts = cand.sum(dim=1, dtype=torch.int32)
+    # non-candidates sort last, so each class's candidates are the first counts[s] of its row
+    key = torch.where(cand, multi_scores[:, 1:].t().float(), float('-inf'))
+    vals, order = key.contiguous().sort(dim=1, descending=True, stable=True)   # [S, n]
     order32 = order.to(torch.int32)
     keep = torch.empty((S, n), dtype=torch.uint8, device=dev)
     overflow = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -565,8 +573,9 @@ def multiclass_nms(multi_bboxes: torch.Tensor, multi_scores: torch.Tensor, score
     if total > max_num:                                              # bbox_nms.py:57-61 (true for max_num = -1 as well)
         k = max_num if max_num >= 0 else total + max_num             # inds[:max_num]: a negative bound drops the tail
         sel = topi[:max(min(k, total), 0)]
-    else:
-        sel = topi[:total].sort().values                             # class-major, score-descending inside a class
+    else:                                                            # class-major, ascending RoI index inside a class
+        sel = topi[:total]
+        sel = sel[(torch.div(sel, n, rounding_mode='floor') * n + order.reshape(-1)[sel]).argsort()]
     cls = torch.div(sel, n, rounding_mode='floor')
     rows = order.reshape(-1)[sel]
     b4 = boxes[rows] if boxes.shape[1] == 4 else boxes.view(n, num_classes, 4)[rows, cls + 1]

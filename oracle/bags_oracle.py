@@ -214,38 +214,61 @@ def head_step(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, labels:
 # ---------------------------------------------------------------------------------------------------
 # test-time consumer of the merged scores: per-class NMS
 # ---------------------------------------------------------------------------------------------------
+def iou_plus1_fp32(a: np.ndarray, b: np.ndarray) -> np.ndarray:
+    """devIoU of the reference op (mmdet/ops/nms/src/nms_kernel.cu:13-21) in its own fp32 arithmetic and operation
+    order: "+1" widths, CUDA's float max/min (fmaxf/fminf: a NaN operand yields the other one).  a, b [..., 4]
+    broadcast; every step rounds to fp32 once, so with integer coordinates below 2^11 the division is the only
+    rounding."""
+    a = np.asarray(a, dtype=np.float32)
+    b = np.asarray(b, dtype=np.float32)
+    one, zero = np.float32(1), np.float32(0)
+    with np.errstate(invalid='ignore', divide='ignore', over='ignore'):
+        left, right = np.fmax(a[..., 0], b[..., 0]), np.fmin(a[..., 2], b[..., 2])
+        top, bottom = np.fmax(a[..., 1], b[..., 1]), np.fmin(a[..., 3], b[..., 3])
+        width, height = np.fmax(right - left + one, zero), np.fmax(bottom - top + one, zero)
+        inter = width * height
+        sa = (a[..., 2] - a[..., 0] + one) * (a[..., 3] - a[..., 1] + one)
+        sb = (b[..., 2] - b[..., 0] + one) * (b[..., 3] - b[..., 1] + one)
+        return inter / (sa + sb - inter)
+
+
+def greedy_keep(boxes: np.ndarray, iou_thr: float) -> np.ndarray:
+    """The reference op's greedy scan over boxes already in visiting order: box j is removed when a box i < j that
+    is still alive has IoU(i, j) > fp32(iou_thr) (nms_kernel.cu:60,117-126).  -> bool keep [n]."""
+    boxes = np.asarray(boxes, dtype=np.float32).reshape(-1, 4)
+    n = boxes.shape[0]
+    thr = np.float32(iou_thr)
+    removed = np.zeros(n, dtype=bool)
+    for i in range(n):
+        if not removed[i] and i + 1 < n:
+            removed[i + 1:] |= iou_plus1_fp32(boxes[i], boxes[i + 1:]) > thr
+    return ~removed
+
+
 def nms_plus1(dets: torch.Tensor, iou_thr: float) -> Tuple[torch.Tensor, torch.Tensor]:
-    """Greedy NMS with the reference op's conventions (mmdet/ops/nms/src/nms_kernel.cu:13-21,60,76-78): boxes visited
-    in descending score order, IoU with "+1" widths, a box is dropped when IoU with a kept box > iou_thr.
-    dets [n,5] (x1,y1,x2,y2,score) -> (kept dets in score order, their indices)."""
+    """Greedy NMS with the reference op's conventions (mmdet/ops/nms/src/nms_kernel.cu:13-21,60,76-78,127-130):
+    boxes visited in descending score order, fp32 IoU with "+1" widths (iou_plus1_fp32), a box is dropped when its
+    IoU with a kept box is > fp32(iou_thr); the kept rows are returned in ASCENDING index order, as the op returns
+    them.  Equal scores are visited lower index first (the op's unstable sort leaves their order open).
+    dets [n,5] (x1,y1,x2,y2,score) -> (dets[inds], inds)."""
     if dets.shape[0] == 0:
         return dets, dets.new_zeros(0, dtype=torch.long)
-    d = dets.detach().double().cpu().numpy()
+    d = dets.detach().float().cpu().numpy()
     order = np.argsort(-d[:, 4], kind='stable')
-    x1, y1, x2, y2 = d[:, 0], d[:, 1], d[:, 2], d[:, 3]
-    area = (x2 - x1 + 1) * (y2 - y1 + 1)
-    removed = np.zeros(len(d), dtype=bool)
-    keep = []
-    for a, i in enumerate(order):
-        if removed[i]:
-            continue
-        keep.append(i)
-        rest = order[a + 1:]
-        w = np.maximum(np.minimum(x2[i], x2[rest]) - np.maximum(x1[i], x1[rest]) + 1, 0)
-        h = np.maximum(np.minimum(y2[i], y2[rest]) - np.maximum(y1[i], y1[rest]) + 1, 0)
-        inter = w * h
-        iou = inter / (area[i] + area[rest] - inter)
-        removed[rest[iou.astype(np.float32) > np.float32(iou_thr)]] = True
-    inds = torch.as_tensor(np.array(keep, dtype=np.int64))
+    keep = greedy_keep(d[order, :4], iou_thr)
+    inds = torch.as_tensor(np.sort(order[keep]).astype(np.int64))
     return dets[inds], inds
 
 
 def multiclass_nms(multi_bboxes: torch.Tensor, multi_scores: torch.Tensor, score_thr: float, iou_thr: float,
-                   max_num: int = -1) -> Tuple[torch.Tensor, torch.Tensor]:
+                   max_num: int = -1, nms_op=None) -> Tuple[torch.Tensor, torch.Tensor]:
     """mmdet/core/post_processing/bbox_nms.py:6-66 restated (nms_cfg = dict(type='nms', iou_thr=...)): column 0 of the
     scores is background and ignored; per class keep score > score_thr, NMS, label = class - 1; concatenate in class
     order; ``if n > max_num`` sort by score and keep ``[:max_num]`` -- including the reference's behaviour for
-    max_num = -1 (n > -1 always holds, so the lowest-scored detection is dropped)."""
+    max_num = -1 (n > -1 always holds, so the lowest-scored detection is dropped).  ``score > score_thr`` compares in
+    the scores' own dtype.  ``nms_op(dets, iou_thr) -> (dets, inds)`` is the per-class NMS (default nms_plus1; the
+    reference's compiled op through oracle.ref_nms.nms_wrapper_op plugs in here)."""
+    nms_op = nms_plus1 if nms_op is None else nms_op
     num_classes = multi_scores.shape[1]
     bboxes, labels = [], []
     for i in range(1, num_classes):
@@ -253,9 +276,9 @@ def multiclass_nms(multi_bboxes: torch.Tensor, multi_scores: torch.Tensor, score
         if not cls_inds.any():
             continue
         _b = multi_bboxes[cls_inds, :] if multi_bboxes.shape[1] == 4 else multi_bboxes[cls_inds, i * 4:(i + 1) * 4]
-        cls_dets, _ = nms_plus1(torch.cat([_b, multi_scores[cls_inds, i][:, None]], 1), iou_thr)
+        cls_dets, _ = nms_op(torch.cat([_b, multi_scores[cls_inds, i][:, None]], 1), iou_thr)
         bboxes.append(cls_dets)
-        labels.append(torch.full((cls_dets.shape[0],), i - 1, dtype=torch.long))
+        labels.append(multi_bboxes.new_full((cls_dets.shape[0],), i - 1, dtype=torch.long))
     if not bboxes:
         return multi_bboxes.new_zeros((0, 5)), multi_bboxes.new_zeros((0,), dtype=torch.long)
     bboxes, labels = torch.cat(bboxes), torch.cat(labels)

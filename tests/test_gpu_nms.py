@@ -53,7 +53,7 @@ def test_get_det_bboxes_runs_native_nms_at_lvis_shape():
         boxes, scores = head.get_det_bboxes(rois, z, None, (800, 1333, 3), 1.0, rescale=False, cfg=None)
     want_b, want_l = O.multiclass_nms(boxes.cpu(), scores.cpu(), 0.0, 0.5, 300)
     assert dets.shape == want_b.shape == (300, 5)
-    # the cut at max_per_img falls between distinct scores, so the kept sets agree exactly
-    key_w = sorted(zip(want_l.tolist(), [tuple(r) for r in want_b.tolist()]))
-    key_g = sorted(zip(labels.cpu().tolist(), [tuple(r) for r in dets.cpu().tolist()]))
-    assert key_w == key_g
+    # the cut at max_per_img falls between distinct scores, so the kept detections agree exactly, in score order
+    assert torch.equal(labels.cpu(), want_l)
+    assert torch.equal(dets.cpu(), want_b)
+    assert (dets[1:, 4] < dets[:-1, 4]).all()

@@ -120,9 +120,10 @@ def test_get_target_matches_reference_bbox_target(ref):
     assert got[0].dtype == torch.long and got[0][:5].tolist() == imgs[0].pos_gt_labels.tolist() and got[0][5:25].sum() == 0
 
 
-def test_multiclass_nms_oracle_matches_reference_loop(ref):
+def test_multiclass_nms_oracle_matches_reference_loop_in_op_order(ref):
     """The oracle's multiclass_nms against the reference's bbox_nms.py (its compiled NMS op replaced by the oracle's
-    greedy "+1" NMS): thresholds, labels, class order and the top-k rule."""
+    greedy "+1" NMS): thresholds, labels, class order, the op's ascending index order inside a class when nothing is
+    cut, and the top-k rule."""
     _, d = ref
     boxes4, boxes_pc, scores = MG.nms_inputs()
     for bi, mb in enumerate((boxes4, boxes_pc)):

@@ -50,6 +50,7 @@ SIGNATURES = {
     'bags_mask_fwd': (_i, [_vp, _i, _vp, _ll, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _sz, _vp, _vp, _sz,
                            _vp]),
     'bags_mask_bwd': (_i, [_vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _i, _i, _i, _i, _vp, _ll, _vp, _vp, _vp]),
+    'bags_mask_logits': (_i, [_vp, _i, _vp, _ll, _vp, _vp, _i, _i, _i, _i, _vp, _vp]),
     'bags_reweight': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     'bags_bwd_scratch_bytes': (_sz, [_i, _ll, _i]),
     'bags_bwd': (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _i, _vp, _ll, _vp, _vp, _ll, _vp, _sz, _i, _i,

@@ -892,6 +892,35 @@ extern "C" int bags_mask_bwd(const float* g, const float* rsum, const float* gou
   return BAGS_OK;
 }
 
+// test-time label-channel logits (fcn_mask_head.py:125-181 and htc.py:403-421 read one channel per detection)
+extern "C" int bags_mask_logits(const void* y, int dtype, const float* w, long long ldw, const float* bias,
+                                const int64_t* channels, int n, int Cin, int HW, int classes, void* out,
+                                void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = check_mask_shape("bags_mask_logits", dtype, ldw, n, Cin, HW, classes)) return rc;
+  BAGS_REQUIRE(n == 0 || (y && w && channels && out), "bags_mask_logits: NULL argument");
+  if (n == 0) return BAGS_OK;
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  MaskLogitsParams p{};
+  p.y = y; p.w = w; p.ldw = ldw; p.bias = bias;
+  p.channels = reinterpret_cast<const long long*>(channels);
+  p.Cin = Cin; p.HW = HW; p.classes = classes;
+  p.tiles = (HW + kMaskTile - 1) / kMaskTile;
+  p.out = out;
+  const dim3 grid(static_cast<unsigned>(n * p.tiles));
+  const bool v4 = mask_vec4(y, dtype, HW);
+  if (dtype == BAGS_DTYPE_BF16) {
+    if (v4) bags_mask_logits_kernel<true, 4><<<grid, kMaskThreads, 0, stream>>>(p);
+    else    bags_mask_logits_kernel<true, 1><<<grid, kMaskThreads, 0, stream>>>(p);
+  } else {
+    if (v4) bags_mask_logits_kernel<false, 4><<<grid, kMaskThreads, 0, stream>>>(p);
+    else    bags_mask_logits_kernel<false, 1><<<grid, kMaskThreads, 0, stream>>>(p);
+  }
+  BAGS_CUDA(cudaGetLastError());
+  return BAGS_OK;
+}
+
 extern "C" int bags_reweight(const int64_t* labels, const int32_t* label2bin, const uint8_t* wmask,
                              const float* cls_weight, int wstride, int N, int G, int classes, float* wfloat,
                              float* avg, void* stream_) {

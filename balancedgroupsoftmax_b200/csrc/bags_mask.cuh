@@ -12,6 +12,9 @@
 //                          the class's RoIs, its (RoI, tile) pairs dealt to 8 warps in ascending order and the warps'
 //                          partials added in warp order (zero for a class without RoIs).  RoI units: one tile of
 //                          dY[p, :, q] = gout g[p,q] W[l, :] (zero for an invalid row).
+//   bags_mask_logits_kernel  test time: one CTA per (detection, tile of kMaskTile pixels), pass 1 of the forward alone
+//                          (the same mask_logit, so the same summation order) for the detection's channel c_d, stored
+//                          in y's dtype; NaN for a channel outside [0, classes).
 // y is read from HBM once; no atomics on floats, so every output is bit-identical from run to run.
 #pragma once
 #include "bags_kernels.cuh"
@@ -48,6 +51,15 @@ struct MaskBwdParams {
   void* dY;
 };
 
+struct MaskLogitsParams {
+  const void* y;                         // [n, Cin, HW] bf16 or fp32
+  const float* w; long long ldw;         // [classes, Cin] fp32
+  const float* bias;                     // [classes] or nullptr
+  const long long* channels;             // [n]
+  int Cin, HW, classes, tiles;
+  void* out;                             // [n, HW] in y's dtype
+};
+
 __device__ __forceinline__ bool mask_valid(long long l, int classes) { return MaskLabelValid()(l, classes); }
 
 // V consecutive elements of y at element offset ``off`` (V = 4: 8- (bf16) or 16-byte (fp32) aligned)
@@ -61,6 +73,41 @@ __device__ __forceinline__ void mask_load(const void* base, long long off, float
   } else {
     v[0] = __ldg(reinterpret_cast<const float*>(base) + off);
   }
+}
+
+// Pass 1 of bags_mask_fwd_kernel and bags_mask_logits_kernel, called by every thread of the CTA (it holds a barrier):
+// z = b[l] + sum_c W[l,c] y[row,c,q] of pixel q = q0 + tid, returned to the threads tid < nq (0 elsewhere).  Each
+// channel group cg sums its channels c = cg, cg + NG, ... with fma in ascending order, V pixels a thread, into
+// s_red[cg]; then the NG groups are added in order and the bias last.  ybase: y's element offset of (row, 0, q0).
+template <bool BF16, int V>
+__device__ __forceinline__ float mask_logit(const void* y, long long ybase, const float* wl, const float* bias, long long l,
+                                            int Cin, int HW, int nq, float (*s_red)[kMaskTile]) {
+  constexpr int QV = kMaskTile / V;            // threads along the tile's pixels
+  constexpr int NG = kMaskThreads / QV;        // channel groups
+  const int tid = threadIdx.x, qv = tid % QV, cg = tid / QV;
+  float acc[V];
+#pragma unroll
+  for (int v = 0; v < V; ++v) acc[v] = 0.f;
+  if (qv * V < nq) {   // V = 4 only when HW % 4 == 0, so the whole vector is inside the tile
+#pragma unroll 4
+    for (int c = cg; c < Cin; c += NG) {
+      const float wc = __ldg(wl + c);
+      float yv[V];
+      mask_load<BF16, V>(y, ybase + static_cast<long long>(c) * HW + qv * V, yv);
+#pragma unroll
+      for (int v = 0; v < V; ++v) acc[v] = fmaf(wc, yv[v], acc[v]);
+    }
+  }
+#pragma unroll
+  for (int v = 0; v < V; ++v) s_red[cg][qv * V + v] = acc[v];
+  __syncthreads();
+  float z = 0.f;
+  if (tid < nq) {
+#pragma unroll 4
+    for (int k = 0; k < NG; ++k) z += s_red[k][tid];
+    if (bias != nullptr) z += __ldg(bias + l);
+  }
+  return z;
 }
 
 __global__ void __launch_bounds__(kBoxThreads)
@@ -88,32 +135,11 @@ bags_mask_fwd_kernel(const MaskFwdParams p) {
   float* rs = p.rsum + (static_cast<long long>(pr) * p.tiles + t) * (p.Cin + 1);
   float tile_loss = 0.f;
   if (mask_valid(l, p.classes)) {   // CTA-uniform
-    // pass 1: per channel group, sum_c W[l,c] y[p,c,q] over its channels; then the groups in order
-    const int qv = tid % QV, cg = tid / QV;
-    const float* wl = p.w + l * p.ldw;
-    float acc[V];
-#pragma unroll
-    for (int v = 0; v < V; ++v) acc[v] = 0.f;
-    if (qv * V < nq) {   // V = 4 only when HW % 4 == 0, so the whole vector is inside the tile
-#pragma unroll 4
-      for (int c = cg; c < p.Cin; c += NG) {
-        const float wc = __ldg(wl + c);
-        float yv[V];
-        mask_load<BF16, V>(p.y, ybase + static_cast<long long>(c) * p.HW + qv * V, yv);
-#pragma unroll
-        for (int v = 0; v < V; ++v) acc[v] = fmaf(wc, yv[v], acc[v]);
-      }
-    }
-#pragma unroll
-    for (int v = 0; v < V; ++v) s_red[cg][qv * V + v] = acc[v];
-    __syncthreads();
+    // pass 1: z of the tile's pixels
+    const float z = mask_logit<BF16, V>(p.y, ybase, p.w + l * p.ldw, p.bias, l, p.Cin, p.HW, nq, s_red);
     if (tid < kMaskTile) {
       float gq = 0.f, lq = 0.f;
       if (tid < nq) {
-        float z = 0.f;
-#pragma unroll 4
-        for (int k = 0; k < NG; ++k) z += s_red[k][tid];
-        if (p.bias != nullptr) z += __ldg(p.bias + l);
         const long long o = static_cast<long long>(pr) * p.HW + q0 + tid;
         const float tq = __ldg(p.targets + o);
         // F.binary_cross_entropy_with_logits: max(z, 0) - z t + log1p(exp(-|z|)); d/dz = sigmoid(z) - t
@@ -173,6 +199,27 @@ bags_mask_fwd_kernel(const MaskFwdParams p) {
     for (int w = 0; w < kMaskThreads / 32; ++w) total += s_warp[w];
     *p.loss = total / p.n;
     *p.counter = 0u;
+  }
+}
+
+template <bool BF16, int V>
+__global__ void __launch_bounds__(kMaskThreads, 4)
+bags_mask_logits_kernel(const MaskLogitsParams p) {
+  constexpr int NG = kMaskThreads / (kMaskTile / V);
+  __shared__ float s_red[NG][kMaskTile];
+  const int tid = threadIdx.x;
+  const int d = blockIdx.x / p.tiles, t = blockIdx.x % p.tiles;
+  const int q0 = t * kMaskTile, nq = min(kMaskTile, p.HW - q0);
+  const long long c = __ldg(p.channels + d);
+  float z = __int_as_float(0x7fc00000);   // an invalid channel: a map of NaN, nothing of W, b or y read
+  if (mask_valid(c, p.classes)) {         // CTA-uniform
+    const long long ybase = static_cast<long long>(d) * p.Cin * p.HW + q0;
+    z = mask_logit<BF16, V>(p.y, ybase, p.w + c * p.ldw, p.bias, c, p.Cin, p.HW, nq, s_red);
+  }
+  if (tid < nq) {
+    const long long o = static_cast<long long>(d) * p.HW + q0 + tid;
+    if constexpr (BF16) reinterpret_cast<__nv_bfloat16*>(p.out)[o] = __float2bfloat16_rn(z);
+    else                reinterpret_cast<float*>(p.out)[o] = z;
   }
 }
 

@@ -8,10 +8,13 @@ configs/bags/gs_mask_rcnn_r50_fpn_1x_lvis.py and configs/bags/gs_htc_*.py build 
     HTCMaskHead     mmdet/models/mask_heads/htc_mask_head.py:7-38
     ConvModule      mmdet/models/utils/conv_module.py (only conv_cfg=None, norm_cfg=None: biased conv, ReLU, kaiming)
 
-The 3x3 convs and the deconv stay ``nn.Conv2d`` / ``nn.ConvTranspose2d``.  What differs is the training loss: a
-training ``forward`` returns a lazy ``MaskPredHandle`` for ``mask_pred`` and ``loss`` computes only the channel of
-each RoI's label inside its BCE (``ops.MaskBCEFunction``) instead of conv_logits' [P, num_classes, 28, 28] logits.
-Everything else -- an eval-mode ``forward``, a materialised handle, another ``loss_mask`` -- runs the reference's ops.
+The 3x3 convs and the deconv stay ``nn.Conv2d`` / ``nn.ConvTranspose2d``.  What differs is conv_logits: on a GPU, a
+training ``forward`` (with autograd) and an eval ``forward`` return a lazy ``MaskPredHandle`` for ``mask_pred``
+instead of its [n, num_classes, 28, 28] logits.  ``loss`` computes only the channel of each RoI's label inside its
+BCE (``ops.MaskBCEFunction``); at test time ``get_seg_masks`` / ``get_seg_masks_without`` and HTC's
+``mask_pred.gather(1, labels)`` compute only each detection's channel (``ops.mask_channel_logits``) when no gradient
+is recorded.  Everything else -- a CPU input, a materialised handle, another ``loss_mask``, multi-scale testing's
+``mask_pred.sigmoid()`` -- runs the reference's ops on the materialised logits.
 """
 from __future__ import annotations
 
@@ -75,11 +78,12 @@ class ConvModule(nn.Module):
 
 # --------------------------------------------------------------------------- lazy logits
 class MaskPredHandle(_LazyHandle):
-    """What a mask head's training ``forward`` returns for ``mask_pred``.
+    """What a mask head's ``forward`` returns for ``mask_pred`` on a GPU, in training with autograd and in eval.
 
-    It records the input ``y`` of ``conv_logits``, so that ``loss`` can compute only the channel of each RoI's label
-    inside mask_cross_entropy (``ops.MaskBCEFunction``) instead of the [P, num_classes, H, W] logits.  ``tensor()`` (or
-    any tensor attribute access, indexing or torch function) materialises them through ``conv_logits``,
+    It records the input ``y`` of ``conv_logits``, so that its consumers can compute only the channel each RoI or
+    detection reads instead of the [n, num_classes, H, W] logits: ``loss`` inside mask_cross_entropy
+    (``ops.MaskBCEFunction``), ``seg_masks`` and ``gather`` at test time (``channel_logits``).  ``tensor()`` (or any
+    other tensor attribute access, indexing or torch function) materialises them through ``conv_logits``,
     autograd-connected."""
 
     y = property(lambda self: self.input)          # earlier names, as in ClsScoreHandle
@@ -91,6 +95,44 @@ class MaskPredHandle(_LazyHandle):
 
     def _project(self):
         return self._head.conv_logits(self.input)
+
+    def label_only(self) -> bool:
+        """True when ``channel_logits`` may stand in for the dense logits: the handle is pending, y is a bf16 or fp32
+        CUDA tensor, and autograd would record nothing of conv_logits(y) (grad mode off, or none of y, the weight and
+        the bias requires grad)."""
+        conv = self._head.conv_logits
+        y = self.input
+        recorded = torch.is_grad_enabled() and any(t is not None and t.requires_grad
+                                                   for t in (y, conv.weight, conv.bias))
+        return self.pending and y.is_cuda and y.dtype in (torch.bfloat16, torch.float32) and not recorded
+
+    def channel_logits(self, channels: torch.Tensor) -> torch.Tensor:
+        """[n, 1, H, W] logits of channel ``channels[d]`` (int64 [n]) of each row d, without the dense tensor
+        (``ops.mask_channel_logits``; NaN for a channel outside [0, num_classes)).  The handle stays pending."""
+        conv = self._head.conv_logits
+        return ops.mask_channel_logits(self.input, conv.weight, conv.bias, channels)
+
+    def gather(self, dim, index, *, sparse_grad=False, out=None):
+        """Tensor.gather on the logits.  HTC's test path (htc.py:403-421) gathers each detection's label channel with
+        ``labels.expand(-1, -1, H, W)``: an int64 [n, 1, H, W] index on y's device that is constant along H and W
+        (stride 0 or size 1) takes ``channel_logits(index[:, 0, 0, 0])`` when ``label_only()``.  Anything else
+        gathers from the materialised logits."""
+        y = self.input
+        if (dim == 1 and not sparse_grad and out is None and isinstance(index, torch.Tensor)
+                and index.dtype == torch.int64 and index.device == y.device and index.dim() == 4
+                and index.shape[:2] == (y.shape[0], 1) and index.shape[2:] == y.shape[2:]
+                and all(index.stride(i) == 0 or index.size(i) == 1 for i in (2, 3)) and self.label_only()):
+            return self.channel_logits(index[:, 0, 0, 0])
+        kw = {} if out is None else dict(out=out)
+        return torch.gather(self.tensor(), dim, index, sparse_grad=sparse_grad, **kw)
+
+    @classmethod
+    def __torch_function__(cls, func, types, args=(), kwargs=None):
+        """torch.gather(handle, ...) and Tensor.gather(handle, ...) go to ``gather``; every other function sees the
+        materialised logits."""
+        if func in (torch.gather, torch.Tensor.gather) and args and isinstance(args[0], MaskPredHandle):
+            return args[0].gather(*args[1:], **(kwargs or {}))
+        return super().__torch_function__(func, types, args, kwargs)
 
 
 def _cfg_get(cfg, key):
@@ -177,7 +219,17 @@ def seg_masks(mask_pred, det_bboxes, det_labels, rcnn_test_cfg, ori_shape, scale
 
     With detections on the GPU this runs natively (``ops.seg_masks_rle``; BAGS_SEGM_NATIVE=0 turns it off): same
     masks, no pycocotools, three host syncs whatever n is.  A box that leaves the image takes the host loop, whose numpy
-    slicing decides what such a paste gives."""
+    slicing decides what such a paste gives.
+
+    A ``MaskPredHandle`` (an eval ``forward`` on a GPU) gives only the channel each detection reads
+    (``channel_logits``) when ``label_only()``; otherwise its materialised logits."""
+    if isinstance(mask_pred, MaskPredHandle):
+        if mask_pred.label_only():
+            channel = det_labels + 1 if label_channel else torch.zeros_like(det_labels)
+            mask_pred = mask_pred.channel_logits(channel.to(mask_pred.device, torch.int64))
+            label_channel = False
+        else:
+            mask_pred = mask_pred.tensor()
     on_gpu = isinstance(mask_pred, np.ndarray) or (isinstance(mask_pred, torch.Tensor) and mask_pred.is_cuda)
     if (os.environ.get('BAGS_SEGM_NATIVE', '1') != '0' and on_gpu and isinstance(det_bboxes, torch.Tensor)
             and det_bboxes.is_cuda):
@@ -288,8 +340,9 @@ class FCNMaskHead(nn.Module):
             nn.init.constant_(m.bias, 0)
 
     def _logits(self, x):
-        """conv_logits(x) -- or, in training with autograd on a GPU, the lazy handle the fused loss consumes."""
-        if self.training and torch.is_grad_enabled() and x.is_cuda:
+        """conv_logits(x) -- or, on a GPU, the lazy handle: in training with autograd for the fused loss, in eval for the
+        label-only test-time logits of seg_masks and MaskPredHandle.gather."""
+        if x.is_cuda and (not self.training or torch.is_grad_enabled()):
             return MaskPredHandle(self, x)
         return self.conv_logits(x)
 

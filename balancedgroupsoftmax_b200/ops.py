@@ -276,6 +276,32 @@ def mask_bwd(g, rsum, gout, w, labels, index, y_shape, y_dtype, need_dw: bool = 
     return dW, db, dY
 
 
+def mask_channel_logits(y, weight, bias, channels):
+    """bags_mask_logits: [n, 1, H, W] logits in y's dtype of one conv_logits channel per row, channel ``channels[d]``
+    of row d -- what conv_logits(y).gather(1, channels[:, None, None, None].expand(-1, 1, H, W)) selects, without the
+    [n, classes, H, W] tensor.  fp32 products from the fp32 weight, summed in bags_mask_fwd's order.  ``y``: bf16 or
+    fp32 [n, Cin, H, W] (made contiguous); ``weight``: conv_logits.weight ([classes, Cin, 1, 1] or [classes, Cin]);
+    ``bias``: [classes] or None; ``channels``: int64 [n] on y's device.  A channel outside [0, classes) gives a map of
+    NaN.  Not differentiable: for callers that record no gradient."""
+    _require_cuda(y, weight, bias, channels)
+    y = y.contiguous()
+    n, Cin, H, W_ = y.shape
+    _, w, bias = _fp32_master_operands(y, weight, bias)
+    w = _row_major(w.reshape(w.shape[0], -1))
+    classes = w.shape[0]
+    if bias is not None:
+        assert bias.numel() == classes, 'mask_channel_logits: bias must be [classes]'
+        bias = bias.contiguous()
+    assert w.shape[1] == Cin, 'mask_channel_logits: weight is [%d, %d], y has %d channels' % (classes, w.shape[1], Cin)
+    assert channels.dtype == torch.int64 and channels.numel() == n, 'mask_channel_logits: channels must be int64 [n]'
+    channels = channels.contiguous()
+    out = torch.empty((n, 1, H, W_), dtype=y.dtype, device=y.device)
+    nat.check(nat.lib().bags_mask_logits(
+        y.data_ptr(), _dtype_code(y.dtype), w.data_ptr(), w.stride(0), nat.ptr(bias), channels.data_ptr(), n, Cin,
+        H * W_, classes, out.data_ptr(), _stream_ptr(y.device)), 'bags_mask_logits')
+    return out
+
+
 def _fused_outputs(x, w, bias, G: int, want_acc: bool, want_dz: bool, want_colsum: bool,
                    clear: Optional[torch.Tensor], acc_out: Optional[torch.Tensor] = None):
     """Operands and outputs shared by bags_fwd, bags_ce_fwd and bags_focal_fwd: row-major x and w of one dtype, the

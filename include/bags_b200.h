@@ -26,6 +26,8 @@
  *     bbox_head.py:118-128, smooth_l1_loss.py
  *   conv_logits + mask_cross_entropy (class-specific)  bags_mask_fwd / bags_mask_bwd
  *     fcn_mask_head.py:82,102,114-123, cross_entropy_loss.py:54-61
+ *   conv_logits + the label channel of each detection     bags_mask_logits
+ *     (test time) fcn_mask_head.py:125-181, htc.py:403-421
  *   autograd backward of the above (dW, db, dX)           bags_bwd
  *     triggered at mmdet/core/utils/dist_utils.py:53
  *   GSBBoxHeadWith0._merge_score                          bags_merge_scores
@@ -242,6 +244,19 @@ int bags_mask_fwd(const void* y, int dtype, const float* w, long long ldw, const
 int bags_mask_bwd(const float* g, const float* rsum, const float* gout, int dtype, const float* w, long long ldw,
                   const int64_t* labels, const int32_t* index, int P, int Cin, int HW, int classes, float* dW,
                   long long lddw, float* db, void* dY, void* stream);
+
+/* Test-time mask logits of one channel per detection -- replaces, where the caller reads only channel c_d of each
+ * detection d, conv_logits' 1x1 conv into [n, classes, H, W] (fcn_mask_head.py:82,102) followed by the channel
+ * selection of get_seg_masks (mask_pred[i, label], fcn_mask_head.py:125-181) or HTC's mask_pred.gather(1, labels)
+ * (htc.py:403-421):
+ *   out[d, q] = bias[c_d] + sum_k W[c_d, k] y[d, k, q]        c_d = channels[d], q < HW = H * W
+ * with fp32 products and accumulation from the fp32 W, in the summation order of bags_mask_fwd's logits, rounded once
+ * to y's dtype.  y: contiguous [n, Cin, HW] bf16 or fp32 (dtype); W: [classes, Cin] fp32 (ldw >= Cin); bias: [classes]
+ * fp32 or NULL; channels: int64 [n] (device); out: contiguous [n, HW] in y's dtype.  A channel outside [0, classes)
+ * gives a row of NaN and reads nothing of W, bias or y.  1 <= classes <= 8192.  One launch, no host sync, no atomics;
+ * y is read from memory once.  n == 0: nothing is launched. */
+int bags_mask_logits(const void* y, int dtype, const float* w, long long ldw, const float* bias, const int64_t* channels,
+                     int n, int Cin, int HW, int classes, void* out, void* stream);
 
 /* ---- reweight head variant (GSBBoxHeadWith0Reweight, mmdet/models/bbox_heads/gs_bbox_head_with0_reweight.py:57-109):
  * per-(bin, RoI) fp32 weights instead of 0/1 masks, consumed by bags_fwd / bags_group_ce as BAGS_WEIGHTS_F32. ----

@@ -61,6 +61,7 @@ SIGNATURES = {
     'bags_grad_allreduce': (_i, [_vp, _vp, _ll, _ll, _i, _i, C.c_float, _i, _vp]),
     'bags_class_nms_dense': (_i, [_vp, _i, _vp, _vp, _i, _i, C.c_float, _vp, _vp, _vp]),
     'bags_segm_rle': (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _i, C.c_double, _vp, _vp, _vp]),
+    'bags_mask_target': (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _vp, _vp]),
     'bags_debug_spin': (_i, [_i, _i, _i, _vp]),
     'bags_cast_bf16': (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp]),
     'bags_linear_act_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _vp]),

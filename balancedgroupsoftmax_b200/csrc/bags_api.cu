@@ -22,6 +22,7 @@
 #include "bags_box.cuh"
 #include "bags_mask.cuh"
 #include "bags_segm.cuh"
+#include "bags_mask_target.cuh"
 
 using namespace bags;
 
@@ -1267,6 +1268,59 @@ extern "C" int bags_segm_rle(const float* probs, int n, int mask_h, int mask_w, 
   bags_segm_rle_kernel<<<n, kSegmThreads, 0, stream>>>(probs, mask_h, mask_w, reinterpret_cast<const int4*>(boxes),
                                                        img_h, img_w, thr, reinterpret_cast<long long*>(lengths), out);
   BAGS_CUDA(cudaGetLastError());
+  return BAGS_OK;
+}
+
+// ----------------------------------------------------------------------------
+// training mask targets (see bags_mask_target.cuh)
+// ----------------------------------------------------------------------------
+extern "C" int bags_mask_target(const float* const* boxes_host, const int64_t* const* gt_inds_host,
+                                const uint8_t* const* masks_host, const int32_t* sizes_host, int n_images, int mask_h,
+                                int mask_w, float* out, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  BAGS_REQUIRE(n_images >= 0, "bags_mask_target: n_images = %d < 0", n_images);
+  BAGS_REQUIRE(mask_h >= 1 && mask_w >= 1 && mask_h <= kMaskTargetMaxSize && mask_w <= kMaskTargetMaxSize,
+               "bags_mask_target: mask size %d x %d outside [1, %d]", mask_h, mask_w, kMaskTargetMaxSize);
+  if (n_images == 0) return BAGS_OK;
+  BAGS_REQUIRE(boxes_host && gt_inds_host && masks_host && sizes_host, "bags_mask_target: NULL argument");
+  long long rows = 0;
+  for (int i = 0; i < n_images; ++i) {
+    const int32_t* s = sizes_host + 4 * static_cast<size_t>(i);
+    BAGS_REQUIRE(s[0] >= 0 && s[1] >= 0 && s[2] >= 0 && s[3] >= 0,
+                 "bags_mask_target: image %d has a negative size (num_pos %d, num_gt %d, H %d, W %d)", i, s[0], s[1],
+                 s[2], s[3]);
+    BAGS_REQUIRE(s[0] == 0 || (boxes_host[i] && gt_inds_host[i]), "bags_mask_target: image %d: NULL boxes or gt_inds",
+                 i);
+    BAGS_REQUIRE(static_cast<long long>(s[1]) * s[2] * s[3] == 0 || masks_host[i],
+                 "bags_mask_target: image %d: NULL masks", i);
+    BAGS_REQUIRE(s[0] == 0 || (aligned(boxes_host[i], 4) && aligned(gt_inds_host[i], 8)),
+                 "bags_mask_target: image %d: boxes must be 4-byte and gt_inds 8-byte aligned", i);
+    rows += s[0];
+  }
+  BAGS_REQUIRE(rows <= 0x7fffffffLL, "bags_mask_target: %lld positive RoIs: at most 2^31 - 1", rows);
+  if (rows == 0) return BAGS_OK;
+  BAGS_REQUIRE(out, "bags_mask_target: NULL argument");
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  // the per-image table travels as a kernel argument: kMaskTargetMaxImages images per launch
+  long long done = 0;
+  for (int i0 = 0; i0 < n_images; i0 += kMaskTargetMaxImages) {
+    MaskTargetParams p{};
+    p.n_images = n_images - i0 < kMaskTargetMaxImages ? n_images - i0 : kMaskTargetMaxImages;
+    p.mask_h = mask_h;
+    p.mask_w = mask_w;
+    p.out = out + done * mask_h * mask_w;
+    int begin = 0;
+    for (int k = 0; k < p.n_images; ++k) {
+      const int32_t* s = sizes_host + 4 * static_cast<size_t>(i0 + k);
+      p.img[k] = MaskTargetImage{boxes_host[i0 + k], reinterpret_cast<const long long*>(gt_inds_host[i0 + k]),
+                                 masks_host[i0 + k], begin, s[1], s[2], s[3]};
+      begin += s[0];
+    }
+    if (begin > 0) bags_mask_target_kernel<<<begin, kMaskTargetThreads, 0, stream>>>(p);
+    BAGS_CUDA(cudaGetLastError());
+    done += begin;
+  }
   return BAGS_OK;
 }
 

@@ -175,9 +175,23 @@ def mask_target_single(pos_proposals, pos_assigned_gt_inds, gt_masks, cfg):
     return torch.from_numpy(np.stack(crops)).float().to(pos_proposals.device)
 
 
+def _native_mask_target(pos_proposals_list, gt_masks_list) -> bool:
+    """True when ``mask_target`` takes ``ops.mask_targets``: the positive proposals are on a GPU, every gt mask is a
+    uint8 [num_gt, H, W] CUDA tensor, and BAGS_MASK_TARGET_NATIVE is not 0."""
+    return (os.environ.get('BAGS_MASK_TARGET_NATIVE', '1') != '0' and len(pos_proposals_list) > 0
+            and all(isinstance(p, torch.Tensor) and p.is_cuda for p in pos_proposals_list)
+            and all(isinstance(m, torch.Tensor) and m.is_cuda and m.dtype == torch.uint8 and m.dim() == 3
+                    for m in gt_masks_list))
+
+
 def mask_target(pos_proposals_list, pos_assigned_gt_inds_list, gt_masks_list, cfg):
-    """mmdet's own ``mask_target`` when mmdet is importable, otherwise ``mask_target_single`` per image,
-    concatenated."""
+    """The mask heads' training targets.  With the proposals and the gt masks on a GPU, ``ops.mask_targets`` builds
+    them in one launch, bitwise as the host loop, with no host sync (a gt index outside the image's masks, or a box the
+    slicing leaves empty, gives a row of NaN where the host loop raises).  Otherwise mmdet's own ``mask_target`` when
+    mmdet is importable, or ``mask_target_single`` per image, concatenated."""
+    if _native_mask_target(pos_proposals_list, gt_masks_list):
+        return ops.mask_targets(pos_proposals_list, pos_assigned_gt_inds_list, gt_masks_list,
+                                _pair(_cfg_get(cfg, 'mask_size')))
     ext = _mmdet_core('mask_target')
     if ext is not None:  # pragma: no cover
         return ext(pos_proposals_list, pos_assigned_gt_inds_list, gt_masks_list, cfg)

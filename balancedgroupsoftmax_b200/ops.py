@@ -638,6 +638,65 @@ def seg_masks_rle(probs: torch.Tensor, boxes: np.ndarray, img_h: int, img_w: int
     return [data[e - l:e] for e, l in zip(ends.tolist(), lens.tolist())]
 
 
+def upload_masks(gt_masks_list, device) -> list:
+    """uint8 [num_gt, H, W] gt masks of each image on ``device``: CUDA tensors there as they are (made contiguous),
+    everything else (mmdet's numpy masks) packed into one pinned host tensor and uploaded with one non-blocking copy.
+    The caching host allocator keeps the pinned tensor until the copy has run, so nothing waits for it."""
+    out = [None] * len(gt_masks_list)
+    host = []
+    for i, m in enumerate(gt_masks_list):
+        if isinstance(m, torch.Tensor) and m.is_cuda:
+            if m.device != torch.device(device) or m.dtype != torch.uint8 or m.dim() != 3:
+                raise nat.BagsNativeError('mask_targets: CUDA gt masks must be uint8 [num_gt, H, W] on %s (got %s %s on '
+                                          '%s)' % (device, m.dtype, tuple(m.shape), m.device))
+            out[i] = m.contiguous()
+        else:
+            a = np.asarray(m.cpu() if isinstance(m, torch.Tensor) else m)
+            if a.dtype != np.uint8 or a.ndim != 3:
+                raise nat.BagsNativeError('mask_targets: gt masks must be uint8 [num_gt, H, W] (got %s %s)'
+                                          % (a.dtype, a.shape))
+            host.append((i, a))
+    if host:
+        staging = torch.empty((sum(a.size for _, a in host),), dtype=torch.uint8, pin_memory=True)
+        flat, at = staging.numpy(), 0
+        for _, a in host:
+            flat[at:at + a.size].reshape(a.shape)[...] = a
+            at += a.size
+        dev_buf, at = staging.to(device, non_blocking=True), 0
+        for i, a in host:
+            out[i] = dev_buf[at:at + a.size].view(a.shape)
+            at += a.size
+    return out
+
+
+def mask_targets(pos_proposals_list, pos_assigned_gt_inds_list, gt_masks_list, mask_size) -> torch.Tensor:
+    """bags_mask_target: the mask heads' training targets (mmdet/core/mask/mask_target.py) of every image in one
+    launch -- each positive RoI's gt mask cut to its proposal box (truncated to int32, at least one pixel wide and
+    high, numpy slice rules) and resized to ``mask_size`` as cv2.resize(uint8, INTER_LINEAR) does, bitwise.  float32
+    [sum P, h, w] on the proposals' device, images in order.  ``pos_proposals_list``: [P, >= 4] CUDA boxes per image;
+    ``pos_assigned_gt_inds_list``: [P] integer gt indices; ``gt_masks_list``: uint8 [num_gt, H, W] per image, CUDA
+    tensors (read in place) or numpy arrays (``upload_masks``).  A gt index outside [0, num_gt) or a crop the slicing
+    leaves empty gives a row of NaN.  No host sync: with CUDA masks it can be captured in a CUDA graph."""
+    mh, mw = (mask_size, mask_size) if isinstance(mask_size, int) else tuple(mask_size)
+    n = len(pos_proposals_list)
+    if not (len(pos_assigned_gt_inds_list) == len(gt_masks_list) == n) or n == 0:
+        raise nat.BagsNativeError('mask_targets: one proposal tensor, gt index tensor and mask array per image '
+                                  '(got %d, %d, %d)' % (n, len(pos_assigned_gt_inds_list), len(gt_masks_list)))
+    _require_cuda(*pos_proposals_list, *pos_assigned_gt_inds_list)
+    dev = pos_proposals_list[0].device
+    boxes = [p[:, :4].float().contiguous() for p in pos_proposals_list]
+    gt_inds = [g.to(torch.int64).contiguous() for g in pos_assigned_gt_inds_list]
+    masks = upload_masks(gt_masks_list, dev)
+    sizes = np.array([(b.shape[0], m.shape[0], m.shape[1], m.shape[2]) for b, m in zip(boxes, masks)], dtype=np.int32)
+    if any(g.numel() != b.shape[0] for b, g in zip(boxes, gt_inds)):
+        raise nat.BagsNativeError('mask_targets: one gt index per positive proposal')
+    out = torch.empty((int(sizes[:, 0].sum()), mh, mw), dtype=torch.float32, device=dev)
+    ptrs = lambda ts: (C.c_void_p * n)(*[t.data_ptr() if t.numel() else None for t in ts])   # noqa: E731
+    nat.check(nat.lib().bags_mask_target(ptrs(boxes), ptrs(gt_inds), ptrs(masks), sizes.ctypes.data, n, mh, mw,
+                                         out.data_ptr(), _stream_ptr(dev)), 'bags_mask_target')
+    return out
+
+
 def gemm_probe(a, a_mn: bool, b, b_mn: bool, M: int, N: int, K: int, block_n: int = 256, splits: int = 1,
                epi: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Test hook for one wgmma GEMM (see bags_gemm_probe)."""

@@ -34,6 +34,8 @@
  *     gs_bbox_head_with0.py:239-273
  *   FCNMaskHead.get_seg_masks: resize, paste, RLE     bags_segm_rle
  *     fcn_mask_head.py:125-239
+ *   FCNMaskHead.get_target: crop + resize gt masks    bags_mask_target
+ *     mmdet/core/mask/mask_target.py
  *   allreduce_grads / _allreduce_coalesced                bags_grad_allreduce
  *     mmdet/core/utils/dist_utils.py:9-41
  *
@@ -345,6 +347,25 @@ int bags_class_nms_dense(const float* boxes, int box_cols, const int32_t* order,
  * sync; the caller reads the lengths back between the passes. */
 int bags_segm_rle(const float* probs, int n, int mask_h, int mask_w, const int32_t* boxes_host, int32_t* boxes,
                   int img_h, int img_w, double thr, int64_t* lengths, char* out, void* stream);
+
+/* Training mask targets -- replaces the per-RoI loop of mask_target / mask_target_single
+ * (mmdet/core/mask/mask_target.py: boxes and gt indices to the host, gt_masks[gt][y1:y1 + h, x1:x1 + w] per RoI,
+ * mmcv.imresize to mask_size, a stacked float upload).  For image i and its positive RoI r:
+ *   (x1, y1, x2, y2) = boxes[r] truncated as numpy's astype(np.int32), w = max(x2 - x1 + 1, 1), h likewise
+ *   crop = masks[gt_inds[r]][y1:y1 + h, x1:x1 + w] by numpy's slice rules (a negative start counts from the end)
+ *   out[row] = cv2.resize(crop, (mask_w, mask_h), INTER_LINEAR) as float, bitwise (8-bit fixed point; a crop of
+ *              exactly the output size is copied, one of exactly twice it on both axes is averaged over 2 x 2 blocks)
+ * with rows of image i after those of the images before it.  A gt index outside [0, num_gt), or a crop the slicing
+ * leaves empty (where the reference raises), gives a row of NaN.  Any uint8 mask values, not only 0 / 1.
+ *   boxes_host   HOST array [n_images] of device fp32 [num_pos, 4] (x1, y1, x2, y2), 4-byte aligned
+ *   gt_inds_host HOST array [n_images] of device int64 [num_pos], 8-byte aligned
+ *   masks_host   HOST array [n_images] of device uint8 [num_gt, H, W], contiguous
+ *   sizes_host   int32 [n_images, 4]: (num_pos, num_gt, H, W), each >= 0
+ *   out          device fp32 [sum num_pos, mask_h, mask_w]; 1 <= mask_h, mask_w <= 256
+ * Pointers of an image without positives (boxes, gt_inds) or without mask pixels (masks) may be NULL.  One launch per
+ * 64 images, no host sync, nothing read on the host from the device: capturable in a CUDA graph. */
+int bags_mask_target(const float* const* boxes_host, const int64_t* const* gt_inds_host, const uint8_t* const* masks_host,
+                     const int32_t* sizes_host, int n_images, int mask_h, int mask_w, float* out, void* stream);
 
 /* test hook: launch `blocks` x `threads` threads that wait `micros` microseconds and exit */
 int bags_debug_spin(int blocks, int threads, int micros, void* stream);

@@ -8,13 +8,10 @@
     N * 1231, the weight broadcast, the three reductions, the op's gradient, and the edge cases;
   * both focal configs' heads against the committed fixture tests/golden/focal_head_ref_n256.npz;
   * the registry building the bbox_head blocks of the three focal configs;
-  * bags_focal_fwd's argument validation (error codes and messages, never exceptions);
-  * the focal kernel's registers: no spills and no serialised wgmma (ptxas -v).
+  * bags_focal_fwd's argument validation (error codes and messages, never exceptions).
 """
 import ctypes as C
 import os
-import re
-import subprocess
 import tempfile
 
 import numpy as np
@@ -225,37 +222,3 @@ def test_focal_fwd_invalid_arguments_return_error_codes():
         assert call(norm=bad) == -1 and b'norm' in lib.bags_last_error(), bad
     assert call(colsum=p, tiles=2) == -1 and b'colsum' in lib.bags_last_error()
     check_fused_operand_rules(lib, 'bags_focal_fwd', call, base)
-
-
-# --------------------------------------------------------------------------- registers
-FOCAL = re.compile(r'bags_focal_fwd_kernel')
-
-
-def test_focal_kernel_fits_its_registers():
-    """ptxas: every bags_focal_fwd_kernel instantiation (bf16, tf32) without spills and without serialised wgmma
-    (warnings C7512 / C7518 ...)."""
-    from balancedgroupsoftmax_b200 import build as B
-    try:
-        nvcc = B._nvcc()
-    except RuntimeError:
-        pytest.skip('nvcc not found')
-    with tempfile.TemporaryDirectory() as tmp:
-        cmd = [nvcc, '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-cubin', '-Xptxas', '-v',
-               '-o', os.path.join(tmp, 'bags_api.cubin')] + B.SOURCES
-        res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert res.returncode == 0, res.stdout
-    found, cur = {}, None
-    serialised = set(re.findall(r"\(C75\d\d\) Potential Performance Loss: wgmma.*'([^']+)'", res.stdout))
-    for line in res.stdout.splitlines():
-        m = re.search(r'Function properties for (\S+)', line)
-        if m:
-            cur = m.group(1)
-            continue
-        m = re.search(r'(\d+) bytes spill stores, (\d+) bytes spill loads', line)
-        if m and cur is not None:
-            if FOCAL.search(cur):
-                found[cur] = (int(m.group(1)), int(m.group(2)), cur in serialised)
-            cur = None
-    assert len(found) == 2, found   # {bf16, tf32}
-    bad = {name: r for name, r in found.items() if r != (0, 0, False)}
-    assert not bad, '(spill store bytes, spill load bytes, wgmma serialised): %s' % bad

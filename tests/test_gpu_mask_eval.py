@@ -19,11 +19,7 @@ into NaN.  The elements past ``out`` hold a sentinel that must survive.  A chann
 NaN (the dense route's torch.gather would raise a device-side assert there).
 """
 import ctypes as C
-import os
-import re
-import subprocess
 import sys
-import tempfile
 import types
 
 import numpy as np
@@ -209,40 +205,6 @@ def test_abi_rejects_bad_arguments():
         assert call(**kw) == -1 and b'bad shape' in lib.bags_last_error(), kw
     assert call(classes=0) == -1 and b'classes' in lib.bags_last_error()
     assert call(n=0) == 0 and call(n=0, y=None, w=None, ch=None, out=None) == 0
-
-
-def test_kernel_fits_its_registers():
-    """ptxas -v reports no spills for the four instantiations of bags_mask_logits_kernel (parsed as in
-    test_kernel_resources.py); the file is bags_mask.cuh with only these kernels instantiated."""
-    from balancedgroupsoftmax_b200 import build as B
-    try:
-        nvcc = B._nvcc()
-    except RuntimeError:
-        pytest.skip('nvcc not found')
-    inst = ''.join('template __global__ void bags::bags_mask_logits_kernel<%s, %d>(const bags::MaskLogitsParams);\n'
-                   % (bf, v) for bf in ('true', 'false') for v in (4, 1))
-    with tempfile.TemporaryDirectory() as tmp:
-        src = os.path.join(tmp, 'mask_logits.cu')
-        with open(src, 'w') as f:
-            f.write('#include "bags_mask.cuh"\n' + inst)
-        cmd = [nvcc, '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-std=c++17', '-cubin', '-Xptxas', '-v',
-               '-I', B.CSRC,
-               '-o', os.path.join(tmp, 'mask_logits.cubin'), src]
-        res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
-    assert res.returncode == 0, res.stdout
-    spills, cur = {}, None
-    for line in res.stdout.splitlines():
-        m = re.search(r'Function properties for (\S+)', line)
-        if m:
-            cur = m.group(1)
-            continue
-        m = re.search(r'(\d+) bytes spill stores, (\d+) bytes spill loads', line)
-        if m and cur is not None:
-            spills[cur] = (int(m.group(1)), int(m.group(2)))
-            cur = None
-    found = {k: v for k, v in spills.items() if 'bags_mask_logits_kernel' in k}
-    assert len(found) == 4, spills
-    assert all(v == (0, 0) for v in found.values()), found
 
 
 # ------------------------------------------------------------------------------------------------ the head routes

@@ -363,7 +363,7 @@ extern "C" int bags_sample_others(const int64_t* labels, const int32_t* label2bi
                                   int classes, double ratio, uint64_t seed, const uint64_t* seed_step,
                                   uint8_t* wmask, float* avg, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  BAGS_REQUIRE(labels && label2bin && wmask && avg, "bags_sample_others: NULL argument");
+  BAGS_REQUIRE(label2bin && avg && (N == 0 || (labels && wmask)), "bags_sample_others: NULL argument");
   BAGS_REQUIRE(G >= 1 && G <= kMaxG && classes >= 1 && N >= 0, "bags_sample_others: bad shape");
   BAGS_REQUIRE(ratio >= 0.0, "bags_sample_others: negative ratio");
   const long long* lab = reinterpret_cast<const long long*>(labels);
@@ -376,7 +376,7 @@ extern "C" int bags_sample_others(const int64_t* labels, const int32_t* label2bi
 
 extern "C" int bags_mask_avg(const uint8_t* wmask, int N, int G, float* avg, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  BAGS_REQUIRE(wmask && avg, "bags_mask_avg: NULL argument");
+  BAGS_REQUIRE(avg && (N == 0 || wmask), "bags_mask_avg: NULL argument");
   BAGS_REQUIRE(G >= 1 && G <= kMaxG && N >= 0, "bags_mask_avg: bad shape");
   mask_avg_kernel<<<G, 256, 0, stream>>>(wmask, N, avg);
   BAGS_CUDA(cudaGetLastError());

@@ -92,12 +92,13 @@ size_t bags_workspace_bytes(void);
  * _sample_others does, but on the device with a counter-based RNG keyed by the effective seed
  * seed + (*seed_step) * 0x9E3779B97F4A7C15, read on the DEVICE (seed_step may be NULL: the seed as given).
  * seed_step serves CUDA-graph replays, where by-value arguments are frozen at capture time: the caller advances the
- * counter between replays (not with the kernel that immediately precedes this one in the stream). */
+ * counter between replays (not with the kernel that immediately precedes this one in the stream).
+ * An empty batch (N == 0; labels and wmask may then be NULL) sets every avg[g] to 1. */
 int bags_sample_others(const int64_t* labels, const int32_t* label2bin, int N, int G, int classes,
                        double ratio, uint64_t seed, const uint64_t* seed_step, uint8_t* wmask,
                        float* avg, void* stream);
 
-/* avg[g] = max(sum_n wmask[g,n], 1) for caller-provided masks */
+/* avg[g] = max(sum_n wmask[g,n], 1) for caller-provided masks (wmask may be NULL when N == 0) */
 int bags_mask_avg(const uint8_t* wmask, int N, int G, float* avg, void* stream);
 
 /* Per-bin softmax cross-entropy over logit slices.

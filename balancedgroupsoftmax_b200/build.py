@@ -13,7 +13,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, 'csrc')
 OUT = os.path.join(_HERE, 'libbags_b200.so')
 SOURCES = [os.path.join(CSRC, 'bags_api.cu')]
-HEADERS = [os.path.join(CSRC, f) for f in ('bags_ptx.cuh', 'bags_wgmma.cuh', 'bags_gemm.cuh', 'bags_kernels.cuh', 'bags_fused_fwd.cuh', 'bags_allreduce.cuh', 'bags_nms.cuh', 'bags_box.cuh', 'bags_mask.cuh', 'bags_segm.cuh', 'bags_mask_target.cuh')] + [
+# kernels compiled as translation units of their own and linked into the same library; bags_api.cu launches them
+# through the host launchers their headers declare
+UNITS = [os.path.join(CSRC, 'bags_roi_align.cu')]
+HEADERS = [os.path.join(CSRC, f) for f in ('bags_ptx.cuh', 'bags_wgmma.cuh', 'bags_gemm.cuh', 'bags_kernels.cuh', 'bags_fused_fwd.cuh', 'bags_allreduce.cuh', 'bags_nms.cuh', 'bags_box.cuh', 'bags_mask.cuh', 'bags_segm.cuh', 'bags_mask_target.cuh', 'bags_roi_align.cuh')] + [
     os.path.join(os.path.dirname(_HERE), 'include', 'bags_b200.h')]
 
 NVCC_FLAGS = [
@@ -33,13 +36,13 @@ def is_stale() -> bool:
     if not os.path.isfile(OUT):
         return True
     t = os.path.getmtime(OUT)
-    return any(os.path.getmtime(f) > t for f in SOURCES + HEADERS)
+    return any(os.path.getmtime(f) > t for f in SOURCES + UNITS + HEADERS)
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not is_stale():
         return OUT
-    cmd = [_nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-o', OUT] + SOURCES
+    cmd = [_nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-o', OUT] + SOURCES + UNITS
     if verbose:
         print(' '.join(cmd))
     res = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)

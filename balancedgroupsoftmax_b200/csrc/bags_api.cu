@@ -23,6 +23,7 @@
 #include "bags_mask.cuh"
 #include "bags_segm.cuh"
 #include "bags_mask_target.cuh"
+#include "bags_roi_align.cuh"
 
 using namespace bags;
 
@@ -1321,6 +1322,100 @@ extern "C" int bags_mask_target(const float* const* boxes_host, const int64_t* c
     BAGS_CUDA(cudaGetLastError());
     done += begin;
   }
+  return BAGS_OK;
+}
+
+// ----------------------------------------------------------------------------
+// FPN RoI feature extractor (see bags_roi_align.cuh; the kernels are in bags_roi_align.cu)
+// ----------------------------------------------------------------------------
+// the launch table shared by bags_roi_align_fwd and bags_roi_align_bwd; `bufs_host` are the levels' features (forward,
+// all required) or gradients (backward, NULL: no gradient for that level)
+static int roi_align_params(const char* who, RoiAlignParams& p, const void* const* bufs_host, bool bwd,
+                            const int32_t* sizes_host, const float* scales_host, int n_levels, int B, int C,
+                            const float* rois_map, const float* rois, int k, int out_h, int out_w, int sample_num,
+                            float finest_scale) {
+  BAGS_REQUIRE(n_levels >= 1 && n_levels <= kRoiAlignMaxLevels, "%s: %d levels: 1 to %d", who, n_levels,
+               kRoiAlignMaxLevels);
+  BAGS_REQUIRE(B >= 1 && C >= 1 && k >= 0, "%s: bad shape (B %d, C %d, k %d)", who, B, C, k);
+  BAGS_REQUIRE(out_h >= 1 && out_w >= 1 && out_h <= kRoiAlignMaxOut && out_w <= kRoiAlignMaxOut,
+               "%s: out size %d x %d outside [1, %d]", who, out_h, out_w, kRoiAlignMaxOut);
+  BAGS_REQUIRE(n_levels == 1 || (finest_scale > 0.f && finest_scale < INFINITY),
+               "%s: finest_scale %g must be positive and finite", who, static_cast<double>(finest_scale));
+  BAGS_REQUIRE(bufs_host && sizes_host && scales_host, "%s: NULL argument", who);
+  p = RoiAlignParams{};
+  for (int l = 0; l < n_levels; ++l) {
+    const int H = sizes_host[2 * l], W = sizes_host[2 * l + 1];
+    BAGS_REQUIRE(H >= 1 && W >= 1 && static_cast<long long>(H) * W <= 0x7fffffffLL,
+                 "%s: level %d is %d x %d: each side at least 1, at most 2^31 - 1 pixels", who, l, H, W);
+    BAGS_REQUIRE(bwd || bufs_host[l], "%s: level %d: NULL features", who, l);
+    BAGS_REQUIRE(aligned(bufs_host[l], 4), "%s: level %d: buffer not 4-byte aligned", who, l);
+    p.lvl[l].feat = bwd ? nullptr : static_cast<const float*>(bufs_host[l]);
+    p.lvl[l].grad = bwd ? static_cast<float*>(const_cast<void*>(bufs_host[l])) : nullptr;
+    p.lvl[l].H = H;
+    p.lvl[l].W = W;
+    p.lvl[l].scale = scales_host[l];
+  }
+  BAGS_REQUIRE(k == 0 || (rois_map && rois), "%s: NULL rois", who);
+  BAGS_REQUIRE(aligned(rois_map, 4) && aligned(rois, 4), "%s: rois not 4-byte aligned", who);
+  const int nbin = out_h * out_w;
+  // about 2048 outputs per CTA; chunk * nbin <= kRoiAlignStage, the backward's staged gout
+  const int per_cta = 2048 / nbin > 1 ? 2048 / nbin : 1;
+  p.chunk = C < per_cta ? C : per_cta;
+  BAGS_REQUIRE((C + p.chunk - 1) / p.chunk <= 65535, "%s: C = %d: too many channels for out size %d x %d", who, C,
+               out_h, out_w);
+  p.n_levels = n_levels;
+  p.B = B;
+  p.C = C;
+  p.k = k;
+  p.out_h = out_h;
+  p.out_w = out_w;
+  p.sample_num = sample_num;
+  p.inv_finest = n_levels == 1 ? 0.f : 1.f / finest_scale;
+  p.rois_map = rois_map;
+  p.rois = rois;
+  return BAGS_OK;
+}
+
+extern "C" int bags_roi_align_fwd(const float* const* feats_host, const int32_t* sizes_host, const float* scales_host,
+                                  int n_levels, int B, int C, const float* rois_map, const float* rois, int k, int out_h,
+                                  int out_w, int sample_num, float finest_scale, float* out, int32_t* levels,
+                                  void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  RoiAlignParams p;
+  if (int rc = roi_align_params("bags_roi_align_fwd", p, reinterpret_cast<const void* const*>(feats_host), false,
+                                sizes_host, scales_host, n_levels, B, C, rois_map, rois, k, out_h, out_w, sample_num,
+                                finest_scale))
+    return rc;
+  BAGS_REQUIRE(k == 0 || out, "bags_roi_align_fwd: NULL out");
+  BAGS_REQUIRE(aligned(out, 4) && aligned(levels, 4), "bags_roi_align_fwd: out / levels not 4-byte aligned");
+  if (k == 0) return BAGS_OK;
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  p.out = out;
+  p.levels = levels;
+  BAGS_CUDA(launch_roi_align_fwd(p, stream));
+  return BAGS_OK;
+}
+
+extern "C" int bags_roi_align_bwd(const float* gout, float* const* grads_host, const int32_t* sizes_host,
+                                  const float* scales_host, int n_levels, int B, int C, const float* rois_map,
+                                  const float* rois, int k, int out_h, int out_w, int sample_num, float finest_scale,
+                                  void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  RoiAlignParams p;
+  if (int rc = roi_align_params("bags_roi_align_bwd", p, reinterpret_cast<const void* const*>(grads_host), true,
+                                sizes_host, scales_host, n_levels, B, C, rois_map, rois, k, out_h, out_w, sample_num,
+                                finest_scale))
+    return rc;
+  BAGS_REQUIRE(k == 0 || gout, "bags_roi_align_bwd: NULL gout");
+  BAGS_REQUIRE(aligned(gout, 4), "bags_roi_align_bwd: gout not 4-byte aligned");
+  bool any = false;
+  for (int l = 0; l < n_levels; ++l) any = any || grads_host[l] != nullptr;
+  if (k == 0 || !any) return BAGS_OK;
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  p.gout = gout;
+  BAGS_CUDA(launch_roi_align_bwd(p, stream));
   return BAGS_OK;
 }
 

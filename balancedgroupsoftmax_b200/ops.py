@@ -697,6 +697,115 @@ def mask_targets(pos_proposals_list, pos_assigned_gt_inds_list, gt_masks_list, m
     return out
 
 
+# --------------------------------------------------------------------------- FPN RoI feature extractor
+@dataclass(frozen=True)
+class RoIAlignSpec:
+    """What bags_roi_align_fwd / _bwd take besides the tensors: the output size, each level's spatial_scale (as the
+    reference's op receives it, a C++ float), the samples per bin (<= 0: adaptive) and map_roi_levels' finest_scale
+    (unused with one level)."""
+    out_size: Tuple[int, int]
+    scales: Tuple[float, ...]
+    sample_num: int = 0
+    finest_scale: float = 56.0
+
+
+def _roi_align_args(spec: RoIAlignSpec, shapes, rois: torch.Tensor, rois_map: torch.Tensor):
+    L = len(shapes)
+    if L != len(spec.scales) or not 1 <= L <= 8:
+        raise nat.BagsNativeError('roi_align: %d feature levels and %d scales (1 to 8 levels)' % (L, len(spec.scales)))
+    B, Cc = shapes[0][0], shapes[0][1]
+    if any(len(s) != 4 or s[0] != B or s[1] != Cc for s in shapes):
+        raise nat.BagsNativeError('roi_align: every level must be [B, C, H, W] with the same B and C (got %s)'
+                                  % [tuple(s) for s in shapes])
+    for r in (rois, rois_map):
+        if r.dtype != torch.float32 or r.dim() != 2 or r.shape[1] != 5 or not r.is_contiguous():
+            raise nat.BagsNativeError('roi_align: rois must be contiguous fp32 [k, 5] (got %s %s)'
+                                      % (r.dtype, tuple(r.shape)))
+    if rois_map.shape[0] != rois.shape[0]:
+        raise nat.BagsNativeError('roi_align: %d RoIs to map, %d to pool' % (rois_map.shape[0], rois.shape[0]))
+    sizes = np.array([(s[2], s[3]) for s in shapes], dtype=np.int32)
+    scales = np.array(spec.scales, dtype=np.float32)
+    oh, ow = spec.out_size
+    return (sizes, scales, L, B, Cc, rois_map.data_ptr(), rois.data_ptr(), rois.shape[0], oh, ow, spec.sample_num,
+            float(spec.finest_scale))
+
+
+def roi_align_fwd(feats, rois: torch.Tensor, spec: RoIAlignSpec, rois_map: Optional[torch.Tensor] = None,
+                  want_levels: bool = False):
+    """bags_roi_align_fwd: every RoI pooled from its level in one launch, bitwise the reference's op; fp32
+    [k, C, out_h, out_w].  ``feats``: contiguous fp32 [B, C, H_l, W_l] per level; ``rois`` (and ``rois_map``, the RoIs
+    the levels are mapped from, ``rois`` when None): contiguous fp32 [k, 5].  With ``want_levels`` also returns the
+    int32 [k] level of each RoI (-1: a NaN scale, which gives a zero row, as a batch index outside [0, B) does)."""
+    feats = list(feats)
+    _require_cuda(rois, rois_map, *feats)
+    rois_map = rois if rois_map is None else rois_map
+    for f in feats:
+        if f.dtype != torch.float32 or not f.is_contiguous():
+            raise nat.BagsNativeError('roi_align: features must be contiguous fp32 (got %s)' % f.dtype)
+    args = _roi_align_args(spec, [f.shape for f in feats], rois, rois_map)
+    sizes, scales, L, B, Cc, pm, pr, k, oh, ow = args[:10]
+    dev = rois.device
+    out = torch.empty((k, Cc, oh, ow), dtype=torch.float32, device=dev)
+    levels = torch.empty((k,), dtype=torch.int32, device=dev) if want_levels else None
+    ptrs = (C.c_void_p * L)(*[f.data_ptr() for f in feats])
+    nat.check(nat.lib().bags_roi_align_fwd(ptrs, sizes.ctypes.data, scales.ctypes.data, *args[2:], nat.ptr(out),
+                                           nat.ptr(levels), _stream_ptr(dev)), 'bags_roi_align_fwd')
+    return (out, levels) if want_levels else out
+
+
+def roi_align_bwd(gout: torch.Tensor, shapes, rois: torch.Tensor, spec: RoIAlignSpec,
+                  rois_map: Optional[torch.Tensor] = None, needs=None):
+    """bags_roi_align_bwd: the gradient of roi_align_fwd for every level in one launch, into fp32 gradients zeroed on
+    the stream.  ``shapes``: each level's [B, C, H, W]; ``needs``: which levels want a gradient (all when None).
+    Returns one fp32 gradient per level, None where it is not wanted; nothing is launched when none is."""
+    _require_cuda(gout, rois, rois_map)
+    rois_map = rois if rois_map is None else rois_map
+    needs = [True] * len(shapes) if needs is None else list(needs)
+    args = _roi_align_args(spec, shapes, rois, rois_map)
+    sizes, scales, L = args[:3]
+    dev = gout.device
+    gout = gout.float().contiguous()
+    if tuple(gout.shape) != (args[7], args[4]) + tuple(spec.out_size):
+        raise nat.BagsNativeError('roi_align: gout must be [k, C, out_h, out_w] (got %s)' % (tuple(gout.shape),))
+    grads = [torch.zeros(tuple(s), dtype=torch.float32, device=dev) if n else None for s, n in zip(shapes, needs)]
+    if any(needs):
+        ptrs = (C.c_void_p * L)(*[nat.ptr(g) for g in grads])
+        nat.check(nat.lib().bags_roi_align_bwd(gout.data_ptr(), ptrs, sizes.ctypes.data, scales.ctypes.data, *args[2:],
+                                               _stream_ptr(dev)), 'bags_roi_align_bwd')
+    return grads
+
+
+class RoIAlignFunction(torch.autograd.Function):
+    """out = roi_align_fwd(feats, rois, spec, rois_map) as an autograd Function over ``(rois, *feats)``; fp32
+    contiguous features (the callers cast).  Its backward is one bags_roi_align_bwd launch for the levels that need a
+    gradient, none when no level does; the RoIs get no gradient, as in the reference."""
+
+    @staticmethod
+    def forward(ctx, spec: RoIAlignSpec, rois_map, rois, *feats):
+        ctx.spec = spec
+        ctx.shapes = [tuple(f.shape) for f in feats]
+        ctx.save_for_backward(rois, rois_map)
+        return roi_align_fwd(feats, rois, spec, rois_map)
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gout):
+        rois, rois_map = ctx.saved_tensors
+        needs = ctx.needs_input_grad[3:]
+        grads = roi_align_bwd(gout, ctx.shapes, rois, ctx.spec, rois_map, needs) if any(needs) else [None] * len(needs)
+        return (None, None, None) + tuple(grads)
+
+
+def roi_align_apply(feats, rois: torch.Tensor, spec: RoIAlignSpec, rois_map: Optional[torch.Tensor] = None):
+    """RoIAlignFunction on any floating features: non-fp32 ones are cast to fp32 first (force_fp32) and take their
+    gradient back through the cast; features and RoIs are made contiguous."""
+    _require_cuda(rois, rois_map, *feats)
+    rois = rois.float().contiguous()
+    rois_map = rois if rois_map is None else rois_map.float().contiguous()
+    feats = [f.float().contiguous() for f in feats]
+    return RoIAlignFunction.apply(spec, rois_map, rois, *feats)
+
+
 def gemm_probe(a, a_mn: bool, b, b_mn: bool, M: int, N: int, K: int, block_n: int = 256, splits: int = 1,
                epi: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Test hook for one wgmma GEMM (see bags_gemm_probe)."""

@@ -1,4 +1,4 @@
-"""HEADS / LOSSES registries and build_from_cfg.
+"""HEADS / LOSSES / ROI_EXTRACTORS registries and build_from_cfg.
 
 Mirrors mmdet/utils/registry.py:6-76, mmdet/models/registry.py:7-8 and
 mmdet/models/builder.py:34-35 so that ``bbox_head=dict(type='GSBBoxHeadWith0', ...)``
@@ -85,12 +85,29 @@ else:
     USING_MMDET_REGISTRY = False
 
 
+def _mmdet_roi_extractors():
+    try:  # pragma: no cover - mmdet is not installable in the build image
+        from mmdet.models.registry import ROI_EXTRACTORS as _R
+        return _R
+    except Exception:
+        return None
+
+
+ROI_EXTRACTORS = _mmdet_roi_extractors()
+if ROI_EXTRACTORS is None:
+    ROI_EXTRACTORS = Registry('roi_extractor')
+
+
 def build_head(cfg):
     return build_from_cfg(cfg, HEADS)
 
 
 def build_loss(cfg):
     return build_from_cfg(cfg, LOSSES)
+
+
+def build_roi_extractor(cfg):
+    return build_from_cfg(cfg, ROI_EXTRACTORS)
 
 
 def register(registry, cls):

@@ -36,6 +36,8 @@
  *     fcn_mask_head.py:125-239
  *   FCNMaskHead.get_target: crop + resize gt masks    bags_mask_target
  *     mmdet/core/mask/mask_target.py
+ *   SingleRoIExtractor.forward + RoIAlign                 bags_roi_align_fwd / bags_roi_align_bwd
+ *     single_level.py, roi_align_kernel.cu
  *   allreduce_grads / _allreduce_coalesced                bags_grad_allreduce
  *     mmdet/core/utils/dist_utils.py:9-41
  *
@@ -367,6 +369,39 @@ int bags_segm_rle(const float* probs, int n, int mask_h, int mask_w, const int32
  * 64 images, no host sync, nothing read on the host from the device: capturable in a CUDA graph. */
 int bags_mask_target(const float* const* boxes_host, const int64_t* const* gt_inds_host, const uint8_t* const* masks_host,
                      const int32_t* sizes_host, int n_images, int mask_h, int mask_w, float* out, void* stream);
+
+/* FPN RoI feature extractor -- replaces SingleRoIExtractor.forward (mmdet/models/roi_extractors/single_level.py:
+ * map_roi_levels :56-75, the per-level loop :93-108 with its host syncs on inds.any(), rois[inds] and
+ * roi_feats[inds] = ...; the len(feats) == 1 path :94-95) and the RoIAlign op it calls per level
+ * (mmdet/ops/roi_align/src/roi_align_kernel.cu: ROIAlignForward :61-119 with bilinear_interpolate :16-59).
+ * Every RoI of every image in one launch:
+ *   level  = clamp(floor(log2f(sqrt((x2 - x1 + 1) (y2 - y1 + 1)) * fp32(1 / finest_scale) + fp32(1e-6))), 0, L - 1),
+ *            each step rounded to fp32 as torch evaluates the reference's expression on CUDA; 0 when L == 1
+ *   out[r] = ROIAlignForward<float> of rois[r] on level `level`, bitwise (its -O2 sm_90a rounding sequence)
+ * A RoI whose level is NaN, or whose batch index (int)rois[r][0] lies outside [0, B), gives a zero row.
+ *   feats_host   HOST array [L] of device fp32 [B, C, H_l, W_l], contiguous, 4-byte aligned; L <= 8
+ *   sizes_host   int32 [L, 2]: (H_l, W_l), each >= 1;  scales_host fp32 [L]: spatial_scale of each level
+ *   rois_map     device fp32 [k, 5] (batch, x1, y1, x2, y2) the levels are mapped from
+ *   rois         device fp32 [k, 5] the RoIs pooled (== rois_map unless roi_scale_factor rescales them)
+ *   out_h, out_w 1 to 64;  sample_num <= 0: ceil(bin size) samples per bin, as the reference
+ *   finest_scale > 0 (unused with one level)
+ *   out          device fp32 [k, C, out_h, out_w];  levels (optional, NULL to skip): int32 [k], -1 for a NaN level
+ * k == 0: nothing is launched.  No host sync: capturable in a CUDA graph. */
+int bags_roi_align_fwd(const float* const* feats_host, const int32_t* sizes_host, const float* scales_host, int n_levels,
+                       int B, int C, const float* rois_map, const float* rois, int k, int out_h, int out_w,
+                       int sample_num, float finest_scale, float* out, int32_t* levels, void* stream);
+
+/* Backward of bags_roi_align_fwd -- replaces ROIAlignBackward (roi_align_kernel.cu:164-282) launched once per level
+ * and the scatter of roi_feats[inds] = ...: the terms gout w_i / count of each sample's four corners, for every RoI
+ * and level in one launch, ADDED to grads_host[level] (the caller zeroes them on the stream).  A CTA sums each pixel
+ * its RoI touches in registers, in a fixed order, and adds it with one reduction; the order across RoIs is open, so
+ * the result is not bitwise reproducible.  grads_host: HOST array [L] of device fp32 [B, C, H_l, W_l] (contiguous,
+ * 4-byte aligned), or NULL for a level that takes no gradient; gout: device fp32 [k, C, out_h, out_w].  Other
+ * arguments as bags_roi_align_fwd.  Zero rows of the forward take no gradient.  k == 0, or every level NULL: nothing
+ * is launched. */
+int bags_roi_align_bwd(const float* gout, float* const* grads_host, const int32_t* sizes_host, const float* scales_host,
+                       int n_levels, int B, int C, const float* rois_map, const float* rois, int k, int out_h,
+                       int out_w, int sample_num, float finest_scale, void* stream);
 
 /* test hook: launch `blocks` x `threads` threads that wait `micros` microseconds and exit */
 int bags_debug_spin(int blocks, int threads, int micros, void* stream);

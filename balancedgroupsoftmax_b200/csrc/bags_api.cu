@@ -24,6 +24,7 @@
 #include "bags_segm.cuh"
 #include "bags_mask_target.cuh"
 #include "bags_roi_align.cuh"
+#include "bags_rpn.cuh"
 
 using namespace bags;
 
@@ -1416,6 +1417,104 @@ extern "C" int bags_roi_align_bwd(const float* gout, float* const* grads_host, c
   if (int rc = device_info(di)) return rc;
   p.gout = gout;
   BAGS_CUDA(launch_roi_align_bwd(p, stream));
+  return BAGS_OK;
+}
+
+// ----------------------------------------------------------------------------
+// RPN proposals (see bags_rpn.cuh; the kernels are in bags_rpn.cu)
+// ----------------------------------------------------------------------------
+// the level shapes and limits shared by bags_rpn_proposals and bags_rpn_scratch_bytes; fills p's levels (but their
+// pointers and base anchors) and lays the scratch out
+static int rpn_params(const char* who, RpnParams& p, const int32_t* levels_host, int n_levels, int B, int nms_pre,
+                      int nms_post, size_t& bytes) {
+  BAGS_REQUIRE(levels_host, "%s: NULL levels", who);
+  BAGS_REQUIRE(n_levels >= 1 && n_levels <= kRpnMaxLevels, "%s: %d levels: 1 to %d", who, n_levels, kRpnMaxLevels);
+  BAGS_REQUIRE(B >= 1 && B <= kRpnMaxImages, "%s: B = %d images: 1 to %d", who, B, kRpnMaxImages);
+  BAGS_REQUIRE(nms_post >= 1, "%s: nms_post = %d must be at least 1", who, nms_post);
+  p = RpnParams{};
+  p.n_levels = n_levels;
+  p.B = B;
+  p.nms_post = nms_post;
+  for (int l = 0; l < n_levels; ++l) {
+    const int H = levels_host[4 * l], W = levels_host[4 * l + 1], A = levels_host[4 * l + 2];
+    const int stride = levels_host[4 * l + 3];
+    BAGS_REQUIRE(A >= 1 && A <= kRpnMaxAnchors, "%s: level %d has %d anchors per location: 1 to %d", who, l, A,
+                 kRpnMaxAnchors);
+    BAGS_REQUIRE(H >= 0 && W >= 0 && stride >= 1, "%s: level %d: H %d, W %d, stride %d", who, l, H, W, stride);
+    const long long n = static_cast<long long>(H) * W * A;
+    BAGS_REQUIRE(n <= 0x7fffffffLL && static_cast<long long>(stride) * (H > W ? H : W) <= (1LL << 24),
+                 "%s: level %d is too large (%d x %d x %d, stride %d)", who, l, H, W, A, stride);
+    RpnLevel& L = p.lvl[l];
+    L.H = H;
+    L.W = W;
+    L.A = A;
+    L.stride = stride;
+    L.n = static_cast<int>(n);
+    L.select = nms_pre > 0 && n > nms_pre;
+    L.K = L.select ? nms_pre : L.n;
+    BAGS_REQUIRE(L.K <= kRpnMaxCand, "%s: level %d has %d candidates (nms_pre %d, %lld anchors): at most %d", who, l,
+                 L.K, nms_pre, n, kRpnMaxCand);
+  }
+  bytes = rpn_layout(p, nullptr);
+  return BAGS_OK;
+}
+
+extern "C" int bags_rpn_scratch_bytes(const int32_t* levels_host, int n_levels, int B, int nms_pre, int nms_post,
+                                      size_t* bytes) {
+  BAGS_REQUIRE(bytes, "bags_rpn_scratch_bytes: NULL bytes");
+  RpnParams p;
+  size_t need = 0;
+  if (int rc = rpn_params("bags_rpn_scratch_bytes", p, levels_host, n_levels, B, nms_pre, nms_post, need)) return rc;
+  *bytes = need;
+  return BAGS_OK;
+}
+
+extern "C" int bags_rpn_proposals(const float* const* logits_host, const float* const* deltas_host,
+                                  const int32_t* levels_host, const float* base_host, int n_levels, int B,
+                                  const int32_t* img_shapes_host, int nms_pre, int nms_post, int max_num,
+                                  float nms_thr, float min_bbox_size, const float* means_host, const float* stds_host,
+                                  void* scratch, size_t scratch_bytes, float* out, int32_t* counts, void* stream_) {
+  const char* who = "bags_rpn_proposals";
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  RpnParams p;
+  size_t need = 0;
+  if (int rc = rpn_params(who, p, levels_host, n_levels, B, nms_pre, nms_post, need)) return rc;
+  BAGS_REQUIRE(max_num >= 1, "%s: max_num = %d must be at least 1", who, max_num);
+  BAGS_REQUIRE(logits_host && deltas_host && base_host && img_shapes_host && means_host && stds_host,
+               "%s: NULL host table", who);
+  BAGS_REQUIRE(scratch && out && counts, "%s: NULL scratch, out or counts", who);
+  BAGS_REQUIRE(aligned(scratch, 256) && aligned(out, 4) && aligned(counts, 4),
+               "%s: scratch must be 256-byte aligned, out and counts 4-byte aligned", who);
+  BAGS_REQUIRE(scratch_bytes >= need, "%s: scratch of %zu bytes, %zu needed", who, scratch_bytes, need);
+  const float* base = base_host;
+  for (int l = 0; l < n_levels; ++l) {
+    RpnLevel& L = p.lvl[l];
+    BAGS_REQUIRE(L.n == 0 || (logits_host[l] && deltas_host[l]), "%s: level %d: NULL logits or deltas", who, l);
+    BAGS_REQUIRE(aligned(logits_host[l], 4) && aligned(deltas_host[l], 4), "%s: level %d: not 4-byte aligned", who, l);
+    L.logits = logits_host[l];
+    L.deltas = deltas_host[l];
+    for (int a = 0; a < L.A; ++a, base += 4) L.base[a] = make_float4(base[0], base[1], base[2], base[3]);
+  }
+  for (int b = 0; b < B; ++b) {
+    p.img_h[b] = img_shapes_host[2 * b];
+    p.img_w[b] = img_shapes_host[2 * b + 1];
+    BAGS_REQUIRE(p.img_h[b] >= 1 && p.img_w[b] >= 1, "%s: image %d: img_shape %d x %d", who, b, p.img_h[b],
+                 p.img_w[b]);
+  }
+  p.max_num = max_num;
+  p.nms_thr = nms_thr;
+  p.min_bbox_size = min_bbox_size;
+  p.max_ratio = static_cast<float>(std::fabs(std::log(16.0 / 1000.0)));   // delta2bbox's wh_ratio_clip, as fp32
+  for (int c = 0; c < 4; ++c) {
+    p.means[c] = means_host[c];
+    p.stds[c] = stds_host[c];
+  }
+  rpn_layout(p, scratch);
+  p.out = out;
+  p.counts = counts;
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  BAGS_CUDA(launch_rpn_proposals(p, stream));
   return BAGS_OK;
 }
 

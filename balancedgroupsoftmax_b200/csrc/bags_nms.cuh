@@ -10,20 +10,12 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "bags_iou.cuh"
+
 namespace bags {
 
 constexpr int kNmsMaxSeg = 1024;
 constexpr int kNmsThreads = 1024;   // 32 warps: the mask rows are dealt to the warps; with 8 the loop was issue-latency bound
-
-__device__ __forceinline__ float iou_plus1(const float4 a, const float4 b) {
-  const float left = fmaxf(a.x, b.x), right = fminf(a.z, b.z);
-  const float top = fmaxf(a.y, b.y), bottom = fminf(a.w, b.w);
-  const float width = fmaxf(right - left + 1.f, 0.f), height = fmaxf(bottom - top + 1.f, 0.f);
-  const float inter = width * height;
-  const float sa = (a.z - a.x + 1.f) * (a.w - a.y + 1.f);
-  const float sb = (b.z - b.x + 1.f) * (b.w - b.y + 1.f);
-  return inter / (sa + sb - inter);
-}
 
 // No candidate list is compacted on the host.  The caller sorts every class's scores once (one batched
 // device sort: order[s][i] = RoI index of the i-th best score of class s+1) and counts the scores above the threshold

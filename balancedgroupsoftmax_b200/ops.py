@@ -697,6 +697,79 @@ def mask_targets(pos_proposals_list, pos_assigned_gt_inds_list, gt_masks_list, m
     return out
 
 
+# --------------------------------------------------------------------------- RPN proposals
+def _rpn_levels(cls_scores, bbox_preds, base_anchors, strides):
+    L = len(cls_scores)
+    if not (L == len(bbox_preds) == len(base_anchors) == len(strides)) or not 1 <= L <= 8:
+        raise nat.BagsNativeError('rpn_proposals: %d score levels, %d delta levels, %d base-anchor tables and %d '
+                                  'strides (1 to 8 levels, the same count of each)'
+                                  % (L, len(bbox_preds), len(base_anchors), len(strides)))
+    B = cls_scores[0].shape[0] if cls_scores[0].dim() == 4 else -1
+    levels = np.zeros((L, 4), dtype=np.int32)
+    for l, (s, d, base) in enumerate(zip(cls_scores, bbox_preds, base_anchors)):
+        A = s.shape[1] if s.dim() == 4 else -1
+        if s.dim() != 4 or d.dim() != 4 or s.shape[0] != B or tuple(d.shape) != (B, 4 * A) + tuple(s.shape[2:]):
+            raise nat.BagsNativeError('rpn_proposals: level %d: scores must be [B, A, H, W] and deltas [B, 4A, H, W] '
+                                      'with one B (got %s and %s)' % (l, tuple(s.shape), tuple(d.shape)))
+        if tuple(np.shape(base)) != (A, 4):
+            raise nat.BagsNativeError('rpn_proposals: level %d: %d anchors per location but base anchors of shape %s'
+                                      % (l, A, tuple(np.shape(base))))
+        levels[l] = (s.shape[2], s.shape[3], A, int(strides[l]))
+    return B, levels
+
+
+def rpn_scratch_bytes(levels: np.ndarray, B: int, nms_pre: int, nms_post: int) -> int:
+    """bags_rpn_scratch_bytes: device scratch bags_rpn_proposals needs; ``levels`` int32 [L, 4] (H, W, A, stride)."""
+    levels = np.ascontiguousarray(levels, dtype=np.int32)
+    out = C.c_size_t(0)
+    nat.check(nat.lib().bags_rpn_scratch_bytes(levels.ctypes.data, levels.shape[0], int(B), int(nms_pre),
+                                               int(nms_post), C.byref(out)), 'bags_rpn_scratch_bytes')
+    return out.value
+
+
+def rpn_proposals(cls_scores, bbox_preds, base_anchors, strides, img_shapes, nms_pre: int, nms_post: int,
+                  max_num: int, nms_thr: float, min_bbox_size: float = 0.0, means=(0., 0., 0., 0.),
+                  stds=(1., 1., 1., 1.)):
+    """bags_rpn_proposals: the proposals of a sigmoid RPN for every image and level in one call (four launches), with
+    no host sync -- capturable in a CUDA graph.
+
+    ``cls_scores`` / ``bbox_preds``: per level, CUDA fp32 [B, A, H, W] logits and [B, 4A, H, W] deltas (made
+    contiguous); ``base_anchors``: per level [A, 4] (AnchorGenerator.base_anchors); ``strides``: per level;
+    ``img_shapes``: per image (h, w, ...).  Returns ``(proposals, counts)``: fp32 [B, max_num, 5] rows (x1, y1, x2, y2,
+    score), the first counts[b] of image b valid and the rest zero, and int32 [B] counts.  Equal to RPNHead.get_bboxes
+    (nms_across_levels=False) per image where no tie decides the result; ties are broken by (score desc, flat index
+    asc) within a level and (score desc, level asc, position asc) across levels."""
+    cls_scores, bbox_preds = list(cls_scores), list(bbox_preds)
+    for t in cls_scores + bbox_preds:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype != torch.float32:
+            raise nat.BagsNativeError('rpn_proposals: scores and deltas must be CUDA fp32 tensors (got %s)'
+                                      % (t.dtype if isinstance(t, torch.Tensor) else type(t).__name__,))
+    B, levels = _rpn_levels(cls_scores, bbox_preds, base_anchors, strides)
+    if len(img_shapes) != B:
+        raise nat.BagsNativeError('rpn_proposals: %d img_shapes for %d images' % (len(img_shapes), B))
+    dev = cls_scores[0].device
+    cls_scores = [t.detach().contiguous() for t in cls_scores]
+    bbox_preds = [t.detach().contiguous() for t in bbox_preds]
+    base = np.ascontiguousarray(np.concatenate([np.asarray(torch.as_tensor(b, dtype=torch.float32).cpu(),
+                                                           dtype=np.float32).reshape(-1, 4) for b in base_anchors]))
+    shapes = np.array([(int(s[0]), int(s[1])) for s in img_shapes], dtype=np.int32).reshape(B, 2)
+    mean = np.asarray(means, dtype=np.float32).reshape(4)
+    std = np.asarray(stds, dtype=np.float32).reshape(4)
+    nbytes = rpn_scratch_bytes(levels, B, nms_pre, nms_post)
+    scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    max_num = int(max_num)
+    out = torch.empty((B, max(max_num, 0), 5), dtype=torch.float32, device=dev)
+    counts = torch.empty((B,), dtype=torch.int32, device=dev)
+    L = len(cls_scores)
+    lp = (C.c_void_p * L)(*[t.data_ptr() for t in cls_scores])
+    dp = (C.c_void_p * L)(*[t.data_ptr() for t in bbox_preds])
+    nat.check(nat.lib().bags_rpn_proposals(lp, dp, levels.ctypes.data, base.ctypes.data, L, B, shapes.ctypes.data,
+                                           int(nms_pre), int(nms_post), max_num, float(nms_thr), float(min_bbox_size),
+                                           mean.ctypes.data, std.ctypes.data, scratch.data_ptr(), nbytes,
+                                           out.data_ptr(), counts.data_ptr(), _stream_ptr(dev)), 'bags_rpn_proposals')
+    return out, counts
+
+
 # --------------------------------------------------------------------------- FPN RoI feature extractor
 @dataclass(frozen=True)
 class RoIAlignSpec:

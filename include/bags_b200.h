@@ -38,6 +38,8 @@
  *     mmdet/core/mask/mask_target.py
  *   SingleRoIExtractor.forward + RoIAlign                 bags_roi_align_fwd / bags_roi_align_bwd
  *     single_level.py, roi_align_kernel.cu
+ *   RPNHead.get_bboxes: RPN proposals                     bags_rpn_proposals (+ bags_rpn_scratch_bytes)
+ *     rpn_head.py:55-104, anchor_head.py:250-276, nms_kernel.cu
  *   allreduce_grads / _allreduce_coalesced                bags_grad_allreduce
  *     mmdet/core/utils/dist_utils.py:9-41
  *
@@ -402,6 +404,39 @@ int bags_roi_align_fwd(const float* const* feats_host, const int32_t* sizes_host
 int bags_roi_align_bwd(const float* gout, float* const* grads_host, const int32_t* sizes_host, const float* scales_host,
                        int n_levels, int B, int C, const float* rois_map, const float* rois, int k, int out_h,
                        int out_w, int sample_num, float finest_scale, void* stream);
+
+/* RPN proposals -- replaces RPNHead.get_bboxes (mmdet/models/anchor_heads/anchor_head.py:250-276: grid_anchors per
+ * level, then the per-image loop) and RPNHead.get_bboxes_single (rpn_head.py:55-104: per level sigmoid, topk(nms_pre),
+ * delta2bbox, min_bbox_size, the NMS op of mmdet/ops/nms/src/nms_kernel.cu:69-130 with its device-to-host copy of the
+ * suppression matrix and CPU scan, [:nms_post]; then topk(min(max_num, total)) over the levels), for a sigmoid RPN
+ * with nms_across_levels=False.  Every image and level in four launches, no host read, no allocation:
+ *   scores   sigmoid(logit) as torch.sigmoid (1 / (1 + expf(-x)) in fp32), flat index (h W + w) A + a;
+ *   select   the top nms_pre by (score desc, flat asc) when the level has more than nms_pre > 0 anchors, else all;
+ *   anchors  base[a] + (w stride, h stride) in fp32;  boxes: delta2bbox with one fp32 rounding per torch op, clamped
+ *            to [0, img_w - 1] x [0, img_h - 1] of the image (NaN kept); boxes with x2 - x1 + 1 or y2 - y1 + 1 below
+ *            min_bbox_size > 0 are dropped;
+ *   suppress greedy in (score desc, flat asc) order, IoU with "+1" widths, suppressed when IoU > nms_thr; the first
+ *            nms_post survivors in the level's input order (score order when selected, anchor order when not);
+ *   merge    the first min(max_num, total) survivors of the image by (score desc, level asc, position asc).
+ *   logits_host  HOST array [L] of device fp32 [B, A_l, H_l, W_l], contiguous, 4-byte aligned; L in [1, 8]
+ *   deltas_host  HOST array [L] of device fp32 [B, 4 A_l, H_l, W_l]
+ *   levels_host  int32 [L, 4]: H_l, W_l (>= 0), A_l (1 to 16), stride_l (>= 1); a level may hold 0 anchors
+ *   base_host    fp32 [sum A_l, 4]: each level's base anchors (x1, y1, x2, y2), level after level
+ *   img_shapes_host int32 [B, 2]: (h, w) of img_shape per image, each >= 1;  B in [1, 32]
+ *   nms_pre (<= 0: no selection), nms_post >= 1, max_num >= 1; each level's candidate count (nms_pre when selected,
+ *            else its anchor count) at most 4096
+ *   means_host, stds_host fp32 [4];  scratch: device, bags_rpn_scratch_bytes() bytes, 256-byte aligned
+ *   out      device fp32 [B, max_num, 5] (x1, y1, x2, y2, score), zero rows after counts[b]; counts: device int32 [B]
+ * No host sync: capturable in a CUDA graph. */
+int bags_rpn_proposals(const float* const* logits_host, const float* const* deltas_host, const int32_t* levels_host,
+                       const float* base_host, int n_levels, int B, const int32_t* img_shapes_host, int nms_pre,
+                       int nms_post, int max_num, float nms_thr, float min_bbox_size, const float* means_host,
+                       const float* stds_host, void* scratch, size_t scratch_bytes, float* out, int32_t* counts,
+                       void* stream);
+
+/* Scratch bytes bags_rpn_proposals needs for these level shapes (levels_host as there), B, nms_pre and nms_post; the
+ * same argument checks.  Writes *bytes. */
+int bags_rpn_scratch_bytes(const int32_t* levels_host, int n_levels, int B, int nms_pre, int nms_post, size_t* bytes);
 
 /* test hook: launch `blocks` x `threads` threads that wait `micros` microseconds and exit */
 int bags_debug_spin(int blocks, int threads, int micros, void* stream);

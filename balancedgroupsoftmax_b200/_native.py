@@ -67,6 +67,10 @@ SIGNATURES = {
     'bags_rpn_proposals': (_i, [_vp, _vp, _vp, _vp, _i, _i, _vp, _i, _i, _i, C.c_float, C.c_float, _vp, _vp, _vp, _sz,
                                 _vp, _vp, _vp]),
     'bags_rpn_scratch_bytes': (_i, [_vp, _i, _i, _i, _i, _vp]),
+    'bags_anchor_target': (_i, [_vp, _vp, _i, _i, _vp, _vp, _i, C.c_float, _i, C.c_float, C.c_float, C.c_float, _i,
+                                C.c_double, _i, C.c_double, C.c_double, C.c_float, _vp, _vp, C.c_uint64, _vp, _vp,
+                                _sz, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'bags_anchor_target_scratch_bytes': (_i, [_vp, _i, _i, _i, _vp]),
     'bags_debug_spin': (_i, [_i, _i, _i, _vp]),
     'bags_cast_bf16': (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp]),
     'bags_linear_act_fwd': (_i, [_vp, _ll, _vp, _ll, _vp, _vp, _ll, _i, _i, _i, _i, _i, _i, _vp]),

@@ -15,8 +15,9 @@ OUT = os.path.join(_HERE, 'libbags_b200.so')
 SOURCES = [os.path.join(CSRC, 'bags_api.cu')]
 # kernels compiled as translation units of their own and linked into the same library; bags_api.cu launches them
 # through the host launchers their headers declare
-UNITS = [os.path.join(CSRC, 'bags_roi_align.cu'), os.path.join(CSRC, 'bags_rpn.cu')]
-HEADERS = [os.path.join(CSRC, f) for f in ('bags_ptx.cuh', 'bags_wgmma.cuh', 'bags_gemm.cuh', 'bags_kernels.cuh', 'bags_fused_fwd.cuh', 'bags_allreduce.cuh', 'bags_iou.cuh', 'bags_nms.cuh', 'bags_box.cuh', 'bags_mask.cuh', 'bags_segm.cuh', 'bags_mask_target.cuh', 'bags_roi_align.cuh', 'bags_rpn.cuh')] + [
+UNITS = [os.path.join(CSRC, 'bags_roi_align.cu'), os.path.join(CSRC, 'bags_rpn.cu'),
+         os.path.join(CSRC, 'bags_anchor_target.cu')]
+HEADERS = [os.path.join(CSRC, f) for f in ('bags_ptx.cuh', 'bags_wgmma.cuh', 'bags_gemm.cuh', 'bags_kernels.cuh', 'bags_fused_fwd.cuh', 'bags_allreduce.cuh', 'bags_iou.cuh', 'bags_nms.cuh', 'bags_box.cuh', 'bags_mask.cuh', 'bags_segm.cuh', 'bags_mask_target.cuh', 'bags_roi_align.cuh', 'bags_rpn.cuh', 'bags_hash.cuh', 'bags_anchor.cuh', 'bags_anchor_target.cuh')] + [
     os.path.join(os.path.dirname(_HERE), 'include', 'bags_b200.h')]
 
 NVCC_FLAGS = [

@@ -25,6 +25,7 @@
 #include "bags_mask_target.cuh"
 #include "bags_roi_align.cuh"
 #include "bags_rpn.cuh"
+#include "bags_anchor_target.cuh"
 
 using namespace bags;
 
@@ -1515,6 +1516,142 @@ extern "C" int bags_rpn_proposals(const float* const* logits_host, const float* 
   DeviceInfo di;
   if (int rc = device_info(di)) return rc;
   BAGS_CUDA(launch_rpn_proposals(p, stream));
+  return BAGS_OK;
+}
+
+// ----------------------------------------------------------------------------
+// RPN training targets (see bags_anchor_target.cuh; the kernels are in bags_anchor_target.cu)
+// ----------------------------------------------------------------------------
+// the level shapes and limits shared by bags_anchor_target and bags_anchor_target_scratch_bytes; fills p's levels (but
+// their base anchors) and lays the scratch out
+static int anchor_target_params(const char* who, AtParams& p, const int32_t* levels_host, int n_levels, int B,
+                                int total_gts, size_t& bytes) {
+  BAGS_REQUIRE(levels_host, "%s: NULL levels", who);
+  BAGS_REQUIRE(n_levels >= 1 && n_levels <= kAtMaxLevels, "%s: %d levels: 1 to %d", who, n_levels, kAtMaxLevels);
+  BAGS_REQUIRE(B >= 1 && B <= kAtMaxImages, "%s: B = %d images: 1 to %d", who, B, kAtMaxImages);
+  BAGS_REQUIRE(total_gts >= B, "%s: %d gts for %d images: every image needs one", who, total_gts, B);
+  p = AtParams{};
+  p.n_levels = n_levels;
+  p.B = B;
+  long long N = 0;
+  for (int l = 0; l < n_levels; ++l) {
+    const int H = levels_host[4 * l], W = levels_host[4 * l + 1], A = levels_host[4 * l + 2];
+    const int stride = levels_host[4 * l + 3];
+    BAGS_REQUIRE(A >= 1 && A <= kAtMaxAnchors, "%s: level %d has %d anchors per location: 1 to %d", who, l, A,
+                 kAtMaxAnchors);
+    BAGS_REQUIRE(H >= 0 && W >= 0 && stride >= 1, "%s: level %d: H %d, W %d, stride %d", who, l, H, W, stride);
+    BAGS_REQUIRE(static_cast<long long>(stride) * (H > W ? H : W) <= (1LL << 24),
+                 "%s: level %d is too large (%d x %d, stride %d)", who, l, H, W, stride);
+    AtLevel& L = p.lvl[l];
+    L.H = H;
+    L.W = W;
+    L.A = A;
+    L.stride = stride;
+    L.n = H * W * A;
+    L.off = static_cast<int>(N);
+    N += static_cast<long long>(H) * W * A;
+    BAGS_REQUIRE(N <= 0x7fffffffLL, "%s: more than 2^31 - 1 anchors per image", who);
+  }
+  BAGS_REQUIRE(N >= 1, "%s: no anchor in any level", who);
+  p.N = static_cast<int>(N);
+  bytes = anchor_target_layout(p, total_gts, nullptr);
+  return BAGS_OK;
+}
+
+extern "C" int bags_anchor_target_scratch_bytes(const int32_t* levels_host, int n_levels, int B, int total_gts,
+                                                size_t* bytes) {
+  BAGS_REQUIRE(bytes, "bags_anchor_target_scratch_bytes: NULL bytes");
+  AtParams p;
+  size_t need = 0;
+  if (int rc = anchor_target_params("bags_anchor_target_scratch_bytes", p, levels_host, n_levels, B, total_gts, need))
+    return rc;
+  *bytes = need;
+  return BAGS_OK;
+}
+
+extern "C" int bags_anchor_target(const int32_t* levels_host, const float* base_host, int n_levels, int B,
+                                  const int32_t* images_host, const float* gts, int total_gts, float pos_iou_thr,
+                                  int neg_on, float neg_lo, float neg_hi, float min_pos_iou, int gt_max_assign_all,
+                                  double allowed_border, int num, double pos_fraction, double neg_pos_ub,
+                                  float pos_weight, const float* means_host, const float* stds_host, uint64_t seed,
+                                  const int64_t* seed_step, void* scratch, size_t scratch_bytes, int64_t* labels,
+                                  float* label_weights, float* bbox_targets, float* bbox_weights, int64_t* totals,
+                                  void* stream_) {
+  const char* who = "bags_anchor_target";
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  AtParams p;
+  size_t need = 0;
+  if (int rc = anchor_target_params(who, p, levels_host, n_levels, B, total_gts, need)) return rc;
+  BAGS_REQUIRE(base_host && images_host && means_host && stds_host, "%s: NULL host table", who);
+  BAGS_REQUIRE(gts && scratch && labels && label_weights && bbox_targets && bbox_weights && totals,
+               "%s: NULL gts, scratch or output", who);
+  BAGS_REQUIRE(aligned(gts, 16) && aligned(bbox_targets, 16) && aligned(bbox_weights, 16),
+               "%s: gts, bbox_targets and bbox_weights must be 16-byte aligned", who);
+  BAGS_REQUIRE(aligned(scratch, 256) && aligned(labels, 8) && aligned(totals, 8) && aligned(label_weights, 4) &&
+                   aligned(seed_step, 8),
+               "%s: scratch must be 256-byte aligned, labels, totals and seed_step 8-byte aligned", who);
+  BAGS_REQUIRE(scratch_bytes >= need, "%s: scratch of %zu bytes, %zu needed", who, scratch_bytes, need);
+  BAGS_REQUIRE(num >= 0 && pos_fraction >= 0.0 && pos_fraction <= 1.0,
+               "%s: num = %d must be >= 0 and pos_fraction = %g in [0, 1]", who, num, pos_fraction);
+  BAGS_REQUIRE(!std::isnan(allowed_border) && !std::isnan(neg_pos_ub), "%s: NaN allowed_border or neg_pos_ub", who);
+  const float* base = base_host;
+  for (int l = 0; l < n_levels; ++l)
+    for (int a = 0; a < p.lvl[l].A; ++a, base += 4) p.lvl[l].base[a] = make_float4(base[0], base[1], base[2], base[3]);
+  const int cols = 4 + 2 * n_levels;
+  int expect_off = 0;
+  for (int b = 0; b < B; ++b) {
+    const int32_t* r = images_host + b * cols;
+    const int img_h = r[0], img_w = r[1];
+    AtImage& im = p.img[b];
+    im.gt_off = r[2];
+    im.gt_cnt = r[3];
+    BAGS_REQUIRE(img_h >= 1 && img_w >= 1, "%s: image %d: img_shape %d x %d", who, b, img_h, img_w);
+    BAGS_REQUIRE(im.gt_cnt >= 1, "%s: image %d has no gt", who, b);
+    BAGS_REQUIRE(im.gt_off == expect_off && static_cast<long long>(im.gt_off) + im.gt_cnt <= total_gts,
+                 "%s: image %d: gts %d .. %d are not the next rows of the %d", who, b, im.gt_off,
+                 im.gt_off + im.gt_cnt, total_gts);
+    expect_off += im.gt_cnt;
+    for (int l = 0; l < n_levels; ++l) {
+      im.valid_h[l] = r[4 + 2 * l];
+      im.valid_w[l] = r[5 + 2 * l];
+      BAGS_REQUIRE(im.valid_h[l] >= 0 && im.valid_h[l] <= p.lvl[l].H && im.valid_w[l] >= 0 &&
+                       im.valid_w[l] <= p.lvl[l].W,
+                   "%s: image %d, level %d: valid %d x %d outside the %d x %d map", who, b, l, im.valid_h[l],
+                   im.valid_w[l], p.lvl[l].H, p.lvl[l].W);
+    }
+    // anchor_inside_flags compares fp32 anchors with the python numbers img_w + allowed_border, img_h + ...
+    im.x_hi = static_cast<float>(img_w + allowed_border);
+    im.y_hi = static_cast<float>(img_h + allowed_border);
+  }
+  BAGS_REQUIRE(expect_off == total_gts, "%s: the images hold %d of the %d gts", who, expect_off, total_gts);
+  p.gts = reinterpret_cast<const float4*>(gts);
+  p.border_on = allowed_border >= 0.0;
+  p.border_lo = static_cast<float>(-allowed_border);
+  p.pos_thr = pos_iou_thr;
+  p.neg_on = neg_on != 0;
+  p.neg_lo = neg_lo;
+  p.neg_hi = neg_hi;
+  p.min_pos = min_pos_iou;
+  p.assign_all = gt_max_assign_all != 0;
+  p.num = num;
+  p.exp_pos = static_cast<int>(num * pos_fraction);   // int(self.num * self.pos_fraction)
+  p.neg_pos_ub = neg_pos_ub;
+  p.pos_weight = pos_weight > 0.f ? pos_weight : 1.f;
+  for (int c = 0; c < 4; ++c) {
+    p.means[c] = means_host[c];
+    p.stds[c] = stds_host[c];
+  }
+  p.seed = seed;
+  p.seed_step = reinterpret_cast<const long long*>(seed_step);
+  anchor_target_layout(p, total_gts, scratch);
+  p.labels = reinterpret_cast<long long*>(labels);
+  p.label_weights = label_weights;
+  p.bbox_targets = reinterpret_cast<float4*>(bbox_targets);
+  p.bbox_weights = reinterpret_cast<float4*>(bbox_weights);
+  p.totals = reinterpret_cast<long long*>(totals);
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  BAGS_CUDA(launch_anchor_target(p, stream));
   return BAGS_OK;
 }
 

@@ -10,6 +10,7 @@
 //   merge_scores_kernel  test-time score merge (gs_bbox_head_with0.py:239-273)
 //   cast kernels         fp32 -> bf16 operand staging
 #pragma once
+#include "bags_hash.cuh"
 #include "bags_ptx.cuh"
 
 namespace bags {
@@ -245,17 +246,7 @@ group_ce_kernel(const float* __restrict__ z, long long ldz, const long long* __r
 // ----------------------------------------------------------------------------
 // "others" sampler  (device replacement of np.random.choice on the host)
 // ----------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t mix32(uint32_t x) {  // murmur3 finaliser
-  x ^= x >> 16; x *= 0x85ebca6bu; x ^= x >> 13; x *= 0xc2b2ae35u; x ^= x >> 16;
-  return x;
-}
-__device__ __forceinline__ uint32_t sample_key(unsigned long long seed, int g, int n) {
-  uint32_t h = mix32(static_cast<uint32_t>(seed) ^ 0x9e3779b9u);
-  h = mix32(h ^ static_cast<uint32_t>(seed >> 32));
-  h = mix32(h ^ (static_cast<uint32_t>(g) * 0x632be5abu + 0x7f4a7c15u));
-  h = mix32(h ^ static_cast<uint32_t>(n));
-  return h;
-}
+// sample_key (bags_hash.cuh): a counter-based 32-bit key of (seed, bin g, row n)
 
 // One CTA (1024 threads) per bin.  Bin 0: all ones.  Bin g>=1:
 //   F = #rows with in-bin label > 0 ; k = int(F * ratio) ; O = N - F

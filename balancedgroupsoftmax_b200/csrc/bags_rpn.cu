@@ -1,6 +1,7 @@
 // Kernels of the RPN proposal generation: see bags_rpn.cuh for what they compute.
 #include <cooperative_groups.h>
 
+#include "bags_anchor.cuh"
 #include "bags_iou.cuh"
 #include "bags_rpn.cuh"
 
@@ -236,9 +237,7 @@ bags_rpn_select_kernel(const __grid_constant__ RpnParams p) {
       const uint32_t f = 0xffffffffu - static_cast<uint32_t>(keys[i]);
       const int a = static_cast<int>(f % static_cast<uint32_t>(A)), hw = static_cast<int>(f / static_cast<uint32_t>(A));
       const int hy = hw / L.W, wx = hw - hy * L.W;
-      const float sx = static_cast<float>(wx * L.stride), sy = static_cast<float>(hy * L.stride);
-      const float4 ba = L.base[a];
-      const float4 an = make_float4(__fadd_rn(ba.x, sx), __fadd_rn(ba.y, sy), __fadd_rn(ba.z, sx), __fadd_rn(ba.w, sy));
+      const float4 an = grid_anchor(L.base[a], wx, hy, L.stride);
       const float* d = deltas + static_cast<size_t>(4 * a) * HW + hw;
       box[e] = decode(p, an, __ldg(d), __ldg(d + HW), __ldg(d + 2 * HW), __ldg(d + 3 * HW), max_w, max_h);
       score[e] = sigmoid_ref(__ldg(logits + static_cast<size_t>(a) * HW + hw));

@@ -770,6 +770,105 @@ def rpn_proposals(cls_scores, bbox_preds, base_anchors, strides, img_shapes, nms
     return out, counts
 
 
+# --------------------------------------------------------------------------- RPN training targets
+def valid_size(pad_shape, stride: int, featmap_size) -> Tuple[int, int]:
+    """AnchorHead.get_anchors' valid_flags size of one level: (min(ceil(pad_h / stride), feat_h), same for w)."""
+    return (min(int(np.ceil(pad_shape[0] / stride)), int(featmap_size[0])),
+            min(int(np.ceil(pad_shape[1] / stride)), int(featmap_size[1])))
+
+
+def _anchor_target_levels(featmap_sizes, base_anchors, strides):
+    L = len(featmap_sizes)
+    if not (L == len(base_anchors) == len(strides)) or not 1 <= L <= 8:
+        raise nat.BagsNativeError('anchor_targets: %d feature maps, %d base-anchor tables and %d strides (1 to 8 '
+                                  'levels, the same count of each)' % (L, len(base_anchors), len(strides)))
+    levels = np.zeros((L, 4), dtype=np.int32)
+    for l, ((h, w), base) in enumerate(zip(featmap_sizes, base_anchors)):
+        levels[l] = (int(h), int(w), int(np.shape(base)[0]), int(strides[l]))
+    base = np.ascontiguousarray(np.concatenate([np.asarray(torch.as_tensor(b, dtype=torch.float32).cpu(),
+                                                           dtype=np.float32).reshape(-1, 4) for b in base_anchors]))
+    return levels, base
+
+
+def anchor_target_scratch_bytes(levels: np.ndarray, B: int, total_gts: int) -> int:
+    """bags_anchor_target_scratch_bytes: device scratch bags_anchor_target needs; ``levels`` int32 [L, 4]
+    (H, W, A, stride)."""
+    levels = np.ascontiguousarray(levels, dtype=np.int32)
+    out = C.c_size_t(0)
+    nat.check(nat.lib().bags_anchor_target_scratch_bytes(levels.ctypes.data, levels.shape[0], int(B), int(total_gts),
+                                                         C.byref(out)), 'bags_anchor_target_scratch_bytes')
+    return out.value
+
+
+def anchor_targets(featmap_sizes, base_anchors, strides, img_shapes, pad_shapes, gt_bboxes, pos_iou_thr=0.7,
+                   neg_iou_thr=0.3, min_pos_iou=0.3, gt_max_assign_all=True, allowed_border=0, num=256,
+                   pos_fraction=0.5, neg_pos_ub=-1, pos_weight=-1, means=(0., 0., 0., 0.), stds=(1., 1., 1., 1.),
+                   seed: int = 0, seed_step: Optional[torch.Tensor] = None):
+    """bags_anchor_target: anchor_target of an RPN (MaxIoUAssigner + the base sampler, no gt labels, no ignored gts)
+    for every image in one call (a memset and four launches), with no host sync -- capturable in a CUDA graph.
+
+    ``featmap_sizes``: per level (H, W); ``base_anchors``: per level [A, 4] (AnchorGenerator.base_anchors);
+    ``strides``: per level; ``img_shapes`` / ``pad_shapes``: per image (h, w, ...); ``gt_bboxes``: per image a CUDA
+    [G_i, 4] tensor, G_i >= 1.  The assigner's and sampler's parameters as in their configs: ``neg_iou_thr`` a float
+    (negatives 0 <= max < thr) or a tuple (lo <= max < hi); any other type gives no negatives, as in the reference.
+    ``seed`` / ``seed_step`` pick the sample as in sample_others: the k positives and then the k negatives with the
+    smallest (sample_key(seed, image, n) << 32 | n), an exact-k uniform subset (statistically, not bitwise, the
+    reference's np.random.shuffle draw).
+
+    Returns ``(labels, label_weights, bbox_targets, bbox_weights, totals)``: int64 [B, N], fp32 [B, N], fp32
+    [B, N, 4], fp32 [B, N, 4] over the N anchors of an image (level after level, location-major), zero outside the
+    inside anchors, and int64 [3] device totals (num_total_pos, num_total_neg, num_total_samples)."""
+    gt_bboxes = list(gt_bboxes)
+    for t in gt_bboxes:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dim() != 2 or t.shape[1] != 4 or t.shape[0] < 1:
+            raise nat.BagsNativeError('anchor_targets: gt_bboxes must be CUDA [G, 4] tensors with G >= 1 (got %s)'
+                                      % (tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__,))
+    _require_cuda(seed_step)
+    levels, base = _anchor_target_levels(featmap_sizes, base_anchors, strides)
+    B, L = len(gt_bboxes), levels.shape[0]
+    if len(img_shapes) != B or len(pad_shapes) != B:
+        raise nat.BagsNativeError('anchor_targets: %d img_shapes and %d pad_shapes for %d images'
+                                  % (len(img_shapes), len(pad_shapes), B))
+    images = np.zeros((B, 4 + 2 * L), dtype=np.int32)
+    off = 0
+    for b in range(B):
+        g = int(gt_bboxes[b].shape[0])
+        images[b, :4] = (int(img_shapes[b][0]), int(img_shapes[b][1]), off, g)
+        off += g
+        for l in range(L):
+            images[b, 4 + 2 * l: 6 + 2 * l] = valid_size(pad_shapes[b], int(strides[l]), featmap_sizes[l])
+    if isinstance(neg_iou_thr, float):
+        neg = (1, 0.0, neg_iou_thr)
+    elif isinstance(neg_iou_thr, tuple):
+        assert len(neg_iou_thr) == 2
+        neg = (1, float(neg_iou_thr[0]), float(neg_iou_thr[1]))
+    else:   # the reference's assigner tests neither branch: no negatives
+        neg = (0, 0.0, 0.0)
+    if seed_step is not None:
+        assert seed_step.dtype == torch.int64 and seed_step.numel() == 1
+    dev = gt_bboxes[0].device
+    gts = torch.cat([t.detach().float() for t in gt_bboxes]).contiguous()
+    mean = np.asarray(means, dtype=np.float32).reshape(4)
+    std = np.asarray(stds, dtype=np.float32).reshape(4)
+    N = int(sum(int(h) * int(w) * int(a) for h, w, a, _ in levels))
+    nbytes = anchor_target_scratch_bytes(levels, B, off)
+    scratch = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=dev)
+    labels = torch.empty((B, N), dtype=torch.int64, device=dev)
+    label_weights = torch.empty((B, N), dtype=torch.float32, device=dev)
+    bbox_targets = torch.empty((B, N, 4), dtype=torch.float32, device=dev)
+    bbox_weights = torch.empty((B, N, 4), dtype=torch.float32, device=dev)
+    totals = torch.empty((3,), dtype=torch.int64, device=dev)
+    images = np.ascontiguousarray(images)
+    nat.check(nat.lib().bags_anchor_target(
+        levels.ctypes.data, base.ctypes.data, L, B, images.ctypes.data, gts.data_ptr(), off, float(pos_iou_thr),
+        neg[0], neg[1], neg[2], float(min_pos_iou), int(bool(gt_max_assign_all)), float(allowed_border), int(num),
+        float(pos_fraction), float(neg_pos_ub), float(pos_weight), mean.ctypes.data, std.ctypes.data,
+        int(seed) & 0xFFFFFFFFFFFFFFFF, nat.ptr(seed_step), scratch.data_ptr(), nbytes, labels.data_ptr(),
+        label_weights.data_ptr(), bbox_targets.data_ptr(), bbox_weights.data_ptr(), totals.data_ptr(),
+        _stream_ptr(dev)), 'bags_anchor_target')
+    return labels, label_weights, bbox_targets, bbox_weights, totals
+
+
 # --------------------------------------------------------------------------- FPN RoI feature extractor
 @dataclass(frozen=True)
 class RoIAlignSpec:

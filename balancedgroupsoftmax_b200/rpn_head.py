@@ -15,10 +15,22 @@ fails); a level with no candidate contributes nothing; an image with none gets a
 A softmax RPN (``use_sigmoid=False``), ``nms_across_levels=True``, a level with more candidates than the kernel
 holds (4096), more than 32 images or 16 anchors per location, or CPU tensors run mmdet's own ``get_bboxes_single``
 per image when mmdet is importable (also under the drop-in, where this RPNHead is the one registered in mmdet's
-HEADS), and raise NotImplementedError naming the setting otherwise.  ``loss`` restates AnchorHead.loss with this package's losses and takes ``anchor_target`` from
-mmdet; without mmdet it raises NotImplementedError.
+HEADS), and raise NotImplementedError naming the setting otherwise.
+
+``loss`` restates AnchorHead.loss with this package's losses.  Its targets are one ops.anchor_targets call for the
+batch (a memset and four launches, no host sync): MaxIoUAssigner's assignment bit for bit the reference's, the box
+targets bbox2delta's op sequence, and a sample drawn as the head's device sampler draws (an exact-k uniform subset by
+counter-based keys; statistically, not bitwise, np.random.shuffle's).  With the device totals as avg_factor and the
+sigmoid labels passed as [N, 1] columns (the one-hot CrossEntropyLoss would build, without its nonzero), the RPN
+loss makes no host sync.  An image with no gt raises ValueError('No gt or bboxes') and one with no inside anchor
+makes the loss None, both decided on the host from shapes and metadata.  A non-sampling RPN (Focal / GHM), another
+assigner or sampler, add_gt_as_proposals=True, ignore_iof_thr > 0 with ignored gts, more than 8 levels, 32 images or
+16 anchors per location, and CPU tensors take mmdet's ``anchor_target`` when mmdet is importable and raise
+NotImplementedError naming the setting otherwise.
 """
 from __future__ import annotations
+
+import os
 
 import numpy as np
 import torch
@@ -100,6 +112,15 @@ def _multi_apply(func, *args, **kwargs):
     import functools
     pfunc = functools.partial(func, **kwargs) if kwargs else func
     return tuple(map(list, zip(*map(pfunc, *args))))
+
+
+def _images_to_levels(target, num_level_anchors):
+    """anchor_target.py:images_to_levels on a batch tensor [B, N, ...]: per level [B, n_l, ...], squeezed at B = 1."""
+    out, start = [], 0
+    for n in num_level_anchors:
+        out.append(target[:, start:start + n].squeeze(0))
+        start += n
+    return out
 
 
 def _cfg(cfg, key, default=None):
@@ -208,8 +229,13 @@ class RPNHead(nn.Module):
     # ------------------------------------------------------------------ training loss
     def loss_single(self, cls_score, bbox_pred, labels, label_weights, bbox_targets, bbox_weights, num_total_samples,
                     cfg):
-        labels = labels.reshape(-1)
-        label_weights = label_weights.reshape(-1)
+        if self.use_sigmoid_cls and self.cls_out_channels == 1 and isinstance(self.loss_cls, CrossEntropyLoss):
+            # [N, 1] columns: the one-hot CrossEntropyLoss would build (labels are 0 / 1), without its nonzero sync
+            labels = labels.reshape(-1, 1)
+            label_weights = label_weights.reshape(-1, 1)
+        else:
+            labels = labels.reshape(-1)
+            label_weights = label_weights.reshape(-1)
         cls_score = cls_score.permute(0, 2, 3, 1).reshape(-1, self.cls_out_channels)
         loss_cls = self.loss_cls(cls_score, labels, label_weights, avg_factor=num_total_samples)
         bbox_targets = bbox_targets.reshape(-1, 4)
@@ -218,25 +244,119 @@ class RPNHead(nn.Module):
         loss_bbox = self.loss_bbox(bbox_pred, bbox_targets, bbox_weights, avg_factor=num_total_samples)
         return loss_cls, loss_bbox
 
-    @force_fp32(apply_to=('cls_scores', 'bbox_preds'))
-    def loss(self, cls_scores, bbox_preds, gt_bboxes, img_metas, cfg, gt_bboxes_ignore=None):
-        """RPNHead.loss / AnchorHead.loss (anchor_head.py:159-205) with mmdet's ``anchor_target``."""
+    def _next_seed(self) -> int:
+        """The sampler's seed of this call: torch's initial seed, the process's rank and a per-call counter (as
+        GSBBoxHeadWith0._next_seed)."""
+        self._sample_calls = getattr(self, '_sample_calls', 0) + 1
+        rank = int(os.environ.get('RANK', '0'))
+        return (torch.initial_seed() * 0x9E3779B97F4A7C15 + rank * 0xD1B54A32D192ED03 + self._sample_calls) \
+            & 0xFFFFFFFFFFFFFFFF
+
+    def _targets_unsupported(self, cfg, cls_scores, gt_bboxes, gt_bboxes_ignore, n_images):
+        """Why ops.anchor_targets cannot compute these targets, or None."""
+        if not self.sampling:
+            return 'sampling=False (a %s RPN)' % self.loss_cls.__class__.__name__
+        assigner, sampler = _cfg(cfg, 'assigner'), _cfg(cfg, 'sampler')
+        if _cfg(assigner, 'type') != 'MaxIoUAssigner':
+            return 'the assigner %r (MaxIoUAssigner only)' % (_cfg(assigner, 'type'),)
+        if _cfg(sampler, 'type') != 'RandomSampler':
+            return 'the sampler %r (RandomSampler only)' % (_cfg(sampler, 'type'),)
+        if _cfg(sampler, 'add_gt_as_proposals', True):
+            return 'add_gt_as_proposals=True'
+        if not 0 <= float(_cfg(sampler, 'pos_fraction')) <= 1:
+            return 'pos_fraction=%r (0 to 1)' % (_cfg(sampler, 'pos_fraction'),)
+        if _cfg(assigner, 'ignore_iof_thr', -1) > 0 and gt_bboxes_ignore is not None and \
+                any(g is not None and g.numel() > 0 for g in gt_bboxes_ignore):
+            return 'ignore_iof_thr > 0 with ignored gts'
+        if not 1 <= len(cls_scores) <= MAX_LEVELS:
+            return '%d levels (1 to %d)' % (len(cls_scores), MAX_LEVELS)
+        if n_images > MAX_IMAGES:
+            return '%d images per batch (at most %d)' % (n_images, MAX_IMAGES)
+        if self.num_anchors > MAX_ANCHORS:
+            return '%d anchors per location (at most %d)' % (self.num_anchors, MAX_ANCHORS)
+        if not all(t.is_cuda for t in list(cls_scores) + list(gt_bboxes)):
+            return 'CPU tensors (the native route runs on the GPU)'
+        return None
+
+    def _reference_anchor_target(self, why, featmap_sizes, gt_bboxes, img_metas, cfg, gt_bboxes_ignore, device):
         anchor_target = _mmdet_core('anchor_target')
         if anchor_target is None:
-            raise NotImplementedError('RPNHead.loss needs mmdet.core.anchor_target (mmdetection v1.x); native RPN '
-                                      'training targets are not implemented')
-        featmap_sizes = [featmap.size()[-2:] for featmap in cls_scores]   # pragma: no cover - needs mmdet
+            raise NotImplementedError('RPNHead.loss: %s has no native route; install mmdetection v1.x for the '
+                                      'reference anchor_target' % why)
         assert len(featmap_sizes) == len(self.anchor_generators)
-        device = cls_scores[0].device
         anchor_list, valid_flag_list = self.get_anchors(featmap_sizes, img_metas, device=device)
         label_channels = self.cls_out_channels if self.use_sigmoid_cls else 1
-        targets = anchor_target(anchor_list, valid_flag_list, gt_bboxes, img_metas, self.target_means,
-                                self.target_stds, cfg, gt_bboxes_ignore_list=gt_bboxes_ignore, gt_labels_list=None,
-                                label_channels=label_channels, sampling=self.sampling)
-        if targets is None:
+        return anchor_target(anchor_list, valid_flag_list, gt_bboxes, img_metas, self.target_means, self.target_stds,
+                             cfg, gt_bboxes_ignore_list=gt_bboxes_ignore, gt_labels_list=None,
+                             label_channels=label_channels, sampling=self.sampling)
+
+    def _has_inside_anchor(self, featmap_sizes, img_meta, allowed_border):
+        """Whether anchor_inside_flags keeps any anchor of this image: host arithmetic on its metadata, the same fp32
+        adds and comparisons (anchors depend on shapes only)."""
+        h, w = img_meta['img_shape'][:2]
+        for l, size in enumerate(featmap_sizes):
+            vh, vw = ops.valid_size(img_meta['pad_shape'], self.anchor_strides[l], size)
+            if vh == 0 or vw == 0:
+                continue
+            if allowed_border < 0:
+                return True
+            base = self.anchor_generators[l].base_anchors.numpy().astype(np.float32)
+            sx = (np.arange(vw) * self.anchor_strides[l]).astype(np.float32)
+            sy = (np.arange(vh) * self.anchor_strides[l]).astype(np.float32)
+            lo = np.float32(-allowed_border)
+            for a in range(base.shape[0]):
+                ok_x = ((base[a, 0] + sx >= lo) & (base[a, 2] + sx < np.float32(w + allowed_border))).any()
+                ok_y = ((base[a, 1] + sy >= lo) & (base[a, 3] + sy < np.float32(h + allowed_border))).any()
+                if ok_x and ok_y:
+                    return True
+        return False
+
+    def anchor_targets(self, featmap_sizes, gt_bboxes, img_metas, cfg, seed=None, seed_step=None):
+        """anchor_target on this head's anchors through ops.anchor_targets: (labels, label_weights, bbox_targets,
+        bbox_weights, totals) as dense [B, N] / [B, N, 4] device tensors and int64 [3] device totals, with no host
+        sync; None when an image has no inside anchor, and ValueError('No gt or bboxes') when one that has some has
+        no gt (both decided from shapes and metadata, as the reference decides them)."""
+        assigner, sampler = _cfg(cfg, 'assigner'), _cfg(cfg, 'sampler')
+        allowed_border = _cfg(cfg, 'allowed_border', 0)
+        inside = [self._has_inside_anchor(featmap_sizes, m, allowed_border) for m in img_metas]
+        if any(ok and g.shape[0] == 0 for ok, g in zip(inside, gt_bboxes)):
+            raise ValueError('No gt or bboxes')
+        if not all(inside):
             return None
-        labels, label_weights, bbox_targets, bbox_weights, num_pos, num_neg = targets
-        num_total_samples = num_pos + num_neg if self.sampling else num_pos
+        L = len(featmap_sizes)
+        return ops.anchor_targets(
+            [tuple(int(v) for v in s) for s in featmap_sizes],
+            [self.anchor_generators[i].base_anchors for i in range(L)], self.anchor_strides[:L],
+            [m['img_shape'] for m in img_metas], [m['pad_shape'] for m in img_metas], gt_bboxes,
+            pos_iou_thr=_cfg(assigner, 'pos_iou_thr'), neg_iou_thr=_cfg(assigner, 'neg_iou_thr'),
+            min_pos_iou=_cfg(assigner, 'min_pos_iou', .0), gt_max_assign_all=_cfg(assigner, 'gt_max_assign_all', True),
+            allowed_border=allowed_border, num=_cfg(sampler, 'num'), pos_fraction=_cfg(sampler, 'pos_fraction'),
+            neg_pos_ub=_cfg(sampler, 'neg_pos_ub', -1), pos_weight=_cfg(cfg, 'pos_weight', -1),
+            means=self.target_means, stds=self.target_stds,
+            seed=self._next_seed() if seed is None else seed, seed_step=seed_step)
+
+    @force_fp32(apply_to=('cls_scores', 'bbox_preds'))
+    def loss(self, cls_scores, bbox_preds, gt_bboxes, img_metas, cfg, gt_bboxes_ignore=None):
+        """RPNHead.loss / AnchorHead.loss (anchor_head.py:159-205).  The targets are one ops.anchor_targets call for
+        the batch, split per level as images_to_levels splits them; with its device totals as avg_factor the loss
+        makes no host sync.  Settings without a native route take mmdet's ``anchor_target``."""
+        featmap_sizes = [featmap.size()[-2:] for featmap in cls_scores]
+        why = self._targets_unsupported(cfg, cls_scores, gt_bboxes, gt_bboxes_ignore, len(img_metas))
+        if why is not None:
+            targets = self._reference_anchor_target(why, featmap_sizes, gt_bboxes, img_metas, cfg, gt_bboxes_ignore,
+                                                    cls_scores[0].device)
+            if targets is None:
+                return None
+            labels, label_weights, bbox_targets, bbox_weights, num_pos, num_neg = targets
+            num_total_samples = num_pos + num_neg if self.sampling else num_pos
+        else:
+            assert len(featmap_sizes) == len(self.anchor_generators)
+            targets = self.anchor_targets(featmap_sizes, gt_bboxes, img_metas, cfg)
+            if targets is None:
+                return None
+            counts = [int(h) * int(w) * self.num_anchors for h, w in featmap_sizes]
+            labels, label_weights, bbox_targets, bbox_weights = [_images_to_levels(t, counts) for t in targets[:4]]
+            num_total_samples = targets[4][2]
         losses_cls, losses_bbox = _multi_apply(self.loss_single, cls_scores, bbox_preds, labels, label_weights,
                                                bbox_targets, bbox_weights, num_total_samples=num_total_samples,
                                                cfg=cfg)

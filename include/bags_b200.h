@@ -40,6 +40,8 @@
  *     single_level.py, roi_align_kernel.cu
  *   RPNHead.get_bboxes: RPN proposals                     bags_rpn_proposals (+ bags_rpn_scratch_bytes)
  *     rpn_head.py:55-104, anchor_head.py:250-276, nms_kernel.cu
+ *   RPNHead.loss: RPN training targets                    bags_anchor_target (+ bags_anchor_target_scratch_bytes)
+ *     anchor_target.py, max_iou_assigner.py, base_sampler.py / random_sampler.py
  *   allreduce_grads / _allreduce_coalesced                bags_grad_allreduce
  *     mmdet/core/utils/dist_utils.py:9-41
  *
@@ -437,6 +439,46 @@ int bags_rpn_proposals(const float* const* logits_host, const float* const* delt
 /* Scratch bytes bags_rpn_proposals needs for these level shapes (levels_host as there), B, nms_pre and nms_post; the
  * same argument checks.  Writes *bytes. */
 int bags_rpn_scratch_bytes(const int32_t* levels_host, int n_levels, int B, int nms_pre, int nms_post, size_t* bytes);
+
+/* RPN training targets -- replaces anchor_target (mmdet/core/anchor/anchor_target.py: per image anchor_inside_flags,
+ * MaxIoUAssigner.assign of core/bbox/assigners/max_iou_assigner.py, the sampler of core/bbox/samplers/
+ * base_sampler.py, bbox2delta and unmap) for an RPN without gt labels or ignored gts.  Every image in one memset and
+ * four launches, no host read, no allocation:
+ *   anchors  per image, level after level, location-major ((h W + w) A + a): base[a] + (w stride, h stride) in fp32;
+ *            inside when h < valid_h and w < valid_w of the level and, when allowed_border >= 0, x1 >= -border,
+ *            y1 >= -border, x2 < img_w + border and y2 < img_h + border (fp32 comparisons);
+ *   assign   IoU = bbox_overlaps(gt, anchor) with one fp32 rounding per torch op (NaN propagates); per anchor the max
+ *            over gts (first gt on ties, NaN wins), per gt the max over the inside anchors; ignored (-1) by default,
+ *            negative when neg_on and neg_lo <= max < neg_hi, positive (argmax) when max >= pos_iou_thr, then for
+ *            each gt in order with max >= min_pos_iou, every inside anchor at that max (or the first only, when
+ *            gt_max_assign_all = 0) is given to it: the last gt wins;
+ *   sample   key(n) = (sample_key(seed', image, n) << 32) | n with seed' = seed + *seed_step * 0x9E3779B97F4A7C15
+ *            when seed_step is given; the k_pos = min(#pos, int(num pos_fraction)) positives and then the
+ *            k_neg = min(#neg, num - k_pos, int(neg_pos_ub max(k_pos, 1)) when neg_pos_ub >= 0) negatives with the
+ *            smallest keys: an exact-k uniform subset, not np.random.shuffle's;
+ *   targets  labels int64 [B, N] 1 at sampled positives; label_weights fp32 [B, N] pos_weight (1 when <= 0) at
+ *            sampled positives and 1 at sampled negatives; bbox_targets fp32 [B, N, 4] bbox2delta(anchor, gt) in
+ *            torch's op sequence, then (d - means) / stds, and bbox_weights 1 at sampled positives; 0 elsewhere;
+ *            totals int64 [3]: sum_b max(k_pos, 1), sum_b max(k_neg, 1) and their sum.
+ *   levels_host  int32 [L, 4]: H_l, W_l (>= 0), A_l (1 to 16), stride_l (>= 1); L in [1, 8]; N = sum H W A >= 1
+ *   base_host    fp32 [sum A_l, 4]: each level's base anchors, level after level
+ *   images_host  int32 [B, 4 + 2 L]: img_h, img_w (>= 1), gt_off, gt_cnt (>= 1; the images' gts consecutive rows of
+ *                gts), then valid_h, valid_w of every level (in [0, H] x [0, W]);  B in [1, 32]
+ *   gts          device fp32 [total_gts, 4], 16-byte aligned;  num >= 0, pos_fraction in [0, 1]
+ *   means_host, stds_host fp32 [4];  seed_step: optional device int64;  scratch: device,
+ *   bags_anchor_target_scratch_bytes() bytes, 256-byte aligned;  bbox_targets / bbox_weights 16-byte aligned
+ * No host sync: capturable in a CUDA graph. */
+int bags_anchor_target(const int32_t* levels_host, const float* base_host, int n_levels, int B,
+                       const int32_t* images_host, const float* gts, int total_gts, float pos_iou_thr, int neg_on,
+                       float neg_lo, float neg_hi, float min_pos_iou, int gt_max_assign_all, double allowed_border,
+                       int num, double pos_fraction, double neg_pos_ub, float pos_weight, const float* means_host,
+                       const float* stds_host, uint64_t seed, const int64_t* seed_step, void* scratch,
+                       size_t scratch_bytes, int64_t* labels, float* label_weights, float* bbox_targets,
+                       float* bbox_weights, int64_t* totals, void* stream);
+
+/* Scratch bytes bags_anchor_target needs for these level shapes (levels_host as there), B and total_gts; the same
+ * argument checks.  Writes *bytes. */
+int bags_anchor_target_scratch_bytes(const int32_t* levels_host, int n_levels, int B, int total_gts, size_t* bytes);
 
 /* test hook: launch `blocks` x `threads` threads that wait `micros` microseconds and exit */
 int bags_debug_spin(int blocks, int threads, int micros, void* stream);
